@@ -5,7 +5,9 @@
 // it is recomputed from (x, eps[, eps_u]) with the same device function the update kernel uses, and
 // the two adjacent order statistics are found by selection on the fp32 bit pattern of |x0|
 // (monotone as uint32 for non-negative floats). They are combined with torch's CPU lerp
-// (fma(w<0.5 ? w : w-1, hi-lo, w<0.5 ? lo : hi)) and floored with max_val (:423).
+// (fma(w<0.5 ? w : w-1, hi-lo, w<0.5 ? lo : hi)) and floored with max_val (:423). Non-finite order statistics
+// follow torch: an infinite one can make the lerp inf - inf = NaN, a NaN anywhere in the sample makes the result
+// NaN, and the floor keeps a NaN (torch.maximum), so the whole sample then becomes NaN.
 //
 // Two implementations behind dpm_dynamic_threshold():
 //
@@ -129,8 +131,10 @@ __device__ __forceinline__ float finish_value(uint32_t key_lo, uint32_t key_hi, 
   const float a = __uint_as_float(key_lo), b = __uint_as_float(key_hi);
   const float d = b - a;
   // at::native::lerp, CPU vectorised path: fmadd(coeff, end - start, base)
+  // an infinite order statistic gives inf - inf = NaN (both infinite, or lo finite with w >= 0.5) exactly as in
+  // torch, and torch.maximum keeps it
   float s = qp.w < 0.5f ? fmaf(qp.w, d, a) : fmaf(qp.w - 1.f, d, b);
-  return fmaxf(s, qp.max_val);  // torch.maximum(s, max_val) :423
+  return max_nan(s, qp.max_val);  // torch.maximum(s, max_val) :423
 }
 
 // =================================== A. streaming pipeline ======================================
@@ -604,11 +608,7 @@ __global__ void __launch_bounds__(kQThreads)
     key_hi = *min0;
   }
   if (crank == 0 && tid == 0) {
-    const float a = __uint_as_float(key_lo), b = __uint_as_float(key_hi);
-    const float d = b - a;
-    // at::native::lerp, CPU vectorised path: fmadd(coeff, end - start, base)
-    float s = qp.w < 0.5f ? fmaf(qp.w, d, a) : fmaf(qp.w - 1.f, d, b);
-    s = fmaxf(s, qp.max_val);  // torch.maximum(s, max_val) :423
+    float s = finish_value(key_lo, key_hi, qp);
     if (*max0 > kInfKey) s = __uint_as_float(0x7fc00000u);   // NaN in the sample: torch.quantile returns NaN
     qp.s_out[sample] = s;
   }
@@ -671,7 +671,12 @@ int launch_quantile(float* s_out, const KParams& p, uint64_t n_samples, float q,
   else if (md == DPM_F16 && sd == DPM_F32) DPM_PICK(__half, float)
   else if (md == DPM_F32 && sd == DPM_BF16) DPM_PICK(float, __nv_bfloat16)   // fp32 network output, 16-bit state
   else if (md == DPM_F32 && sd == DPM_F16) DPM_PICK(float, __half)
-  else { set_error("dynamic threshold: unsupported dtype mix (model %d, state %d)", md, sd); return DPM_ERR_UNSUPPORTED; }
+  else if ((md == DPM_BF16 && sd == DPM_F16) || (md == DPM_F16 && sd == DPM_BF16)) {
+    // two different 16-bit types have no packet instantiation: the VEC = false kernels read every operand
+    // through load_any with the runtime dtypes (the template types are unused there)
+    vec = false;
+    DPM_PICK(float, float)
+  } else { set_error("dynamic threshold: unsupported dtype mix (model %d, state %d)", md, sd); return DPM_ERR_UNSUPPORTED; }
 #undef DPM_PICK
 
   // torch.quantile rank arithmetic, in fp32: pos = fl(q * (n-1))

@@ -3,7 +3,8 @@
     python oracle/build_ref.py [--reference DIR]
 
 The reference is Python: "building" it means `py_compile` of the handful of files on the hot path,
-straight from the sources of a reference checkout ($DPM_REFERENCE, default ../reference next to this repository)
+straight from the sources of a reference checkout ($DPM_REFERENCE, default a `reference` directory next to this
+repository or next to one of its parent directories)
 into oracle/_ref/*.pyc (git-ignored; the bytecode may be copied to a GPU machine like our own .so, the sources never
 enter the repo). A machine with the same CPython (same magic number) imports the .pyc files unchanged -- that is
 how `-m gpu` tests, smoke() and `bench.py --impl reference` execute the real reference on the box
@@ -19,7 +20,26 @@ import py_compile
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-DEFAULT_REFERENCE = os.environ.get("DPM_REFERENCE", os.path.join(os.path.dirname(os.path.dirname(HERE)), "reference"))
+
+
+def _find_reference():
+    """$DPM_REFERENCE, else a `reference` checkout next to this repository or next to any directory above it (a
+    clean checkout may sit a few levels below the directory that holds the reference)."""
+    if os.environ.get("DPM_REFERENCE"):
+        return os.environ["DPM_REFERENCE"]
+    repo = os.path.dirname(HERE)
+    d = os.path.dirname(repo)
+    while True:
+        cand = os.path.join(d, "reference")
+        if os.path.isfile(os.path.join(cand, "dpm_solver_pytorch.py")):
+            return cand
+        up = os.path.dirname(d)
+        if up == d:
+            return os.path.join(os.path.dirname(repo), "reference")
+        d = up
+
+
+DEFAULT_REFERENCE = _find_reference()
 OUT = os.path.join(HERE, "_ref")
 
 # logical name -> path under the reference tree

@@ -289,15 +289,25 @@ def cfg_combine(eps_uncond, eps_cond, scale):      # model_fn :330
 
 
 def _fma32(a, b, c):
-    """Correctly rounded fp32 fma(a, b, c) via exact rationals."""
+    """Correctly rounded fp32 fma(a, b, c): exact rationals for finite operands, IEEE semantics otherwise.
+
+    With an infinite or NaN operand the result is inf or NaN, and float64 arithmetic gives the IEEE one: the
+    product of two fp32 values is exact there, inf * 0 and inf - inf are NaN. A finite result beyond the fp32
+    range rounds to inf, which takes part in round-to-nearest-even as 2^128 with an even significand."""
+    a, b, c = np.float32(a), np.float32(b), np.float32(c)
+    if not (np.isfinite(a) and np.isfinite(b) and np.isfinite(c)):
+        with np.errstate(invalid="ignore", over="ignore"):
+            return np.float32(np.float64(a) * np.float64(b) + np.float64(c))
     r = Fraction(float(a)) * Fraction(float(b)) + Fraction(float(c))
-    f = np.float32(float(r))
-    cands = {float(f), float(np.nextafter(f, np.float32(np.inf))), float(np.nextafter(f, np.float32(-np.inf)))}
+    with np.errstate(over="ignore"):
+        f = np.float32(float(r))
+        cands = {float(f), float(np.nextafter(f, np.float32(np.inf))), float(np.nextafter(f, np.float32(-np.inf)))}
     best = None
     for cnd in cands:
-        if not math.isfinite(cnd):
+        if math.isnan(cnd):
             continue
-        d = abs(Fraction(cnd) - r)
+        v = Fraction(cnd) if math.isfinite(cnd) else Fraction(2 ** 128) * (1 if cnd > 0 else -1)
+        d = abs(v - r)
         even = (np.float32(cnd).view(np.uint32) & 1) == 0
         key = (d, 0 if even else 1)
         if best is None or key < best[0]:
@@ -307,7 +317,8 @@ def _fma32(a, b, c):
 
 def quantile_abs(x0, q):
     """torch.quantile(|x0|.reshape(B,-1), q, dim=1) (:422): sort, fp32 rank q*(n-1), lerp between the
-    two adjacent order statistics with ATen's CPU lerp: fma(w<0.5 ? w : w-1, hi-lo, w<0.5 ? lo : hi)."""
+    two adjacent order statistics with ATen's CPU lerp: fma(w<0.5 ? w : w-1, hi-lo, w<0.5 ? lo : hi).
+    Non-finite order statistics follow torch: inf - inf in the lerp gives NaN, a NaN in the row gives NaN."""
     a = np.abs(np.asarray(x0, dtype=np.float32)).reshape(x0.shape[0], -1)
     n = a.shape[1]
     srt = np.sort(a, axis=1)
@@ -321,7 +332,8 @@ def quantile_abs(x0, q):
             out[b] = np.float32(np.nan)
             continue
         vl, vh = srt[b, lo], srt[b, min(hi, n - 1)]
-        d = np.float32(vh - vl)
+        with np.errstate(invalid="ignore"):
+            d = np.float32(vh - vl)
         out[b] = _fma32(w, d, vl) if w < np.float32(0.5) else _fma32(np.float32(w - np.float32(1)), d, vh)
     return out
 

@@ -4,8 +4,8 @@ package never imports it.
 
     ref = ref_loader.load("dpm_solver_pytorch")      # module with NoiseScheduleVP, model_wrapper, DPM_Solver
 
-Falls back to the sources of the reference checkout (oracle/build_ref.py: $DPM_REFERENCE, default ../reference next
-to this repository) when the bytecode has not been built yet. `available()` is the skip condition for tests.
+Falls back to the sources of the reference checkout (oracle/build_ref.py: $DPM_REFERENCE, default a `reference`
+directory next to this repository or above it) when the bytecode has not been built yet. `available()` is the skip condition for tests.
 """
 import importlib.machinery
 import importlib.util

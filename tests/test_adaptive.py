@@ -71,6 +71,74 @@ def test_error_norm_kernel(cuda_backend, shape, dt):
     assert abs(got - ref) <= 2e-6 * ref
 
 
+# Relative error of the kernel's E against float64 on the same (widened) inputs, from its accumulation order
+# (csrc/adaptive.cu). Each term v^2, v = (h - l) / max(atol, rtol*max(|l|, |p|)), carries 4 fp32 roundings (rtol*m,
+# h - l, the division, the square): 7 units of u = 2^-24 in v^2. The sum of non-negative terms then gains at most one
+# u per addition on its path: a per-thread fp32 sum of <= 32 terms (31), a 5-level warp shuffle tree (5) and a
+# sequential sum of 8 warp partials (7); the fp64 sum across chunks adds nothing at this scale. The mean is rounded
+# to fp32 (1) and sqrtf rounds once more (1 in E); sqrt halves the relative error of the sum. The batch maximum
+# keeps the bound. 10 % on top covers the second-order terms.
+_U = 2.0 ** -24
+ERR_NORM_RTOL = 1.1 * ((7 + 31 + 5 + 7 + 1) / 2 + 1) * _U        # 1.7e-6
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("seed", range(4))
+def test_error_norm_kernel_fuzz(cuda_backend, seed):
+    """dpm_adaptive_error against float64 on random batches: f32 / bf16 / f16, B from 1 to 1000 (beyond the 256
+    threads of k_err_final), per_sample around the 8192-element chunk and the 8-element packet, misaligned views (the
+    scalar path), both tolerance settings, and the regimes E = 0, NaN, inf and 0/0. Non-finite results must match
+    exactly, finite ones within ERR_NORM_RTOL; two calls on one input give the same bits."""
+    import random
+    rng = random.Random(700 + seed)
+    for case in range(12):
+        dt = rng.choice([torch.float32, torch.bfloat16, torch.float16])
+        B = rng.choice([1, rng.randint(2, 16), rng.randint(257, 1000)])
+        ps = rng.choice([1, 7, 8, rng.randint(8191, 8193), 8 * rng.randint(2, 1 << 17)])
+        if rng.random() < 0.1:
+            ps = 1 << 20
+        B = min(B, max(1, (1 << 22) // ps))                       # at most 4 M elements per case
+        off = rng.choice([0, 0, 1, 3])                             # element offset: 1, 3 take the scalar path
+        atol, rtol = rng.choice([(0.0078, 0.05), (0.0, 0.05)])
+        regime = rng.choice(["random", "random", "equal", "nan", "inf", "zeros"])
+        n = B * ps
+        g = torch.Generator().manual_seed(rng.randint(0, 1 << 30))
+        xh = torch.randn(n + off, generator=g) * rng.choice([0.1, 1.0, 30.0])
+        xl = xh + 0.01 * torch.randn(n + off, generator=g)
+        xp = torch.randn(n + off, generator=g)
+        b = rng.randrange(B)
+        at = off + b * ps + rng.randrange(ps)
+        if regime == "equal":
+            xl = xh.clone()
+        elif regime == "nan":
+            rng.choice([xh, xl, xp])[at] = float("nan")
+        elif regime == "inf":
+            xh[at] = float("inf")
+        elif regime == "zeros":
+            atol = 0.0
+            for t in (xh, xl, xp):
+                t[off + b * ps: off + (b + 1) * ps] = 0.0
+        xh, xl, xp = (t.to(dt) for t in (xh, xl, xp))
+        dev = [t.cuda()[off:].view(B, ps) for t in (xh, xl, xp)]
+        got = cuda_backend.error_norm(*dev, atol, rtol)
+        again = cuda_backend.error_norm(*dev, atol, rtol)
+        got, again = got.cpu().numpy(), again.cpu().numpy()
+        assert got.tobytes() == again.tobytes(), "error norm is not deterministic"
+        h, l, p = (t[off:].double().numpy().reshape(B, ps) for t in (xh, xl, xp))
+        with np.errstate(all="ignore"):
+            delta = np.maximum(np.float64(np.float32(atol)), np.float64(np.float32(rtol)) * np.maximum(np.abs(l), np.abs(p)))
+            ref = np.sqrt(np.mean(np.square((h - l) / delta), axis=-1))
+        ref = np.float64(np.nan) if np.isnan(ref).any() else ref.max()   # torch .max(): NaN wins
+        e = float(got[0])
+        desc = dict(seed=seed, case=case, dt=dt, B=B, ps=ps, off=off, atol=atol, rtol=rtol, regime=regime, got=e, ref=ref)
+        if not np.isfinite(ref):
+            assert (np.isnan(e) and np.isnan(ref)) or e == ref, desc
+            continue
+        assert abs(e - ref) <= ERR_NORM_RTOL * ref, desc
+        if regime == "equal":
+            assert e == 0.0, desc
+
+
 # ---- the controller on the device (csrc/adaptive_ctl.cu) ------------------------------------------------------------
 def _adaptive_cfgs(n, seed):
     import random

@@ -140,6 +140,35 @@ def test_dynamic_thresholding_propagates_nan(dev, shape):
     np.testing.assert_array_equal(have.numpy(), want.numpy())      # NaNs compare equal positionally
 
 
+@pytest.mark.parametrize("ratio", [0.995, 0.997, 1.0])
+@pytest.mark.parametrize("shape", [(3, 3, 16, 16), (3, 3, 64, 64)])     # cluster kernel / streaming pipeline
+def test_dynamic_thresholding_infinite_order_statistics(dev, shape, ratio):
+    """+-inf in x0 reaches the quantile's order statistics. With pos = fl(ratio*(n-1)), lo = floor(pos), w = pos - lo
+    and k infinities in a sample of n: k = n - lo puts both order statistics at inf (inf - inf in the lerp: NaN),
+    k = n - lo - 1 puts only the upper one there (fma(w, inf, lo) = inf for w < 0.5, fma(w-1, inf, inf) = NaN for
+    w >= 0.5), k = n - lo - 2 leaves both finite. ratio 0.995 gives w = 0.165 (n = 768) and 0.565 (n = 12288), 0.997
+    gives 0.70 and 0.14, 1.0 gives w = 0 with lo = n - 1, where a single inf is already inf - inf. The quantile
+    becomes NaN or inf, torch.maximum keeps a NaN, and clamp / division spread it over the sample (:422-424)."""
+    import dpm_solver_b200 as new
+    ref = ref_loader.load("dpm_solver_pytorch")
+    B, n = shape[0], int(np.prod(shape[1:]))
+    pos = np.float32(ratio) * np.float32(n - 1)
+    lo = int(np.floor(pos))
+    x0 = (seeded(shape, 9) * 2.0).reshape(B, n)
+    rs = np.random.RandomState(n)
+    for b, k in enumerate((n - lo - 2, n - lo, n - lo - 1)):
+        k = max(k, 1)
+        idx = torch.from_numpy(rs.permutation(n)[:k])
+        x0[b, idx] = torch.from_numpy(np.where(rs.rand(k) < 0.5, np.inf, -np.inf).astype(np.float32))
+    x0 = x0.reshape(shape)
+    want = ref.DPM_Solver(None, _sched(ref), dynamic_thresholding_ratio=ratio).dynamic_thresholding_fn(x0, None)
+    have = new.DPM_Solver(None, _sched(new), dynamic_thresholding_ratio=ratio).dynamic_thresholding_fn(x0.to(dev), None).cpu()
+    assert torch.isnan(want[1]).all()                              # both order statistics infinite
+    if ratio < 1.0:
+        assert torch.isfinite(want[0]).all()
+    np.testing.assert_array_equal(have.numpy(), want.numpy())      # NaNs compare equal positionally
+
+
 def test_adaptive_raises_on_nan_error_estimate(dev):
     """The reference would spin forever on a NaN error estimate (:1002-1008); the product raises."""
     import dpm_solver_b200 as new

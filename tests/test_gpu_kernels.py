@@ -205,6 +205,52 @@ def test_dynamic_threshold_ties_and_constants(cuda_backend):
             np.testing.assert_array_equal(got, O.quantile_abs(x.numpy(), q))
 
 
+def _plain_x0(x):
+    """StepArgs whose x0 is x itself: noise network, eps = 0, alpha 1, sigma 0."""
+    B, ps = x.shape
+    return StepArgs(form=FORM_NONE, n_model=1, e_cond=torch.zeros(B * ps), xe=x.reshape(-1).contiguous(), predict_x0=True,
+                    alpha_e=1.0, sigma_e=0.0, per_sample=ps, state_dtype=torch.float32)
+
+
+def test_dynamic_threshold_pivot_defeating_sample(cuda_backend):
+    """k_q_pivots reads 256 groups of 4 consecutive elements at a stride of per_sample/256 = 64: a sample whose
+    elements 64k..64k+3 are small and all others large hides the target rank from the pivots. The exact counts then
+    refuse the bracket and the finish kernel selects over the whole sample (path 2); the result is still exact."""
+    from oracle import dpm_oracle as O
+    ps, B = 16384, 3
+    g = torch.Generator().manual_seed(8)
+    x = 10.0 + torch.rand(B, ps, generator=g) * 5.0
+    probe = (torch.arange(ps) % 64) < 4
+    x[:, probe] = torch.rand(B, int(probe.sum()), generator=g)
+    for q in (0.995, 0.5):
+        got, hdr = cuda_backend.dynamic_threshold(to_dev(_plain_x0(x)), q, 0.0, return_stats=True)
+        assert (hdr[:, 4] == 2).all(), hdr[:, 4]
+        np.testing.assert_array_equal(got.cpu().numpy(), O.quantile_abs(x.numpy(), q))
+
+
+def test_dynamic_threshold_count_cta_overflow(cuda_backend):
+    """One count CTA (16384 elements at the default shape) meets more bracket keys than its block-local list holds
+    (kLocalCand = 2048) while the sample's bracket count stays within the candidate capacity (16384/16 + 2048 = 3072):
+    2500 ties span the 0.995 rank. The CTA poisons the count (bit 30 of header word 3), which forces the exact fallback
+    (path 2) rather than a select over an incomplete candidate list."""
+    from oracle import dpm_oracle as O
+    ps, B, ties, below = 16384, 2, 2500, 13850
+    g = torch.Generator().manual_seed(9)
+    x = torch.empty(B, ps)
+    for b in range(B):
+        v = torch.cat([torch.rand(below, generator=g), torch.full((ties,), 5.0),
+                       6.0 + torch.rand(ps - below - ties, generator=g)])
+        x[b] = v[torch.randperm(ps, generator=g)] * torch.where(torch.rand(ps, generator=g) < 0.5, -1.0, 1.0)
+    lo = int(np.floor(np.float32(0.995) * np.float32(ps - 1)))
+    assert below <= lo and lo + 1 < below + ties                   # both order statistics are tied keys
+    got, hdr = cuda_backend.dynamic_threshold(to_dev(_plain_x0(x)), 0.995, 0.0, return_stats=True)
+    words = hdr[:, 3].cpu().numpy().view(np.uint32)
+    assert ((words & (1 << 30)) != 0).all(), words
+    assert ((words & ((1 << 30) - 1)) <= 3072).all(), words      # within capacity: only the poison forces the fallback
+    assert (hdr[:, 4] == 2).all(), hdr[:, 4]
+    np.testing.assert_array_equal(got.cpu().numpy(), O.quantile_abs(x.numpy(), 0.995))
+
+
 def test_quantile_golden(golden, cuda_backend):
     """Directly against torch.quantile outputs recorded from the reference's code path."""
     g = golden["glue"]

@@ -133,3 +133,59 @@ def test_sample_loops_torch_namespace_bit_exact(golden, name):
     y, _, calls = run_oracle_case(CASES[name], xp=TH)
     np.testing.assert_array_equal(y.numpy(), g[f"{name}/y"])
     np.testing.assert_array_equal(np.asarray([c[0] for c in calls], dtype=np.float32), g[f"{name}/calls_t"])
+
+
+def _quantile_rows(rs):
+    """|x0| rows whose order statistics are non-finite, tied or degenerate, each row as long as the others."""
+    n = 11
+    rows = []
+    for k in range(1, n + 1):                                   # k of the n values +inf, the rest 1
+        rows.append(np.r_[np.ones(n - k), np.full(k, np.inf)])
+    rows.append(np.r_[rs.randn(n - 2), np.inf, -np.inf])        # |.| turns -inf into +inf
+    rows.append(np.r_[rs.randn(n - 1), np.nan])
+    rows.append(np.r_[np.nan, np.full(n - 1, np.inf)])
+    rows.append(np.full(n, np.nan))
+    rows.append(np.round(rs.randn(n) * 2) / 4)                  # heavy ties
+    rows.append(np.full(n, 0.75))                               # constant
+    rows.append(np.zeros(n))
+    rows.append(np.r_[np.zeros(n - 1), np.inf])
+    rows.append(np.r_[np.full(n - 1, 3.0e38), -3.4028235e38])   # finite extremes: hi - lo stays finite
+    rows += [rs.randn(n) * s for s in (1e-30, 1.0, 1e30)]
+    return np.asarray(rows, dtype=np.float32)
+
+
+def test_quantile_abs_matches_torch_on_non_finite_rows():
+    """quantile_abs == torch.quantile(|x|, q, dim=1) bit for bit (NaN equal to NaN) where order statistics are
+    infinite: for nine 1s and two +inf (n = 11) q = 0.93 lerps between two infs, 0.90 lands on an inf with w = 0,
+    0.87 and 0.83 lerp from 1 to inf with w >= 0.5 (inf - inf: NaN) and w < 0.5 (inf). Plus NaN rows, ties,
+    constants, zeros and q in {0, 1}. Every q is used with every row, so each +inf count meets each case."""
+    rs = np.random.RandomState(17)
+    x = _quantile_rows(rs)
+    a = np.abs(x)
+    for q in (0.93, 0.90, 0.87, 0.83, 0.0, 1.0, 0.995, 0.5, 0.05, 0.31):
+        with np.errstate(invalid="ignore"):
+            got = O.quantile_abs(x, q)
+        want = torch.quantile(torch.from_numpy(a), q, dim=1).numpy()
+        np.testing.assert_array_equal(got, want, err_msg=f"q={q}")
+        assert got.dtype == np.float32
+    # the table's four cases on the row of nine 1s and two infs
+    row = np.r_[np.ones(9), np.full(2, np.inf)].astype(np.float32)[None]
+    assert [str(O.quantile_abs(row, q)[0]) for q in (0.93, 0.90, 0.87, 0.83)] == ["nan", "nan", "nan", "inf"]
+    # the floor keeps NaN (torch.maximum), so dynamic thresholding turns that whole sample into NaN
+    with np.errstate(invalid="ignore"):
+        thr = O.dynamic_thresholding(np.r_[np.ones(9), np.full(2, np.inf)].astype(np.float32)[None], 0.87, 1.0)
+    assert np.isnan(thr).all()
+
+
+def test_fma32_follows_ieee_on_non_finite_operands():
+    inf, nan = np.float32(np.inf), np.float32(np.nan)
+    one = np.float32(1)
+    cases = [((one, inf, one), inf), ((np.float32(0), inf, one), nan), ((np.float32(-0.13), inf, inf), nan),
+             ((np.float32(0.5), one, inf), inf), ((one, one, nan), nan), ((np.float32(-1), inf, -inf), -inf),
+             ((np.float32(3e38), np.float32(2), np.float32(0)), inf),            # finite operands, overflowing result
+             ((np.float32(3.4028235e38), one, np.float32(2.0 ** 103)), inf),    # exactly halfway to 2^128: to even (inf)
+             ((np.float32(3.4028235e38), one, np.float32(2.0 ** 102)), np.float32(3.4028235e38))]
+    for (a, b, c), want in cases:
+        got = O._fma32(a, b, c)
+        assert got.dtype == np.float32
+        assert got.tobytes() == np.float32(want).tobytes() or (np.isnan(got) and np.isnan(want)), (a, b, c, got)
