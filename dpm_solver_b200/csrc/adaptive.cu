@@ -124,9 +124,12 @@ int launch_adaptive_error(float* out, const void* xh, const void* xl, const void
   auto al = [&](const void* q) { return (reinterpret_cast<uintptr_t>(q) & (dtype == DPM_F32 ? 31 : 15)) == 0; };
   const bool vec = per_sample % kPacket == 0 && al(xh) && al(xl) && al(xp);
   const unsigned grid = (unsigned)(p.n_samples * p.chunks);
-  if (dtype == DPM_F32) { if (vec) k_err_partial<float, true><<<grid, kEThreads, 0, stream>>>(p); else k_err_partial<float, false><<<grid, kEThreads, 0, stream>>>(p); }
-  else if (dtype == DPM_BF16) { if (vec) k_err_partial<__nv_bfloat16, true><<<grid, kEThreads, 0, stream>>>(p); else k_err_partial<__nv_bfloat16, false><<<grid, kEThreads, 0, stream>>>(p); }
-  else { if (vec) k_err_partial<__half, true><<<grid, kEThreads, 0, stream>>>(p); else k_err_partial<__half, false><<<grid, kEThreads, 0, stream>>>(p); }
+  typedef void (*EKernel)(const EParams);
+  EKernel k = with_packet_pair(dtype, dtype, [&](auto pair) -> EKernel {
+    using T = typename decltype(pair)::TS;
+    return vec ? k_err_partial<T, true> : k_err_partial<T, false>;
+  });
+  k<<<grid, kEThreads, 0, stream>>>(p);
   k_err_final<<<1, kEThreads, 0, stream>>>(p);
   count_launch();
   count_launch();

@@ -28,31 +28,27 @@ bool pdl_enabled() {
   return on;
 }
 
-int sm_count() {
+int launch_error(const char* what, cudaError_t e) {
+  set_error("%s: %s", what, cudaGetErrorString(e));
+  cudaGetLastError();
+  return (int)e;
+}
+
+// attribute A of the current device, read once per device; FALLBACK (the H100's value) when it cannot be read
+template <cudaDeviceAttr A, int FALLBACK>
+static int device_attr() {
   static int cache[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return FALLBACK;
   if (cache[dev] == 0) {
     int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0)
-      v = 132;
+    if (cudaDeviceGetAttribute(&v, A, dev) != cudaSuccess || v <= 0) v = FALLBACK;
     cache[dev] = v;
   }
   return cache[dev];
 }
-int max_smem_optin() {
-  static int cache[64] = {0};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 227 * 1024;
-  if (cache[dev] == 0) {
-    int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess ||
-        v <= 0)
-      v = 227 * 1024;
-    cache[dev] = v;
-  }
-  return cache[dev];
-}
+int sm_count() { return device_attr<cudaDevAttrMultiProcessorCount, 132>(); }
+int max_smem_optin() { return device_attr<cudaDevAttrMaxSharedMemoryPerBlockOptin, 227 * 1024>(); }
 
 int ensure_max_smem(const void* kernel, bool nonportable_cluster) {
   static std::mutex mu;
@@ -67,11 +63,7 @@ int ensure_max_smem(const void* kernel, bool nonportable_cluster) {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, room);
   if (e == cudaSuccess && nonportable_cluster)
     e = cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-  if (e != cudaSuccess) {
-    set_error("shared-memory opt-in failed: %s", cudaGetErrorString(e));
-    cudaGetLastError();
-    return (int)e;
-  }
+  if (e != cudaSuccess) return launch_error("shared-memory opt-in failed", e);
   done.insert({dev, kernel});
   return 0;
 }
@@ -114,11 +106,11 @@ static int build_params(const dpm_step_desc* d, KParams* kp, Needs* nd, bool for
   }
   if ((d->n >> 3) > 0xffffffffull) { set_error("n too large (max 2^35-1 elements per call)"); return DPM_ERR_ARG; }
 
-  nd->x = form != DPM_FORM_NONE;
+  const FormReads reads = form_reads(form);
+  nd->x = reads.x;
   nd->m0 = d->n_model == 0;
-  nd->m1 = form == DPM_FORM_LIN2 || form == DPM_FORM_LIN3 || form == DPM_FORM_DIFF2 ||
-           form == DPM_FORM_MS3 || form == DPM_FORM_SS3T;
-  nd->m2 = form == DPM_FORM_LIN3 || form == DPM_FORM_MS3 || form == DPM_FORM_SS3T;
+  nd->m1 = reads.m1;
+  nd->m2 = reads.m2;
   nd->ec = d->n_model >= 1;
   nd->eu = d->n_model == 2;
   nd->xe = d->n_model >= 1 && (d->param == DPM_PARAM_X_START || d->param == DPM_PARAM_V || d->predict_x0);
@@ -206,14 +198,12 @@ static KParams shifted(const KParams& p, uint64_t elems) {
   return t;
 }
 
-static int finish(cudaStream_t) {
+// the result of an entry point whose launcher returned rc: rc itself when it failed, else the launch error the
+// runtime has pending (a <<<>>> launch reports its failure only there)
+static int finish(int rc) {
+  if (rc != DPM_OK) return rc;
   cudaError_t e = cudaPeekAtLastError();
-  if (e != cudaSuccess) {
-    set_error("CUDA launch failed: %s", cudaGetErrorString(e));
-    cudaGetLastError();
-    return (int)e;
-  }
-  return DPM_OK;
+  return e != cudaSuccess ? launch_error("CUDA launch failed", e) : DPM_OK;
 }
 
 static int step_impl(const dpm_step_desc* d, cudaStream_t stream) {
@@ -244,8 +234,7 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream) {
   } else if (p.n % kPacket) {
     rc = launch_step_scalar(shifted(p, (uint64_t)p.npk * kPacket), stream);  // tail
   }
-  if (rc != DPM_OK) return rc;
-  return finish(stream);
+  return finish(rc);
 }
 
 }  // namespace dpm
@@ -362,11 +351,9 @@ int dpm_duplicate(void* out, const void* x, uint64_t n, int dtype, dpm_stream_t 
   if (r == 1) {   // unaligned views: two plain device-to-device copies
     cudaError_t e = cudaMemcpyAsync(out, x, bytes, cudaMemcpyDeviceToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(static_cast<char*>(out) + bytes, x, bytes, cudaMemcpyDeviceToDevice, st);
-    if (e != cudaSuccess) { set_error("duplicate: %s", cudaGetErrorString(e)); cudaGetLastError(); return (int)e; }
-    return DPM_OK;
+    return e != cudaSuccess ? launch_error("duplicate", e) : DPM_OK;
   }
-  if (r != 0) return r;
-  return finish(st);
+  return finish(r);
 }
 
 int dpm_philox_policy(uint64_t numel, uint32_t* grid, uint64_t* counter_offset) {
@@ -379,18 +366,16 @@ int dpm_add_noise_philox(void* xt, const void* x, uint64_t n, int t_count, const
                          uint64_t seed, uint64_t offset, int x_dtype, int out_dtype, dpm_stream_t stream) {
   if (n == 0 || t_count == 0) return DPM_OK;
   if (!xt || !x || !alpha_t || !sigma_t || !valid_dtype(x_dtype) || !valid_dtype(out_dtype)) { set_error("add_noise: NULL argument or bad dtype"); return DPM_ERR_ARG; }
-  int rc = launch_noise_philox(xt, x, nullptr, nullptr, 0, n, t_count, alpha_t, sigma_t, seed, offset, x_dtype, out_dtype,
-                               static_cast<cudaStream_t>(stream));
-  return rc != DPM_OK ? rc : finish(static_cast<cudaStream_t>(stream));
+  return finish(launch_noise_philox(xt, x, nullptr, nullptr, 0, n, t_count, alpha_t, sigma_t, seed, offset, x_dtype,
+                                    out_dtype, static_cast<cudaStream_t>(stream)));
 }
 
 int dpm_diffedit_corrector(void* out, const void* x, const void* x0, const float* mask, uint64_t mask_n, uint64_t n,
                            float alpha_t, float sigma_t, uint64_t seed, uint64_t offset, int dtype, dpm_stream_t stream) {
   if (n == 0) return DPM_OK;
   if (!out || !x || !x0 || !mask || mask_n == 0 || n % mask_n != 0 || !valid_dtype(dtype)) { set_error("corrector: NULL argument, bad dtype or a mask that does not tile x"); return DPM_ERR_ARG; }
-  int rc = launch_noise_philox(out, x0, x, mask, mask_n, n, 1, &alpha_t, &sigma_t, seed, offset, dtype, dtype,
-                               static_cast<cudaStream_t>(stream));
-  return rc != DPM_OK ? rc : finish(static_cast<cudaStream_t>(stream));
+  return finish(launch_noise_philox(out, x0, x, mask, mask_n, n, 1, &alpha_t, &sigma_t, seed, offset, dtype, dtype,
+                                    static_cast<cudaStream_t>(stream)));
 }
 
 size_t dpm_dynamic_threshold_workspace(uint64_t n_samples, uint64_t per_sample) {
@@ -407,29 +392,23 @@ int dpm_dynamic_threshold(float* s_out, const dpm_step_desc* desc, float q, floa
   int rc = build_params(desc, &p, &nd, true);
   if (rc != DPM_OK) return rc;
   if (p.n == 0) return DPM_OK;
-  rc = launch_quantile(s_out, p, p.n / p.per_sample, q, max_val, workspace, workspace_bytes,
-                       static_cast<cudaStream_t>(stream));
-  if (rc != DPM_OK) return rc;
-  return finish(static_cast<cudaStream_t>(stream));
+  return finish(launch_quantile(s_out, p, p.n / p.per_sample, q, max_val, workspace, workspace_bytes,
+                                static_cast<cudaStream_t>(stream)));
 }
 
 int dpm_adaptive_init(const dpm_adaptive_ctl* ctl, float t_T, float h_init, dpm_stream_t stream) {
-  int rc = launch_adaptive_init(ctl, t_T, h_init, static_cast<cudaStream_t>(stream));
-  return rc != DPM_OK ? rc : finish(static_cast<cudaStream_t>(stream));
+  return finish(launch_adaptive_init(ctl, t_T, h_init, static_cast<cudaStream_t>(stream)));
 }
 int dpm_adaptive_plan(const dpm_adaptive_ctl* ctl, dpm_stream_t stream) {
-  int rc = launch_adaptive_plan(ctl, static_cast<cudaStream_t>(stream));
-  return rc != DPM_OK ? rc : finish(static_cast<cudaStream_t>(stream));
+  return finish(launch_adaptive_plan(ctl, static_cast<cudaStream_t>(stream)));
 }
 int dpm_adaptive_decide(const dpm_adaptive_ctl* ctl, dpm_stream_t stream) {
-  int rc = launch_adaptive_decide(ctl, static_cast<cudaStream_t>(stream));
-  return rc != DPM_OK ? rc : finish(static_cast<cudaStream_t>(stream));
+  return finish(launch_adaptive_decide(ctl, static_cast<cudaStream_t>(stream)));
 }
 int dpm_select_copy(void* dst, const void* src, const float* state, uint64_t bytes, dpm_stream_t stream) {
   if (bytes == 0) return DPM_OK;
   if (!dst || !src || !state) { set_error("select copy: NULL argument"); return DPM_ERR_ARG; }
-  int rc = launch_select_copy(dst, src, state, bytes, static_cast<cudaStream_t>(stream));
-  return rc != DPM_OK ? rc : finish(static_cast<cudaStream_t>(stream));
+  return finish(launch_select_copy(dst, src, state, bytes, static_cast<cudaStream_t>(stream)));
 }
 
 size_t dpm_adaptive_error_workspace(uint64_t n, uint64_t per_sample) {
@@ -441,10 +420,8 @@ int dpm_adaptive_error(float* e_out, const void* x_higher, const void* x_lower, 
                        size_t workspace_bytes, dpm_stream_t stream) {
   if (!e_out || !x_higher || !x_lower || !x_prev) { set_error("adaptive error: NULL tensor"); return DPM_ERR_ARG; }
   if (!valid_dtype(dtype) || per_sample == 0 || n == 0 || n % per_sample) { set_error("adaptive error: bad dtype or sizes"); return DPM_ERR_ARG; }
-  int rc = launch_adaptive_error(e_out, x_higher, x_lower, x_prev, atol, rtol, per_sample, n, dtype, workspace,
-                                 workspace_bytes, static_cast<cudaStream_t>(stream));
-  if (rc != DPM_OK) return rc;
-  return finish(static_cast<cudaStream_t>(stream));
+  return finish(launch_adaptive_error(e_out, x_higher, x_lower, x_prev, atol, rtol, per_sample, n, dtype, workspace,
+                                      workspace_bytes, static_cast<cudaStream_t>(stream)));
 }
 
 }  // extern "C"

@@ -87,26 +87,6 @@ __device__ __forceinline__ void ldg_pk(Raw<T16>& v, const T16* p) {
                : "=r"(v.r[0]), "=r"(v.r[1]), "=r"(v.r[2]), "=r"(v.r[3])
                : "l"(p));
 }
-// the same loads with an L2 eviction-priority hint (createpolicy ... L2::evict_last / evict_first): used by experiments
-// on keeping a sample group's (x, eps) resident between the quantile's count pass and the step that re-reads them
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t pol;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
-__device__ __forceinline__ void ldg_pk_hint(Raw<float>& v, const float* p, uint64_t pol) {
-  asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v4.b32 {%0,%1,%2,%3}, [%8], %9;\n\t"
-               "ld.global.L1::no_allocate.L2::cache_hint.v4.b32 {%4,%5,%6,%7}, [%8+16], %9;"
-               : "=r"(v.r[0]), "=r"(v.r[1]), "=r"(v.r[2]), "=r"(v.r[3]), "=r"(v.r[4]),
-                 "=r"(v.r[5]), "=r"(v.r[6]), "=r"(v.r[7])
-               : "l"(p), "l"(pol));
-}
-template <typename T16>
-__device__ __forceinline__ void ldg_pk_hint(Raw<T16>& v, const T16* p, uint64_t pol) {
-  asm volatile("ld.global.L1::no_allocate.L2::cache_hint.v4.b32 {%0,%1,%2,%3}, [%4], %5;"
-               : "=r"(v.r[0]), "=r"(v.r[1]), "=r"(v.r[2]), "=r"(v.r[3])
-               : "l"(p), "l"(pol));
-}
 __device__ __forceinline__ void stg_pk(float* p, const Raw<float>& v) {
   asm volatile("st.global.L1::no_allocate.v4.b32 [%0], {%1,%2,%3,%4};\n\t"
                "st.global.L1::no_allocate.v4.b32 [%0+16], {%5,%6,%7,%8};" ::"l"(p),
@@ -119,28 +99,6 @@ __device__ __forceinline__ void stg_pk(T16* p, const Raw<T16>& v) {
   asm volatile("st.global.L1::no_allocate.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.r[0]),
                "r"(v.r[1]), "r"(v.r[2]), "r"(v.r[3])
                : "memory");
-}
-
-// shared-memory packet access (TMA variant)
-__device__ __forceinline__ void lds_pk(Raw<float>& v, const float* p) {
-  const uint4* q = reinterpret_cast<const uint4*>(p);
-  uint4 a = q[0], b = q[1];
-  v.r[0] = a.x; v.r[1] = a.y; v.r[2] = a.z; v.r[3] = a.w;
-  v.r[4] = b.x; v.r[5] = b.y; v.r[6] = b.z; v.r[7] = b.w;
-}
-template <typename T16>
-__device__ __forceinline__ void lds_pk(Raw<T16>& v, const T16* p) {
-  uint4 a = *reinterpret_cast<const uint4*>(p);
-  v.r[0] = a.x; v.r[1] = a.y; v.r[2] = a.z; v.r[3] = a.w;
-}
-__device__ __forceinline__ void sts_pk(float* p, const Raw<float>& v) {
-  uint4* q = reinterpret_cast<uint4*>(p);
-  q[0] = make_uint4(v.r[0], v.r[1], v.r[2], v.r[3]);
-  q[1] = make_uint4(v.r[4], v.r[5], v.r[6], v.r[7]);
-}
-template <typename T16>
-__device__ __forceinline__ void sts_pk(T16* p, const Raw<T16>& v) {
-  *reinterpret_cast<uint4*>(p) = make_uint4(v.r[0], v.r[1], v.r[2], v.r[3]);
 }
 
 // unpack / pack -----------------------------------------------------------------------------
@@ -335,48 +293,6 @@ __device__ __forceinline__ float model_value(const KParams& p, float xe, float e
   return eps;
 }
 
-// Same computation for a packet of 8 elements, with the launch-uniform switches hoisted out of
-// the element loop (hand loop-unswitching): noise-parameterised networks -- the common case --
-// run straight-line code; everything else takes the generic per-element function above.
-// `thr8` is only read when clamp is set.
-template <int NE>
-__device__ __forceinline__ void model_values8(const KParams& p, const float (&xe)[8],
-                                              const float (&ec)[8], const float (&eu)[8],
-                                              const float (&thr8)[8], bool clamp, bool thr_uniform,
-                                              float (&T)[8]) {
-  if (p.fast_div && p.param == DPM_PARAM_NOISE && (!clamp || thr_uniform)) {
-    float eps[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) eps[i] = (NE == 2) ? eu[i] + p.guidance * (ec[i] - eu[i]) : ec[i];  // :330
-    if (!p.predict_x0) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) T[i] = eps[i];
-      return;
-    }
-    float x0[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) x0[i] = xe[i] - p.sigma_e * eps[i];
-    div_const8(x0, p.alpha_e, p.r_alpha);  // :439
-    if (clamp) {
-      const float s = thr8[0];
-      if (recip_div_ok(s)) {
-        const float rs = __frcp_rn(s);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) x0[i] = clamp_sym(x0[i], s);
-        div_const8(x0, s, rs);  // :424
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) x0[i] = clamp_sym(x0[i], s) / s;
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) T[i] = x0[i];
-    return;
-  }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) T[i] = model_value<NE>(p, xe[i], ec[i], NE == 2 ? eu[i] : 0.f, thr8[i], clamp);
-}
-
 // round a packet to its storage type once: returns the packed words and rewrites f[] with the
 // values as they will read back (so fused and unfused paths agree bit for bit)
 __device__ __forceinline__ void round_pack(Raw<float>& r, float (&f)[8]) { pack(r, f); }
@@ -498,13 +414,16 @@ __host__ __forceinline__ bool fast_path_ok(const KParams& p) {
   return true;
 }
 
-// compile-time stream requirements of a form
-template <int FORM> struct FormNeeds {
-  static constexpr bool kX = FORM != DPM_FORM_NONE;
-  static constexpr bool kM1 = FORM == DPM_FORM_LIN2 || FORM == DPM_FORM_LIN3 ||
-                              FORM == DPM_FORM_DIFF2 || FORM == DPM_FORM_MS3 ||
-                              FORM == DPM_FORM_SS3T;
-  static constexpr bool kM2 = FORM == DPM_FORM_LIN3 || FORM == DPM_FORM_MS3 || FORM == DPM_FORM_SS3T;
+// the state and buffer streams a form reads: the kernels (at compile time), the generic kernel, the TMA stage
+// layout and the host-side argument and alignment checks all take them from here
+struct FormReads {
+  bool x, m1, m2;
 };
+__host__ __device__ constexpr FormReads form_reads(int form) {
+  return {form != DPM_FORM_NONE,
+          form == DPM_FORM_LIN2 || form == DPM_FORM_LIN3 || form == DPM_FORM_DIFF2 || form == DPM_FORM_MS3 ||
+              form == DPM_FORM_SS3T,
+          form == DPM_FORM_LIN3 || form == DPM_FORM_MS3 || form == DPM_FORM_SS3T};
+}
 
 }  // namespace dpm

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace dpm {
@@ -20,6 +22,59 @@ void count_launch();                // bump the library launch counter
 // cluster sizes) the first time it is used on the current device; later calls are a hash lookup
 int ensure_max_smem(const void* kernel, bool nonportable_cluster = false);
 void set_error(const char* fmt, ...);
+int launch_error(const char* what, cudaError_t e);   // records "what: <CUDA error>", clears it, returns its code
+
+// ---- runtime -> compile-time dispatch of the kernel pickers ----------------------------------------
+template <typename TE_, typename TS_> struct PacketPair {
+  using TE = TE_;   // network output
+  using TS = TS_;   // state and buffers
+};
+// Calls f(PacketPair<TE, TS>{}) for a runtime (model dtype, state dtype) that is one of the five pairs the packet
+// kernels are built for: f32/f32, bf16/bf16, f16/f16, bf16->f32, f16->f32. Other pairs give a value-initialised result.
+template <typename F>
+static inline auto with_packet_pair(int md, int sd, F&& f) -> decltype(f(PacketPair<float, float>{})) {
+  if (md == DPM_F32 && sd == DPM_F32) return f(PacketPair<float, float>{});
+  if (md == DPM_BF16 && sd == DPM_BF16) return f(PacketPair<__nv_bfloat16, __nv_bfloat16>{});
+  if (md == DPM_F16 && sd == DPM_F16) return f(PacketPair<__half, __half>{});
+  if (md == DPM_BF16 && sd == DPM_F32) return f(PacketPair<__nv_bfloat16, float>{});
+  if (md == DPM_F16 && sd == DPM_F32) return f(PacketPair<__half, float>{});
+  return {};
+}
+// Calls f(std::integral_constant<int, FORM>{}) for a runtime dpm_form. Other values give a value-initialised result.
+template <typename F>
+static inline auto with_form(int form, F&& f) -> decltype(f(std::integral_constant<int, DPM_FORM_NONE>{})) {
+  switch (form) {
+    case DPM_FORM_NONE: return f(std::integral_constant<int, DPM_FORM_NONE>{});
+    case DPM_FORM_LIN1: return f(std::integral_constant<int, DPM_FORM_LIN1>{});
+    case DPM_FORM_LIN2: return f(std::integral_constant<int, DPM_FORM_LIN2>{});
+    case DPM_FORM_LIN3: return f(std::integral_constant<int, DPM_FORM_LIN3>{});
+    case DPM_FORM_DIFF2: return f(std::integral_constant<int, DPM_FORM_DIFF2>{});
+    case DPM_FORM_MS3: return f(std::integral_constant<int, DPM_FORM_MS3>{});
+    case DPM_FORM_SS3T: return f(std::integral_constant<int, DPM_FORM_SS3T>{});
+  }
+  return {};
+}
+// The step kernel pick(PacketPair<TE, TS>{}, NE, FORM) names for a launch (NE and FORM as std::integral_constant).
+// A launch without network outputs (NE == 0) reads state-typed streams only: it is served by the same-type pairs
+// (TE = TS, picked by the state dtype), and not for FORM_NONE, which would compute nothing.
+template <typename R, typename Pick>
+static inline R pick_step(const KParams& p, Pick&& pick) {
+  const int md = p.n_model == 0 ? p.state_dtype : p.model_dtype;
+  return with_packet_pair(md, p.state_dtype, [&](auto pair) -> R {
+    return with_form(p.form, [&](auto form) -> R {
+      using Pair = decltype(pair);
+      switch (p.n_model) {
+        case 0:
+          if constexpr (decltype(form)::value != DPM_FORM_NONE && std::is_same_v<typename Pair::TE, typename Pair::TS>)
+            return pick(pair, std::integral_constant<int, 0>{}, form);
+          return R{};
+        case 1: return pick(pair, std::integral_constant<int, 1>{}, form);
+        case 2: return pick(pair, std::integral_constant<int, 2>{}, form);
+      }
+      return R{};
+    });
+  });
+}
 
 // Programmatic dependent launch (PDL): the step kernels call pdl_wait() after their prologue (barrier init, index
 // setup) and before touching global memory, and pdl_trigger() at entry; launched with the programmatic-stream-

@@ -39,6 +39,8 @@ constexpr int kBins = 2048;
 constexpr int kSamples = 1024;      // sample keys per sample (pivot kernel)
 constexpr int kPThreads = 256;      // pivot / count / finish kernels
 constexpr int kLocalCand = 2048;    // bracket keys one count-CTA may collect
+constexpr int kQUnroll = 2;         // count kernel: packets per thread per chunk
+constexpr int kQIters = 4;          // count kernel: consecutive chunks per CTA
 
 struct QParams {
   uint64_t lo;        // floor(pos)
@@ -51,9 +53,7 @@ struct QParams {
   float* s_out;
   uint32_t* work;     // pipeline workspace: [n_samples][8] header words, then [n_samples][cap] candidates
   uint64_t n_samples;
-  uint32_t iters;     // count kernel: consecutive chunks per CTA
   uint32_t num_space; // pipeline: bracket keys are |numerator| patterns (plain eps -> x0 map, alpha > 0)
-  uint32_t evict_last; // experiment (DPM_Q_EVICT_LAST=1): count-pass loads ask L2 to keep the lines (evict_last)
 };
 // header words per sample
 enum { H_LO = 0, H_HI = 1, H_LT = 2, H_IN = 3, H_PATH = 4, H_ALO = 5, H_AHI = 6, H_NAN = 7, H_WORDS = 8 };
@@ -109,13 +109,18 @@ __device__ __forceinline__ Sel select_bin(const uint32_t* tot, uint64_t k, uint3
 template <int NE, typename TE, typename TS>
 __device__ __forceinline__ void keys_of_packet(const KParams& p, const Raw<TS>& rx, const Raw<TE>& rc,
                                                const Raw<TE>& ru, uint32_t (&k8)[8]) {
-  float fx[8], fc[8], fu[8], one[8], fT[8];
+  float fx[8], fc[8], fu[8], fT[8];
   unpack(rx, fx);
   unpack(rc, fc);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) { fu[i] = 0.f; one[i] = 1.f; }
+  for (int i = 0; i < 8; ++i) fu[i] = 0.f;
   if (NE == 2) unpack(ru, fu);
-  model_values8<NE>(p, fx, fc, fu, one, false, true, fT);
+  if (p.fast_div && p.param == DPM_PARAM_NOISE) {
+    fast_model8<NE>(p, fx, fc, fu, false, 1.f, fT);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) fT[i] = model_value<NE>(p, fx[i], fc[i], fu[i], 1.f, false);
+  }
 #pragma unroll
   for (int i = 0; i < 8; ++i) k8[i] = __float_as_uint(fabsf(fT[i]));
 }
@@ -302,8 +307,8 @@ __global__ void __launch_bounds__(kPThreads) k_q_count(const __grid_constant__ K
     }
   };
 #pragma unroll 1
-  for (uint32_t it = 0; it < qp.iters; ++it) {
-    const uint64_t c_begin = ((uint64_t)part * qp.iters + it) * kChunk;
+  for (uint32_t it = 0; it < kQIters; ++it) {
+    const uint64_t c_begin = ((uint64_t)part * kQIters + it) * kChunk;
     if (c_begin >= p.per_sample) break;
     const uint64_t c_end = c_begin + kChunk < p.per_sample ? c_begin + kChunk : p.per_sample;
     const uint32_t cnt = (uint32_t)(c_end - c_begin);
@@ -320,16 +325,9 @@ __global__ void __launch_bounds__(kPThreads) k_q_count(const __grid_constant__ K
         const uint32_t pk = u * kPThreads + tid;
         if (pk < npk) {
           const size_t e = e0 + (size_t)pk * kPacket;
-          if (qp.evict_last) {
-            const uint64_t pol = l2_policy_evict_last();
-            ldg_pk_hint(rx[u], gxe + e, pol);
-            ldg_pk_hint(rc[u], gec + e, pol);
-            if (NE == 2) ldg_pk_hint(ru[u], geu + e, pol);
-          } else {
-            ldg_pk(rx[u], gxe + e);
-            ldg_pk(rc[u], gec + e);
-            if (NE == 2) ldg_pk(ru[u], geu + e);
-          }
+          ldg_pk(rx[u], gxe + e);
+          ldg_pk(rc[u], gec + e);
+          if (NE == 2) ldg_pk(ru[u], geu + e);
         }
       }
 #pragma unroll
@@ -617,25 +615,9 @@ __global__ void __launch_bounds__(kQThreads)
 
 
 typedef void (*QKernel)(const KParams, const QParams);
-
-template <typename TE, typename TS>
-static QKernel pick_cluster(int ne, bool vec) {
-  if (ne == 2) return vec ? k_quantile_cluster<TE, TS, 2, true> : k_quantile_cluster<TE, TS, 2, false>;
-  return vec ? k_quantile_cluster<TE, TS, 1, true> : k_quantile_cluster<TE, TS, 1, false>;
-}
-template <typename TE, typename TS>
-static QKernel pick_count(int ne, bool vec, int u) {
-  if (u == 2) {
-    if (ne == 2) return vec ? k_q_count<TE, TS, 2, true, 2> : k_q_count<TE, TS, 2, false, 2>;
-    return vec ? k_q_count<TE, TS, 1, true, 2> : k_q_count<TE, TS, 1, false, 2>;
-  }
-  if (ne == 2) return vec ? k_q_count<TE, TS, 2, true, 4> : k_q_count<TE, TS, 2, false, 4>;
-  return vec ? k_q_count<TE, TS, 1, true, 4> : k_q_count<TE, TS, 1, false, 4>;
-}
-static int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return (e && *e) ? atoi(e) : dflt;
-}
+struct QKernels {
+  QKernel cluster, count;
+};
 
 static uint32_t pipeline_cap(uint64_t ps) {
   // the 4-sigma bracket of a 1024-key sample holds <= 2*(4*sqrt(1024*q(1-q))+3)+1 sample ranks; for
@@ -661,23 +643,31 @@ int launch_quantile(float* s_out, const KParams& p, uint64_t n_samples, float q,
   auto al = [](const void* ptr, int dt) { return (reinterpret_cast<uintptr_t>(ptr) & (dt == DPM_F32 ? 31 : 15)) == 0; };
   if (!al(p.xe, sd) || !al(p.ec, md) || (p.n_model == 2 && !al(p.eu, md))) vec = false;
 
-  QKernel kc = nullptr, kn = nullptr;
-  const int cu = env_int("DPM_Q_UNROLL", 2) == 4 ? 4 : 2;   // packets per thread per iteration (tuning)
-#define DPM_PICK(TE, TS) { kc = pick_cluster<TE, TS>(p.n_model, vec); kn = pick_count<TE, TS>(p.n_model, vec, cu); }
-  if (md == DPM_F32 && sd == DPM_F32) DPM_PICK(float, float)
-  else if (md == DPM_BF16 && sd == DPM_BF16) DPM_PICK(__nv_bfloat16, __nv_bfloat16)
-  else if (md == DPM_F16 && sd == DPM_F16) DPM_PICK(__half, __half)
-  else if (md == DPM_BF16 && sd == DPM_F32) DPM_PICK(__nv_bfloat16, float)
-  else if (md == DPM_F16 && sd == DPM_F32) DPM_PICK(__half, float)
-  else if (md == DPM_F32 && sd == DPM_BF16) DPM_PICK(float, __nv_bfloat16)   // fp32 network output, 16-bit state
-  else if (md == DPM_F32 && sd == DPM_F16) DPM_PICK(float, __half)
-  else if ((md == DPM_BF16 && sd == DPM_F16) || (md == DPM_F16 && sd == DPM_BF16)) {
-    // two different 16-bit types have no packet instantiation: the VEC = false kernels read every operand
-    // through load_any with the runtime dtypes (the template types are unused there)
-    vec = false;
-    DPM_PICK(float, float)
-  } else { set_error("dynamic threshold: unsupported dtype mix (model %d, state %d)", md, sd); return DPM_ERR_UNSUPPORTED; }
-#undef DPM_PICK
+  auto pick = [&](auto pair) -> QKernels {
+    using TE = typename decltype(pair)::TE;
+    using TS = typename decltype(pair)::TS;
+    if (p.n_model == 2)
+      return {vec ? k_quantile_cluster<TE, TS, 2, true> : k_quantile_cluster<TE, TS, 2, false>,
+              vec ? k_q_count<TE, TS, 2, true, kQUnroll> : k_q_count<TE, TS, 2, false, kQUnroll>};
+    return {vec ? k_quantile_cluster<TE, TS, 1, true> : k_quantile_cluster<TE, TS, 1, false>,
+            vec ? k_q_count<TE, TS, 1, true, kQUnroll> : k_q_count<TE, TS, 1, false, kQUnroll>};
+  };
+  QKernels k = with_packet_pair(md, sd, pick);   // the step kernels' five pairs
+  if (k.cluster == nullptr) {
+    if (md == DPM_F32 && sd == DPM_BF16) {   // fp32 network output, 16-bit state
+      k = pick(PacketPair<float, __nv_bfloat16>{});
+    } else if (md == DPM_F32 && sd == DPM_F16) {
+      k = pick(PacketPair<float, __half>{});
+    } else if ((md == DPM_BF16 && sd == DPM_F16) || (md == DPM_F16 && sd == DPM_BF16)) {
+      // two different 16-bit types have no packet instantiation: the VEC = false kernels read every operand
+      // through load_any with the runtime dtypes (the template types are unused there)
+      vec = false;
+      k = pick(PacketPair<float, float>{});
+    } else {
+      set_error("dynamic threshold: unsupported dtype mix (model %d, state %d)", md, sd);
+      return DPM_ERR_UNSUPPORTED;
+    }
+  }
 
   // torch.quantile rank arithmetic, in fp32: pos = fl(q * (n-1))
   const float pos = q * (float)(ps - 1);
@@ -704,20 +694,17 @@ int launch_quantile(float* s_out, const KParams& p, uint64_t n_samples, float q,
     const double f = ps > 1 ? (double)qp.lo / (double)(ps - 1) : 0.0;
     qp.margin = (int32_t)(6.0 * sqrt((double)kSamples * f * (1.0 - f)) + 3.0);   // 4 sigma at ~kSamples/2 effective draws
     qp.cap = pipeline_cap(ps);
-    qp.iters = (uint32_t)env_int("DPM_Q_ITERS", 4);
-    if (qp.iters < 1) qp.iters = 1;
-    const uint64_t per_cta = (uint64_t)cu * kPacket * kPThreads * qp.iters;
+    const uint64_t per_cta = (uint64_t)kQUnroll * kPacket * kPThreads * kQIters;
     qp.slice = (uint32_t)((ps + per_cta - 1) / per_cta);
     qp.work = static_cast<uint32_t*>(workspace);
     // division-free classification and |numerator| candidates need the plain eps -> x0 map with a positive alpha
     qp.num_space = (vec && p.param == DPM_PARAM_NOISE && p.predict_x0 && p.alpha_e > 0.f) ? 1u : 0u;
-    qp.evict_last = env_int("DPM_Q_EVICT_LAST", 0) ? 1u : 0u;
     if (n_samples * qp.slice > 0x7fffffffull) { set_error("too many chunks"); return DPM_ERR_UNSUPPORTED; }
     QKernel kp = p.n_model == 2 ? k_q_pivots<2> : k_q_pivots<1>;
     QKernel kf = p.n_model == 2 ? k_q_finish<2> : k_q_finish<1>;
     kp<<<(unsigned)n_samples, kPThreads, 0, stream>>>(p, qp);
-    e = launch_pdl(kn, (unsigned)(n_samples * qp.slice), kPThreads, 0, stream, p, qp);
-    if (e != cudaSuccess) { set_error("quantile count launch failed: %s", cudaGetErrorString(e)); cudaGetLastError(); return (int)e; }
+    e = launch_pdl(k.count, (unsigned)(n_samples * qp.slice), kPThreads, 0, stream, p, qp);
+    if (e != cudaSuccess) return launch_error("quantile count launch failed", e);
     // finish: stage the candidates in shared memory when they fit next to 3 co-resident CTAs (else read L2)
     QParams qf = qp;
     const size_t fsmem = (size_t)qp.cap * sizeof(uint32_t);
@@ -727,7 +714,7 @@ int launch_quantile(float* s_out, const KParams& p, uint64_t n_samples, float q,
       if (rc != 0) return rc;
     }
     e = launch_pdl(kf, (unsigned)n_samples, kPThreads, qf.slice ? fsmem : 0, stream, p, qf);
-    if (e != cudaSuccess) { set_error("quantile finish launch failed: %s", cudaGetErrorString(e)); cudaGetLastError(); return (int)e; }
+    if (e != cudaSuccess) return launch_error("quantile finish launch failed", e);
     count_launch();
     count_launch();
     count_launch();
@@ -755,7 +742,7 @@ int launch_quantile(float* s_out, const KParams& p, uint64_t n_samples, float q,
   if (slice > 0xffffffffull) { set_error("per_sample too large"); return DPM_ERR_UNSUPPORTED; }
 
   const size_t smem = fixed + (size_t)cap * sizeof(uint32_t);
-  int rc = ensure_max_smem(reinterpret_cast<const void*>(kc), /*nonportable_cluster=*/true);
+  int rc = ensure_max_smem(reinterpret_cast<const void*>(k.cluster), /*nonportable_cluster=*/true);
   if (rc != 0) return rc;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
@@ -770,8 +757,8 @@ int launch_quantile(float* s_out, const KParams& p, uint64_t n_samples, float q,
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, kc, p, qp);
-  if (e != cudaSuccess) { set_error("quantile launch failed: %s", cudaGetErrorString(e)); return (int)e; }
+  e = cudaLaunchKernelEx(&cfg, k.cluster, p, qp);
+  if (e != cudaSuccess) return launch_error("quantile launch failed", e);
   count_launch();
   return DPM_OK;
 }

@@ -8,10 +8,7 @@
 
 namespace dpm {
 
-#ifndef DPM_UNROLL
-#define DPM_UNROLL 2
-#endif
-constexpr int kUnroll = DPM_UNROLL;
+constexpr int kUnroll = 2;
 constexpr int kMaxThreads = 512;
 
 // FAST: the straight-line packet code of common.cuh (fast_model8 / fast_update8; launch-time test
@@ -22,7 +19,7 @@ constexpr int kMaxThreads = 512;
 template <typename TE, typename TS, int NE, int FORM, bool FAST, bool RND = false>
 __global__ void __launch_bounds__(kMaxThreads)
     k_step_direct(const __grid_constant__ KParams p) {
-  using Needs = FormNeeds<FORM>;
+  constexpr bool kX = form_reads(FORM).x, kM1 = form_reads(FORM).m1, kM2 = form_reads(FORM).m2;
   const TS* __restrict__ gx = static_cast<const TS*>(p.x);
   const TS* __restrict__ gxe = static_cast<const TS*>(p.xe);
   const TS* __restrict__ gm0 = static_cast<const TS*>(p.m0);
@@ -36,7 +33,7 @@ __global__ void __launch_bounds__(kMaxThreads)
 
   const uint32_t npk = p.npk;
   const uint32_t tile_pk = blockDim.x * kUnroll;
-  const bool sep_xe = (NE > 0) && p.use_xe && !(Needs::kX && p.xe_is_x);
+  const bool sep_xe = (NE > 0) && p.use_xe && !(kX && p.xe_is_x);
   const bool clamp = (NE > 0) && (p.thr != nullptr);
   pdl_trigger();
   pdl_wait();
@@ -51,7 +48,7 @@ __global__ void __launch_bounds__(kMaxThreads)
       const uint64_t pk = tile0 + (uint64_t)u * blockDim.x + threadIdx.x;
       if (pk < npk) {
         const size_t e = (size_t)pk * kPacket;
-        if (Needs::kX) ldg_pk(rx[u], gx + e);
+        if (kX) ldg_pk(rx[u], gx + e);
         if (NE > 0) {
           ldg_pk(rec[u], gec + e);
           if (NE == 2) ldg_pk(reu[u], geu + e);
@@ -59,8 +56,8 @@ __global__ void __launch_bounds__(kMaxThreads)
         } else {
           ldg_pk(rm0[u], gm0 + e);
         }
-        if (Needs::kM1) ldg_pk(rm1[u], gm1 + e);
-        if (Needs::kM2) ldg_pk(rm2[u], gm2 + e);
+        if (kM1) ldg_pk(rm1[u], gm1 + e);
+        if (kM2) ldg_pk(rm2[u], gm2 + e);
       }
     }
     // ---- compute + store ----
@@ -70,9 +67,9 @@ __global__ void __launch_bounds__(kMaxThreads)
       if (pk < npk) {
         const size_t e = (size_t)pk * kPacket;
         float fx[8], fxe[8], fT[8], fm1[8], fm2[8], fo[8];
-        if (Needs::kX) unpack(rx[u], fx);
-        if (Needs::kM1) unpack(rm1[u], fm1);
-        if (Needs::kM2) unpack(rm2[u], fm2);
+        if (kX) unpack(rx[u], fx);
+        if (kM1) unpack(rm1[u], fm1);
+        if (kM2) unpack(rm2[u], fm2);
         if (NE > 0 && FAST) {
           float fec[8], feu[8];
           unpack(rec[u], fec);
@@ -93,7 +90,7 @@ __global__ void __launch_bounds__(kMaxThreads)
           if (NE == 2) unpack(reu[u], feu);
           if (sep_xe) {
             unpack(rxe[u], fxe);
-          } else if (Needs::kX) {
+          } else if (kX) {
 #pragma unroll
             for (int i = 0; i < 8; ++i) fxe[i] = fx[i];
           } else {
@@ -130,8 +127,8 @@ __global__ void __launch_bounds__(kMaxThreads)
           } else {
 #pragma unroll
             for (int i = 0; i < 8; ++i)
-              fo[i] = update_value<FORM, RND>(p, fx[i], fT[i], Needs::kM1 ? fm1[i] : 0.f,
-                                              Needs::kM2 ? fm2[i] : 0.f);
+              fo[i] = update_value<FORM, RND>(p, fx[i], fT[i], kM1 ? fm1[i] : 0.f,
+                                              kM2 ? fm2[i] : 0.f);
           }
           Raw<TS> ro;
           pack(ro, fo);
@@ -144,7 +141,8 @@ __global__ void __launch_bounds__(kMaxThreads)
 }
 
 // ---- fully generic element-wise kernel: any dtype mix, any alignment, tails ------------------
-// RND = true: reference-rounding mode (common.cuh); the only kernel that implements it so far.
+// RND = true: reference-rounding mode (common.cuh) for the launches the <RND> vector kernels do not serve:
+// unaligned views, tails and fp32 network outputs.
 template <bool RND>
 __global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KParams pc) {
   KParams p = pc;
@@ -157,11 +155,8 @@ __global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KPa
     p.fast_div = 0;
   }
   const int sd = p.state_dtype, md = p.model_dtype;
-  const bool need_x = p.form != DPM_FORM_NONE;
-  const bool need_m1 = p.form == DPM_FORM_LIN2 || p.form == DPM_FORM_LIN3 ||
-                       p.form == DPM_FORM_DIFF2 || p.form == DPM_FORM_MS3 ||
-                       p.form == DPM_FORM_SS3T;
-  const bool need_m2 = p.form == DPM_FORM_LIN3 || p.form == DPM_FORM_MS3 || p.form == DPM_FORM_SS3T;
+  const FormReads reads = form_reads(p.form);
+  const bool need_x = reads.x, need_m1 = reads.m1, need_m2 = reads.m2;
   const bool clamp = p.n_model > 0 && p.thr != nullptr;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n;
        i += (size_t)gridDim.x * blockDim.x) {
@@ -199,77 +194,30 @@ __global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KPa
 // ---- dispatch ---------------------------------------------------------------------------------
 typedef void (*StepKernel)(const KParams);
 
-// NE == 0 has no model conversion: only SS3T (division by w4) has a generic twin there.
-template <typename TE, typename TS, int NE, bool FAST>
-static StepKernel pick_form(int form) {
-  constexpr bool kTwin = NE > 0 || !FAST;   // is <FAST = false> a distinct kernel for this (NE, form)?
-  switch (form) {
-    case DPM_FORM_NONE: return NE > 0 ? k_step_direct<TE, TS, NE, DPM_FORM_NONE, FAST> : nullptr;
-    case DPM_FORM_LIN1: return k_step_direct<TE, TS, NE, DPM_FORM_LIN1, FAST || NE == 0>;
-    case DPM_FORM_LIN2: return k_step_direct<TE, TS, NE, DPM_FORM_LIN2, FAST || NE == 0>;
-    case DPM_FORM_LIN3: return k_step_direct<TE, TS, NE, DPM_FORM_LIN3, FAST || NE == 0>;
-    case DPM_FORM_DIFF2: return k_step_direct<TE, TS, NE, DPM_FORM_DIFF2, FAST || NE == 0>;
-    case DPM_FORM_MS3: return k_step_direct<TE, TS, NE, DPM_FORM_MS3, FAST || NE == 0>;
-    case DPM_FORM_SS3T: return k_step_direct<TE, TS, NE, DPM_FORM_SS3T, FAST>;
-  }
-  (void)kTwin;
-  return nullptr;
-}
-template <typename TE, typename TS, int NE>
-static StepKernel pick_fast(int form, bool fast) {
-  return fast ? pick_form<TE, TS, NE, true>(form) : pick_form<TE, TS, NE, false>(form);
-}
-template <typename TE, typename TS>
-static StepKernel pick_ne(int ne, int form, bool fast) {
-  switch (ne) {
-    case 1: return pick_fast<TE, TS, 1>(form, fast);
-    case 2: return pick_fast<TE, TS, 2>(form, fast);
-  }
-  return nullptr;
-}
-static StepKernel pick_direct(int md, int sd, int ne, int form, bool fast) {
-  if (ne == 0) {
-    switch (sd) {
-      case DPM_F32: return pick_fast<float, float, 0>(form, fast);
-      case DPM_BF16: return pick_fast<__nv_bfloat16, __nv_bfloat16, 0>(form, fast);
-      case DPM_F16: return pick_fast<__half, __half, 0>(form, fast);
+// FAST: NE == 0 has no model conversion, so there only SS3T (division by w4) has a <FAST = false> twin.
+// RND: an fp32 state with raw network outputs in bf16 / f16 (NE >= 1), or fp32 buffers holding such raw outputs
+// (NE == 0, differences rounded).
+static StepKernel pick_direct(const KParams& p) {
+  const bool fast = fast_path_ok(p), rnd = p.raw_round != 0;
+  return pick_step<StepKernel>(p, [&](auto pair, auto ne, auto form) -> StepKernel {
+    using TE = typename decltype(pair)::TE;
+    using TS = typename decltype(pair)::TS;
+    constexpr int NE = decltype(ne)::value, FORM = decltype(form)::value;
+    if (rnd) {
+      if constexpr (std::is_same_v<TS, float> && (NE == 0) == std::is_same_v<TE, float>)
+        return k_step_direct<TE, TS, NE, FORM, false, true>;
+      else
+        return nullptr;
     }
-    return nullptr;
-  }
-  if (md == DPM_F32 && sd == DPM_F32) return pick_ne<float, float>(ne, form, fast);
-  if (md == DPM_BF16 && sd == DPM_BF16) return pick_ne<__nv_bfloat16, __nv_bfloat16>(ne, form, fast);
-  if (md == DPM_F16 && sd == DPM_F16) return pick_ne<__half, __half>(ne, form, fast);
-  if (md == DPM_BF16 && sd == DPM_F32) return pick_ne<__nv_bfloat16, float>(ne, form, fast);
-  if (md == DPM_F16 && sd == DPM_F32) return pick_ne<__half, float>(ne, form, fast);
-  return nullptr;  // other mixes run on the generic kernel
-}
-
-// reference-rounding mode: fp32 state; raw network outputs in bf16 / f16 (NE >= 1), or fp32 buffers holding such raw
-// outputs (NE == 0, differences rounded)
-template <typename TE, int NE>
-static StepKernel pick_rnd_form(int form) {
-  switch (form) {
-    case DPM_FORM_NONE: return NE > 0 ? k_step_direct<TE, float, NE, DPM_FORM_NONE, false, true> : nullptr;
-    case DPM_FORM_LIN1: return k_step_direct<TE, float, NE, DPM_FORM_LIN1, false, true>;
-    case DPM_FORM_LIN2: return k_step_direct<TE, float, NE, DPM_FORM_LIN2, false, true>;
-    case DPM_FORM_LIN3: return k_step_direct<TE, float, NE, DPM_FORM_LIN3, false, true>;
-    case DPM_FORM_DIFF2: return k_step_direct<TE, float, NE, DPM_FORM_DIFF2, false, true>;
-    case DPM_FORM_MS3: return k_step_direct<TE, float, NE, DPM_FORM_MS3, false, true>;
-    case DPM_FORM_SS3T: return k_step_direct<TE, float, NE, DPM_FORM_SS3T, false, true>;
-  }
-  return nullptr;
-}
-static StepKernel pick_rnd(int md, int sd, int ne, int form) {
-  if (sd != DPM_F32) return nullptr;
-  if (ne == 0) return pick_rnd_form<float, 0>(form);
-  if (md == DPM_BF16) return ne == 1 ? pick_rnd_form<__nv_bfloat16, 1>(form) : pick_rnd_form<__nv_bfloat16, 2>(form);
-  if (md == DPM_F16) return ne == 1 ? pick_rnd_form<__half, 1>(form) : pick_rnd_form<__half, 2>(form);
-  return nullptr;
+    if constexpr (NE == 0 && FORM != DPM_FORM_SS3T)
+      return k_step_direct<TE, TS, NE, FORM, true>;
+    else
+      return fast ? k_step_direct<TE, TS, NE, FORM, true> : k_step_direct<TE, TS, NE, FORM, false>;
+  });
 }
 
 int launch_step_direct(const KParams& p, const Tuning& t, cudaStream_t stream) {
-  StepKernel k = p.raw_round ? pick_rnd(p.model_dtype, p.state_dtype, p.n_model, p.form)
-                             : pick_direct(p.model_dtype, p.state_dtype, p.n_model, p.form, fast_path_ok(p));
+  StepKernel k = pick_direct(p);
   if (k == nullptr) return 1;  // not served here
   const int threads = t.threads > 0 ? t.threads : 256;
   const uint32_t tile_pk = (uint32_t)threads * kUnroll;
@@ -278,7 +226,7 @@ int launch_step_direct(const KParams& p, const Tuning& t, cudaStream_t stream) {
   uint32_t grid = (uint32_t)(tiles < cap ? tiles : cap);
   if (grid == 0) return 0;
   cudaError_t le = launch_pdl(k, grid, (unsigned)threads, 0, stream, p);
-  if (le != cudaSuccess) { set_error("step launch failed: %s", cudaGetErrorString(le)); cudaGetLastError(); return (int)le; }
+  if (le != cudaSuccess) return launch_error("step launch failed", le);
   count_launch();
   return 0;
 }

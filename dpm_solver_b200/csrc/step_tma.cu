@@ -12,17 +12,14 @@
 //   fence.proxy.async -> thread 0: bulk wait_group.read(S-2) (frees the out-buffers of the
 //   next stage) -> __syncthreads -> thread 0: bulk-store stage s, commit, then refill the
 //   input buffers of stage s with tile i+S.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "launch.cuh"
 
 namespace dpm {
 
-#ifndef DPM_TMA_UNITS
-#define DPM_TMA_UNITS 2
-#endif
-constexpr int kTmaUnits = DPM_TMA_UNITS;   // packets per thread per tile (tile = threads * units packets); compile time
+// packets per thread per tile (tile = threads * kUnits packets), compile time: both packets' LDS issue before the
+// first use
+constexpr int kUnits = 2;
 constexpr int kTmaMaxThreads = 512;
 constexpr int kMaxStages = 8;
 
@@ -31,37 +28,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
-               "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra DONE_%=;\n"
-      "bra WAIT_%=;\n"
-      "DONE_%=:\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes,
-                                         uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::
-          "r"(smem_u32(dst)),
-      "l"(src), "r"(bytes), "r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void bulk_s2g(void* dst, const void* src, uint32_t bytes) {
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst),
-               "r"(smem_u32(src)), "r"(bytes)
-               : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read(int pending) {
@@ -126,8 +92,6 @@ __device__ __forceinline__ void mbar_wait32(uint32_t bar, uint32_t parity) {
       : "memory");
 }
 
-constexpr int kUnits = kTmaUnits;   // packets per thread per tile, compile time: both packets' LDS issue before the first use
-
 // Fast path only (launch_step_tma: fast_path_ok and no per-sample threshold): noise-parameterised network,
 // exact constant division. Everything that is uniform over a tile lives in uniform registers, computed once per
 // tile from 32-bit quantities (npk < 2^32): shared-window addresses of the stage's stream buffers, the tile's
@@ -136,7 +100,7 @@ template <typename TE, typename TS, int NE, int FORM>
 __global__ void __launch_bounds__(kTmaMaxThreads)
     k_step_tma(const __grid_constant__ KParams p, const __grid_constant__ StageLayout L,
                const int stages, const int /*units: compile time (kUnits)*/) {
-  using Needs = FormNeeds<FORM>;
+  constexpr bool kX = form_reads(FORM).x, kM1 = form_reads(FORM).m1, kM2 = form_reads(FORM).m2;
   extern __shared__ __align__(128) unsigned char smem[];
   const uint32_t sbar = smem_u32(smem);           // [kMaxStages] mbarriers
   const uint32_t sring = sbar + 128;
@@ -149,11 +113,11 @@ __global__ void __launch_bounds__(kTmaMaxThreads)
   // quantisation of the grid but scatters (CTAs x streams) concurrent streams over HBM and measured slower on the
   // first target GPU: kept round-robin.
   const uint32_t ntiles = (p.npk + tile_pk - 1) / tile_pk;
-  const bool has_x = Needs::kX || (NE > 0 && p.use_xe);  // state slot: x, or xe when no update
-  const bool sep_xe = (NE > 0) && p.use_xe && Needs::kX && !p.xe_is_x;  // extra slot: evaluation state
+  const bool has_x = kX || (NE > 0 && p.use_xe);  // state slot: x, or xe when no update
+  const bool sep_xe = (NE > 0) && p.use_xe && kX && !p.xe_is_x;  // extra slot: evaluation state
   const bool has_mo = (NE > 0) && (p.m_out != nullptr);
   const bool has_o2 = (FORM != DPM_FORM_NONE) && (p.out2 != nullptr);
-  const char* gstate = static_cast<const char*>(Needs::kX ? p.x : p.xe);
+  const char* gstate = static_cast<const char*>(kX ? p.x : p.xe);
   constexpr uint32_t kBS = Traits<TS>::kBytes * kPacket, kBM = Traits<TE>::kBytes * kPacket;   // bytes per packet
 
   pdl_trigger();
@@ -176,16 +140,16 @@ __global__ void __launch_bounds__(kTmaMaxThreads)
     if (NE >= 1) tx += bm;
     if (NE == 2) tx += bm;
     if (NE == 0) tx += bs;
-    if (Needs::kM1) tx += bs;
-    if (Needs::kM2) tx += bs;
+    if (kM1) tx += bs;
+    if (kM2) tx += bs;
     mbar_expect_tx32(bar, tx);
     if (has_x) bulk_g2s32(st + L.x, gstate + os, bs, bar);
     if (sep_xe) bulk_g2s32(st + L.xe, static_cast<const char*>(p.xe) + os, bs, bar);
     if (NE >= 1) bulk_g2s32(st + L.ec, static_cast<const char*>(p.ec) + om, bm, bar);
     if (NE == 2) bulk_g2s32(st + L.eu, static_cast<const char*>(p.eu) + om, bm, bar);
     if (NE == 0) bulk_g2s32(st + L.m0, static_cast<const char*>(p.m0) + os, bs, bar);
-    if (Needs::kM1) bulk_g2s32(st + L.m1, static_cast<const char*>(p.m1) + os, bs, bar);
-    if (Needs::kM2) bulk_g2s32(st + L.m2, static_cast<const char*>(p.m2) + os, bs, bar);
+    if (kM1) bulk_g2s32(st + L.m1, static_cast<const char*>(p.m1) + os, bs, bar);
+    if (kM2) bulk_g2s32(st + L.m2, static_cast<const char*>(p.m2) + os, bs, bar);
   };
 
   if (tid == 0) {
@@ -212,8 +176,8 @@ __global__ void __launch_bounds__(kTmaMaxThreads)
       if (lp < pk_here) {
         if (has_x) lds_pk32(rx[u], st + L.x + lp * kBS);
         if (sep_xe) lds_pk32(rxe[u], st + L.xe + lp * kBS);
-        if (Needs::kM1) lds_pk32(rm1[u], st + L.m1 + lp * kBS);
-        if (Needs::kM2) lds_pk32(rm2[u], st + L.m2 + lp * kBS);
+        if (kM1) lds_pk32(rm1[u], st + L.m1 + lp * kBS);
+        if (kM2) lds_pk32(rm2[u], st + L.m2 + lp * kBS);
         if (NE >= 1) lds_pk32(rec[u], st + L.ec + lp * kBM);
         if (NE == 2) lds_pk32(reu[u], st + L.eu + lp * kBM);
         if (NE == 0) lds_pk32(rm0[u], st + L.m0 + lp * kBS);
@@ -225,8 +189,8 @@ __global__ void __launch_bounds__(kTmaMaxThreads)
       if (lp < pk_here) {
         float fx[8], fT[8], fm1[8], fm2[8], fo[8];
         if (has_x) unpack(rx[u], fx);
-        if (Needs::kM1) unpack(rm1[u], fm1);
-        if (Needs::kM2) unpack(rm2[u], fm2);
+        if (kM1) unpack(rm1[u], fm1);
+        if (kM2) unpack(rm2[u], fm2);
         if (NE > 0) {
           float fec[8], feu[8];
           unpack(rec[u], fec);
@@ -274,55 +238,22 @@ __global__ void __launch_bounds__(kTmaMaxThreads)
 
 typedef void (*TmaKernel)(const KParams, const StageLayout, const int, const int);
 
-template <typename TE, typename TS, int NE>
-static TmaKernel tma_form(int form) {
-  switch (form) {
-    case DPM_FORM_NONE: return NE > 0 ? k_step_tma<TE, TS, NE, DPM_FORM_NONE> : nullptr;
-    case DPM_FORM_LIN1: return k_step_tma<TE, TS, NE, DPM_FORM_LIN1>;
-    case DPM_FORM_LIN2: return k_step_tma<TE, TS, NE, DPM_FORM_LIN2>;
-    case DPM_FORM_LIN3: return k_step_tma<TE, TS, NE, DPM_FORM_LIN3>;
-    case DPM_FORM_DIFF2: return k_step_tma<TE, TS, NE, DPM_FORM_DIFF2>;
-    case DPM_FORM_MS3: return k_step_tma<TE, TS, NE, DPM_FORM_MS3>;
-    case DPM_FORM_SS3T: return k_step_tma<TE, TS, NE, DPM_FORM_SS3T>;
-  }
-  return nullptr;
-}
-template <typename TE, typename TS>
-static TmaKernel tma_ne(int ne, int form) {
-  switch (ne) {
-    case 1: return tma_form<TE, TS, 1>(form);
-    case 2: return tma_form<TE, TS, 2>(form);
-  }
-  return nullptr;
-}
-static TmaKernel pick_tma(int md, int sd, int ne, int form) {
-  if (ne == 0) {
-    if (sd == DPM_F32) return tma_form<float, float, 0>(form);
-    if (sd == DPM_BF16) return tma_form<__nv_bfloat16, __nv_bfloat16, 0>(form);
-    if (sd == DPM_F16) return tma_form<__half, __half, 0>(form);
-    return nullptr;
-  }
-  if (md == DPM_F32 && sd == DPM_F32) return tma_ne<float, float>(ne, form);
-  if (md == DPM_BF16 && sd == DPM_BF16) return tma_ne<__nv_bfloat16, __nv_bfloat16>(ne, form);
-  if (md == DPM_F16 && sd == DPM_F16) return tma_ne<__half, __half>(ne, form);
-  if (md == DPM_BF16 && sd == DPM_F32) return tma_ne<__nv_bfloat16, float>(ne, form);
-  if (md == DPM_F16 && sd == DPM_F32) return tma_ne<__half, float>(ne, form);
-  return nullptr;
-}
-
 int launch_step_tma(const KParams& p, const Tuning& t, cudaStream_t stream) {
   if (!fast_path_ok(p) || p.thr != nullptr) return 1;   // other parameterisations, non-refinable divisors, per-sample
                                                         // thresholds: the direct variant
-  const bool need_x = p.form != DPM_FORM_NONE;
-  TmaKernel k = pick_tma(p.model_dtype, p.state_dtype, p.n_model, p.form);
+  TmaKernel k = pick_step<TmaKernel>(p, [](auto pair, auto ne, auto form) -> TmaKernel {
+    using Pair = decltype(pair);
+    return k_step_tma<typename Pair::TE, typename Pair::TS, decltype(ne)::value, decltype(form)::value>;
+  });
   if (k == nullptr) return 1;
+  const FormReads reads = form_reads(p.form);
+  const bool need_x = reads.x;
   const uint32_t ss = p.state_dtype == DPM_F32 ? 4 : 2, ms = p.model_dtype == DPM_F32 ? 4 : 2;
+  const bool has_x = need_x || (p.n_model > 0 && p.use_xe);   // state slot: x, or xe when no update
   const bool sep_xe = p.n_model > 0 && p.use_xe && need_x && !p.xe_is_x;
-  const bool m1 = p.form == DPM_FORM_LIN2 || p.form == DPM_FORM_LIN3 || p.form == DPM_FORM_DIFF2 ||
-                  p.form == DPM_FORM_MS3 || p.form == DPM_FORM_SS3T;
-  const bool m2 = p.form == DPM_FORM_LIN3 || p.form == DPM_FORM_MS3 || p.form == DPM_FORM_SS3T;
-  const int n_streams = (need_x || (p.n_model > 0 && p.use_xe)) + sep_xe + p.n_model + (p.n_model == 0) + m1 + m2 +
-                        (p.n_model > 0 && p.m_out != nullptr) + need_x;
+  const bool has_mo = p.n_model > 0 && p.m_out != nullptr;
+  // the shared-memory streams of a stage, one per take() below
+  const int n_streams = has_x + sep_xe + p.n_model + (p.n_model == 0) + reads.m1 + reads.m2 + has_mo + need_x;
   // Launch shape, decided inside the sampling loop on the first target GPU (not re-swept on H100): launches
   // with <= 4 shared-memory streams run best as 256 threads x 3 CTAs/SM, 5 streams as 256 x 2; when the tile is
   // also stored twice (out2: 6 HBM streams, the CFG steps of c3) one 512-thread CTA per SM with two 80 KB stages.
@@ -337,7 +268,7 @@ int launch_step_tma(const KParams& p, const Tuning& t, cudaStream_t stream) {
 
   StageLayout L;
   int threads = 0, stages = 0;
-  const int units = kTmaUnits;   // compile-time constant of the kernel
+  const int units = kUnits;   // compile-time constant of the kernel
   // tile = threads * units packets. Default 256 threads x 2 CTAs/SM (512 resident threads):
   // sweeps showed two stages at that size beat more, smaller stages; the tile only
   // shrinks when two stages of it do not fit.
@@ -346,14 +277,14 @@ int launch_step_tma(const KParams& p, const Tuning& t, cudaStream_t stream) {
     const uint32_t tile_el = (uint32_t)cand[c] * units * kPacket;
     uint32_t o = 0;
     auto take = [&](bool on, uint32_t es) { uint32_t r = 0xffffffffu; if (on) { r = o; o += tile_el * es; } return r; };
-    L.x = take(need_x || (p.n_model > 0 && p.use_xe), ss);
+    L.x = take(has_x, ss);
     L.xe = take(sep_xe, ss);
     L.ec = take(p.n_model >= 1, ms);
     L.eu = take(p.n_model == 2, ms);
     L.m0 = take(p.n_model == 0, ss);
-    L.m1 = take(m1, ss);
-    L.m2 = take(m2, ss);
-    L.mo = take(p.n_model > 0 && p.m_out != nullptr, ss);
+    L.m1 = take(reads.m1, ss);
+    L.m2 = take(reads.m2, ss);
+    L.mo = take(has_mo, ss);
     L.o = take(need_x, ss);
     L.bytes = o;
     int st = (int)((budget - 128) / L.bytes);
@@ -373,7 +304,7 @@ int launch_step_tma(const KParams& p, const Tuning& t, cudaStream_t stream) {
   int rc = ensure_max_smem(reinterpret_cast<const void*>(k));  // once per kernel and device
   if (rc != 0) return rc;
   cudaError_t le = launch_pdl(k, grid, (unsigned)threads, smem, stream, p, L, stages, units);
-  if (le != cudaSuccess) { set_error("TMA step launch failed: %s", cudaGetErrorString(le)); cudaGetLastError(); return (int)le; }
+  if (le != cudaSuccess) return launch_error("TMA step launch failed", le);
   count_launch();
   return 0;
 }
@@ -388,17 +319,17 @@ constexpr uint32_t kDupTileBytes = 32 * 1024;
 __global__ void __launch_bounds__(32) k_dup_tma(const char* __restrict__ src, char* __restrict__ dst0,
                                                 char* __restrict__ dst1, const uint64_t bytes) {
   extern __shared__ __align__(128) unsigned char smem[];
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem);
-  unsigned char* ring = smem + 128;
+  const uint32_t full = smem_u32(smem);   // [kDupStages] mbarriers
+  const uint32_t ring = full + 128;
   const uint64_t ntiles = (bytes + kDupTileBytes - 1) / kDupTileBytes;
   if (threadIdx.x != 0) return;     // one elected thread drives the copy engine; the warp exists for the launch only
-  for (int s = 0; s < kDupStages; ++s) mbar_init(&full[s], 1);
+  for (int s = 0; s < kDupStages; ++s) mbar_init(reinterpret_cast<uint64_t*>(smem) + s, 1);
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   auto load = [&](uint64_t tile, int s) {
     const uint64_t b0 = tile * kDupTileBytes;
     const uint32_t nb = (uint32_t)((bytes - b0) < kDupTileBytes ? (bytes - b0) : kDupTileBytes);
-    mbar_expect_tx(&full[s], nb);
-    bulk_g2s(ring + (size_t)s * kDupTileBytes, src + b0, nb, &full[s]);
+    mbar_expect_tx32(full + s * 8, nb);
+    bulk_g2s32(ring + s * kDupTileBytes, src + b0, nb, full + s * 8);
   };
   for (int s = 0; s < kDupStages; ++s) {
     const uint64_t tile = (uint64_t)blockIdx.x + (uint64_t)s * gridDim.x;
@@ -407,11 +338,11 @@ __global__ void __launch_bounds__(32) k_dup_tma(const char* __restrict__ src, ch
   uint32_t it = 0;
   for (uint64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
     const int s = it % kDupStages;
-    mbar_wait(&full[s], (it / kDupStages) & 1u);
+    mbar_wait32(full + s * 8, (it / kDupStages) & 1u);
     const uint64_t b0 = tile * kDupTileBytes;
     const uint32_t nb = (uint32_t)((bytes - b0) < kDupTileBytes ? (bytes - b0) : kDupTileBytes);
-    bulk_s2g(dst0 + b0, ring + (size_t)s * kDupTileBytes, nb);
-    bulk_s2g(dst1 + b0, ring + (size_t)s * kDupTileBytes, nb);
+    bulk_s2g32(dst0 + b0, ring + s * kDupTileBytes, nb);
+    bulk_s2g32(dst1 + b0, ring + s * kDupTileBytes, nb);
     bulk_commit();
     const uint64_t next = tile + (uint64_t)kDupStages * gridDim.x;
     if (next < ntiles) {

@@ -218,8 +218,9 @@ class DPM_Solver:
         reproduce the two places where the reference computes in the network's 16-bit output type -- the
         CFG combine (:329-330, three rounded ops) and, for the eps-solver, the differences of the
         buffered raw outputs (:823, :880-881, :636, :735, :741-742). Default False: both are evaluated in
-        fp32 on the widened values (closer to the exact result, and the fast kernels). Runs on the generic
-        kernel for now.
+        fp32 on the widened values (closer to the exact result, and the fast kernels). Runs on the
+        reference-rounding instantiations of the direct vector kernels (tails and unaligned views on the
+        generic kernel).
 
         predict_x0 / thresholding / max_val: keyword spelling of the older constructor that the JAX twin
         still uses (dpm_solver_jax.py:351): predict_x0=True selects "dpmsolver++", thresholding=True

@@ -119,7 +119,8 @@ typedef struct dpm_step_desc {
                           the CFG combine :329-330 then rounds to it after each of its three ops, as the
                           reference's eager 16-bit ops do; bit 2 (+4) = the buffered values are such raw
                           outputs, so their differences (:823, :880-881, :636, :735, :741-742) are rounded
-                          to that type before the fp32 coefficients widen them. Generic kernel only.   */
+                          to that type before the fp32 coefficients widen them. Served by the vector
+                          kernels for bf16 / f16 network outputs, else by the generic kernel.          */
   float guidance;      /* CFG scale s: eps = eps_u + s*(eps_c - eps_u) :330                */
   float alpha_e;       /* alpha, sigma at the model evaluation time                         */
   float sigma_e;
