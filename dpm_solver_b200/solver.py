@@ -938,9 +938,13 @@ class DPM_Solver:
         if noise is None:
             noise = torch.randn((th.shape[0], *x.shape), device=x.device)
         # result dtype: the reference's fp32 (t_size,1,..) coefficient tensors promote a 16-bit x to fp32 (:1026)
-        xs = self._state_like(x, self._sdtype(x))
+        sd = self._sdtype(x)
+        # with a 16-bit state, fp32 noise stays fp32: alpha*x + sigma*noise is rounded to the state dtype once, as the
+        # in-kernel noise path does (rounding the noise to the state dtype first would round twice)
+        wd = torch.float32 if noise.dtype == torch.float32 else sd
+        xs = self._state_like(x, wd)
         noise = noise.reshape((th.shape[0], *x.shape))
-        outs = [ops.lincomb(xs, [self._state_like(noise[i], xs.dtype)], float(alpha_t[i]), [float(sigma_t[i])])
+        outs = [ops.lincomb(xs, [self._state_like(noise[i], wd)], float(alpha_t[i]), [float(sigma_t[i])]).to(sd)
                 for i in range(th.shape[0])]
         if th.shape[0] == 1:
             return outs[0]

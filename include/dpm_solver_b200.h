@@ -207,8 +207,12 @@ DPM_API int dpm_data_prediction(void* x0, const void* x, const void* eps, float 
                         dpm_stream_t stream);
 
 /* ---- noise drawn inside the kernel (torch.randn-compatible Philox) ------------------------------------------
- * ATen's launch policy for a randn of `numel` elements on the current device: the virtual grid the kernels below
- * replay, and the amount the caller must advance the torch CUDA generator's philox offset by afterwards. */
+ * ATen's launch policy for an fp32 randn of `numel` elements on the current device.
+ *   grid: the grid of one launch over all `numel` elements (calc_execution_policy).
+ *   counter_offset: the TOTAL amount the caller must advance the torch CUDA generator's philox offset by afterwards.
+ *     Up to 2^29 elements that is the one launch's counter offset. Above, ATen splits the tensor into pieces that
+ *     fit 32-bit indexing and draws each with its own grid and philox state, so the total is the whole tensor's
+ *     counter offset plus each piece's; the kernels below replay the same pieces. */
 DPM_API int dpm_philox_policy(uint64_t numel, uint32_t* grid, uint64_t* counter_offset);
 
 /* DPM_Solver.add_noise(x, t, noise=None) :1012-1030 with the noise generated in registers:

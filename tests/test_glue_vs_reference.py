@@ -94,6 +94,22 @@ def test_add_noise_golden_and_reference(dev, golden):
         np.testing.assert_array_equal(have.float().cpu().numpy(), want.float().numpy())
 
 
+@pytest.mark.parametrize("sdt", [torch.bfloat16, torch.float16])
+@pytest.mark.parametrize("xdt", [torch.float32, "state"])
+def test_add_noise_16bit_state_rounds_once(dev, sdt, xdt):
+    """A 16-bit state with fp32 noise: the reference's fp32 result rounded once to the state dtype, not a sum of
+    noise already rounded to 16 bits."""
+    import dpm_solver_b200 as new
+    ref = ref_loader.load("dpm_solver_pytorch")
+    x = seeded((2, 4, 8, 8), 3).to(sdt if xdt == "state" else xdt)
+    nz = seeded((2, 2, 4, 8, 8), 4)
+    t = torch.tensor([0.3, 0.8])
+    want = ref.DPM_Solver(None, _sched(ref, "sd")).add_noise(x, t, noise=nz).to(sdt)
+    have = new.DPM_Solver(None, _sched(new, "sd"), state_dtype=sdt).add_noise(x.to(dev), t.to(dev), noise=nz.to(dev))
+    assert have.dtype == sdt and have.shape == want.shape
+    np.testing.assert_array_equal(have.float().cpu().numpy(), want.float().numpy())
+
+
 # ---- 'cosine' schedule of the older vendored copies -----------------------------------------------------
 def test_cosine_schedule_scalars_match_vendored_copy():
     """NoiseScheduleVP('cosine') (examples/stable-diffusion/.../dpm_solver.py:114-175): every marginal and the inverse."""
