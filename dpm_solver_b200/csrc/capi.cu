@@ -206,13 +206,26 @@ static int finish(int rc) {
   return e != cudaSuccess ? launch_error("CUDA launch failed", e) : DPM_OK;
 }
 
-static int step_impl(const dpm_step_desc* d, cudaStream_t stream) {
+// rs (optional): guidance rescale of an n_model == 2 step -- ratio [n/per_sample] and the weights phi, psi
+struct Rescale {
+  const float* ratio;
+  float phi, psi;
+};
+
+static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale* rs = nullptr) {
   KParams p;
   Needs nd;
   if (d != nullptr && d->n == 0) return DPM_OK;  // empty tensors: nothing to do (pointers may be NULL)
   int rc = build_params(d, &p, &nd, false);
   if (rc != DPM_OK) return rc;
   if (p.n == 0) return DPM_OK;
+  if (rs != nullptr) {
+    if (rs->ratio == nullptr || d->n_model != 2 || d->raw_round != 0 || d->per_sample == 0 || d->n % d->per_sample) {
+      set_error("rescaled step: needs ratio, n_model == 2, raw_round == 0 and per_sample dividing n");
+      return DPM_ERR_ARG;
+    }
+    p.ratio = rs->ratio; p.phi = rs->phi; p.psi = rs->psi;
+  }
   Tuning t{g_variant.load(), g_threads.load(), g_ctas.load()};
 
   bool body_done = false;
@@ -222,6 +235,7 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream) {
     // fp32 state: direct vector loads already sit near the HBM roofline (fewer instructions per
     // byte); 16-bit state is issue-limited there and gains from the ring (measured on the first target GPU)
     const bool tma = p.raw_round == 0 &&   // reference-rounding mode: the direct variant's <RND> kernels
+                     p.ratio == nullptr &&  // guidance rescale: the direct variant's <RS> kernels
                      (t.variant == 1 || (t.variant == 2 && p.state_dtype != DPM_F32 &&
                                          p.npk >= (uint32_t)sm_count() * 1024u));
     if (tma) r = launch_step_tma(p, t, stream);
@@ -263,6 +277,26 @@ int dpm_get_tuning(int* variant, int* threads, int* ctas_per_sm) {
 
 int dpm_step(const dpm_step_desc* desc, dpm_stream_t stream) {
   return step_impl(desc, static_cast<cudaStream_t>(stream));
+}
+
+int dpm_step_rescaled(const dpm_step_desc* desc, const float* ratio, float phi, float one_minus_phi,
+                      dpm_stream_t stream) {
+  const Rescale rs{ratio, phi, one_minus_phi};
+  return step_impl(desc, static_cast<cudaStream_t>(stream), &rs);
+}
+
+size_t dpm_cfg_rescale_workspace(uint64_t n_samples, uint64_t per_sample) {
+  return cfg_rescale_workspace_bytes(n_samples, per_sample);
+}
+
+int dpm_cfg_rescale_ratio(float* ratio_out, const void* e_cond, const void* e_uncond, float guidance,
+                          uint64_t per_sample, uint64_t n, int model_dtype, void* workspace, size_t workspace_bytes,
+                          dpm_stream_t stream) {
+  if (n == 0) return DPM_OK;
+  if (!ratio_out || !e_cond || !e_uncond) { set_error("cfg rescale: NULL tensor"); return DPM_ERR_ARG; }
+  if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) { set_error("cfg rescale: bad dtype or sizes"); return DPM_ERR_ARG; }
+  return finish(launch_cfg_rescale_ratio(ratio_out, e_cond, e_uncond, guidance, per_sample, n, model_dtype, workspace,
+                                         workspace_bytes, static_cast<cudaStream_t>(stream)));
 }
 
 static dpm_step_desc base_desc(void* out, const void* x, uint64_t n, int dtype, int form) {

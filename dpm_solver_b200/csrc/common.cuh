@@ -57,6 +57,10 @@ struct KParams {
   float r_w4;
   int32_t fast_div;
   const float* dev_coef;   // optional: scalars read from device memory (dpm_step_desc.dev_coef); generic kernel only
+  // guidance rescale (dpm_step_rescaled): per-sample ratio std(out_c)/std(g), fp32 [n/per_sample], and the two
+  // host-rounded weights phi, psi = fl32(1 - phi). Only the <RS = true> instantiations read them.
+  const float* ratio;
+  float phi, psi;
 };
 
 // ---- storage types ------------------------------------------------------------------------
@@ -271,11 +275,24 @@ __device__ __forceinline__ float convert_param(int param, float out, float xe, f
 // raw network output(s) -> buffered model value (eps, or x0 for dpmsolver++)
 // RND: reference-rounding mode. A network that returns 16-bit noise makes the reference evaluate the
 // CFG combine in that type (python-float scale, :329-330): three ops, each rounded to 16 bits.
-template <int NE, bool RND = false>
+// guidance rescale (Lin et al. 2023; diffusers' rescale_noise_cfg), in the network's output space:
+// g' = phi*(g*r) + psi*g, r = std(out_c)/std(g) of the sample, each op rounded
+__device__ __forceinline__ float rescale_value(const KParams& p, float g, float r) {
+  return p.phi * (g * r) + p.psi * g;
+}
+
+// RS: guidance rescale (NE == 2). The combine then runs on the raw outputs, the rescale follows, and the
+// parameterisation converts the rescaled prediction -- the order of a rescaling network wrapped by :288-298.
+template <int NE, bool RND = false, bool RS = false>
 __device__ __forceinline__ float model_value(const KParams& p, float xe, float ec, float eu,
-                                             float thr, bool clamp) {
-  float eps = convert_param(p.param, ec, xe, p.alpha_e, p.sigma_e);
-  if (NE == 2) {
+                                             float thr, bool clamp, float r = 1.f) {
+  float eps;
+  if (RS) {
+    eps = convert_param(p.param, rescale_value(p, eu + p.guidance * (ec - eu), r), xe, p.alpha_e, p.sigma_e);
+  } else {
+    eps = convert_param(p.param, ec, xe, p.alpha_e, p.sigma_e);
+  }
+  if (NE == 2 && !RS) {
     float epu = convert_param(p.param, eu, xe, p.alpha_e, p.sigma_e);
     if (RND && p.param == DPM_PARAM_NOISE) {
       const int dt = p.raw_round & 3;
@@ -352,11 +369,17 @@ __device__ __forceinline__ float update_value(const KParams& p, float x, float T
 // Launch-uniform switches are taken once per PACKET (uniform branches), every loop below is
 // straight-line code over 8 elements. Callers guarantee: p.param == NOISE; p.fast_div when a division
 // is needed; a clamp threshold `s` that is uniform over the packet.
-template <int NE>
+// RS: guidance rescale with the sample's ratio r (uniform over the packet, like s).
+template <int NE, bool RS = false>
 __device__ __forceinline__ void fast_model8(const KParams& p, const float (&xe)[8], const float (&ec)[8],
-                                            const float (&eu)[8], bool clamp, float s, float (&T)[8]) {
+                                            const float (&eu)[8], bool clamp, float s, float (&T)[8],
+                                            float r = 1.f) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) T[i] = (NE == 2) ? eu[i] + p.guidance * (ec[i] - eu[i]) : ec[i];  // :330
+  if (RS) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) T[i] = rescale_value(p, T[i], r);
+  }
   if (!p.predict_x0) return;
 #pragma unroll
   for (int i = 0; i < 8; ++i) T[i] = xe[i] - p.sigma_e * T[i];
@@ -410,7 +433,7 @@ __host__ __forceinline__ bool fast_path_ok(const KParams& p) {
   if (p.n_model == 0) return true;
   if (p.param != DPM_PARAM_NOISE) return false;
   if (p.predict_x0 && !p.fast_div) return false;
-  if (p.thr != nullptr && p.pk_per_sample == 0) return false;
+  if ((p.thr != nullptr || p.ratio != nullptr) && p.pk_per_sample == 0) return false;
   return true;
 }
 

@@ -121,5 +121,8 @@ size_t quantile_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
 size_t adaptive_workspace_bytes(uint64_t n, uint64_t per_sample);
 int launch_adaptive_error(float* out, const void* xh, const void* xl, const void* xp, float atol, float rtol,
                           uint64_t per_sample, uint64_t n, int dtype, void* ws, size_t ws_bytes, cudaStream_t stream);
+size_t cfg_rescale_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
+int launch_cfg_rescale_ratio(float* ratio, const void* ec, const void* eu, float guidance, uint64_t per_sample,
+                             uint64_t n, int dtype, void* ws, size_t ws_bytes, cudaStream_t stream);
 
 }  // namespace dpm

@@ -16,7 +16,9 @@ constexpr int kMaxThreads = 512;
 // RND (only with FAST = false): reference-rounding mode (dpm_step_desc.raw_round) on the vector path -- the 16-bit
 // CFG combine (three rounded ops) and the rounded differences of raw 16-bit buffers, per element, between 128/256-bit
 // loads and stores.
-template <typename TE, typename TS, int NE, int FORM, bool FAST, bool RND = false>
+// RS (only with NE == 2 and RND = false): guidance rescale (dpm_step_rescaled) with the per-sample ratio p.ratio, read
+// like the per-sample thresholds.
+template <typename TE, typename TS, int NE, int FORM, bool FAST, bool RND = false, bool RS = false>
 __global__ void __launch_bounds__(kMaxThreads)
     k_step_direct(const __grid_constant__ KParams p) {
   constexpr bool kX = form_reads(FORM).x, kM1 = form_reads(FORM).m1, kM2 = form_reads(FORM).m2;
@@ -75,11 +77,12 @@ __global__ void __launch_bounds__(kMaxThreads)
           unpack(rec[u], fec);
           if (NE == 2) unpack(reu[u], feu);
           const float s_thr = clamp ? __ldg(p.thr + (uint32_t)pk / p.pk_per_sample) : 1.f;   // packet index < 2^32 (npk)
+          const float r = RS ? __ldg(p.ratio + (uint32_t)pk / p.pk_per_sample) : 1.f;
           if (sep_xe) {
             unpack(rxe[u], fxe);
-            fast_model8<NE>(p, fxe, fec, feu, clamp, s_thr, fT);
+            fast_model8<NE, RS>(p, fxe, fec, feu, clamp, s_thr, fT, r);
           } else {
-            fast_model8<NE>(p, fx, fec, feu, clamp, s_thr, fT);   // fx is only read when predict_x0 (then it is loaded)
+            fast_model8<NE, RS>(p, fx, fec, feu, clamp, s_thr, fT, r);   // fx is only read when predict_x0 (then it is loaded)
           }
           Raw<TS> rmo;
           round_pack(rmo, fT);
@@ -112,9 +115,22 @@ __global__ void __launch_bounds__(kMaxThreads)
 #pragma unroll
             for (int i = 0; i < 8; ++i) thr8[i] = 1.f;
           }
+          float r8[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) r8[i] = 1.f;
+          if (RS) {
+            if (thr_uniform) {
+              const float rpk = __ldg(p.ratio + (uint32_t)(pk / p.pk_per_sample));
+#pragma unroll
+              for (int i = 0; i < 8; ++i) r8[i] = rpk;
+            } else {
+#pragma unroll
+              for (int i = 0; i < 8; ++i) r8[i] = __ldg(p.ratio + (e + i) / p.per_sample);
+            }
+          }
 #pragma unroll
           for (int i = 0; i < 8; ++i)
-            fT[i] = model_value<NE, RND>(p, fxe[i], fec[i], NE == 2 ? feu[i] : 0.f, thr8[i], clamp);
+            fT[i] = model_value<NE, RND, RS>(p, fxe[i], fec[i], NE == 2 ? feu[i] : 0.f, thr8[i], clamp, r8[i]);
           Raw<TS> rmo;
           round_pack(rmo, fT);
           if (gmo != nullptr) stg_pk(gmo + e, rmo);
@@ -143,7 +159,8 @@ __global__ void __launch_bounds__(kMaxThreads)
 // ---- fully generic element-wise kernel: any dtype mix, any alignment, tails ------------------
 // RND = true: reference-rounding mode (common.cuh) for the launches the <RND> vector kernels do not serve:
 // unaligned views, tails and fp32 network outputs.
-template <bool RND>
+// RS = true: guidance rescale (n_model == 2) for unaligned views, tails and dev_coef launches.
+template <bool RND, bool RS = false>
 __global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KParams pc) {
   KParams p = pc;
   if (pc.dev_coef != nullptr) {
@@ -169,8 +186,13 @@ __global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KPa
       float ec = load_any(p.ec, md, i);
       float eu = p.n_model == 2 ? load_any(p.eu, md, i) : 0.f;
       float thr = clamp ? p.thr[(i + p.elem_offset) / p.per_sample] : 1.f;
-      float mv = p.n_model == 2 ? model_value<2, RND>(p, xe, ec, eu, thr, clamp)
-                                : model_value<1, RND>(p, xe, ec, eu, thr, clamp);
+      float mv;
+      if (RS) {
+        mv = model_value<2, false, true>(p, xe, ec, eu, thr, clamp, p.ratio[(i + p.elem_offset) / p.per_sample]);
+      } else {
+        mv = p.n_model == 2 ? model_value<2, RND>(p, xe, ec, eu, thr, clamp)
+                            : model_value<1, RND>(p, xe, ec, eu, thr, clamp);
+      }
       T0 = round_any(sd, mv);
       if (p.m_out) store_any(p.m_out, sd, i, mv);
     } else {
@@ -197,12 +219,19 @@ typedef void (*StepKernel)(const KParams);
 // FAST: NE == 0 has no model conversion, so there only SS3T (division by w4) has a <FAST = false> twin.
 // RND: an fp32 state with raw network outputs in bf16 / f16 (NE >= 1), or fp32 buffers holding such raw outputs
 // (NE == 0, differences rounded).
+// RS: guidance rescale, NE == 2 only (the C-ABI rejects it together with raw_round).
 static StepKernel pick_direct(const KParams& p) {
-  const bool fast = fast_path_ok(p), rnd = p.raw_round != 0;
+  const bool fast = fast_path_ok(p), rnd = p.raw_round != 0, rs = p.ratio != nullptr;
   return pick_step<StepKernel>(p, [&](auto pair, auto ne, auto form) -> StepKernel {
     using TE = typename decltype(pair)::TE;
     using TS = typename decltype(pair)::TS;
     constexpr int NE = decltype(ne)::value, FORM = decltype(form)::value;
+    if (rs) {
+      if constexpr (NE == 2)
+        return fast ? k_step_direct<TE, TS, 2, FORM, true, false, true> : k_step_direct<TE, TS, 2, FORM, false, false, true>;
+      else
+        return nullptr;
+    }
     if (rnd) {
       if constexpr (std::is_same_v<TS, float> && (NE == 0) == std::is_same_v<TE, float>)
         return k_step_direct<TE, TS, NE, FORM, false, true>;
@@ -238,6 +267,7 @@ int launch_step_scalar(const KParams& p, cudaStream_t stream) {
   uint64_t cap = (uint64_t)sm_count() * 8;
   uint32_t grid = (uint32_t)(blocks < cap ? blocks : cap);
   if (p.raw_round) k_step_scalar<true><<<grid, threads, 0, stream>>>(p);
+  else if (p.ratio) k_step_scalar<false, true><<<grid, threads, 0, stream>>>(p);
   else k_step_scalar<false><<<grid, threads, 0, stream>>>(p);
   count_launch();
   return 0;

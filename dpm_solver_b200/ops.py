@@ -57,6 +57,9 @@ class StepArgs:
     m_out: Optional[torch.Tensor] = None
     raw_round: int = 0                # reference-rounding mode (dpm_step_desc.raw_round); 0 = off
     coef_dev: Optional[torch.Tensor] = None   # 16 fp32 on the device: the launch reads its scalars there (dev_coef)
+    # guidance rescale (dpm_step_rescaled; n_model == 2, per_sample set): fp32 [B] from cfg_rescale_ratio, and phi
+    ratio: Optional[torch.Tensor] = None
+    phi: float = 0.0
 
     def state_tensors(self):
         return [t for t in (self.x, self.xe, self.m0, self.m1, self.m2) if t is not None]
@@ -201,8 +204,38 @@ class CudaBackend:
                 if self._layout(a.out2) != layout:      # dense, laid out like `out` (a channels_last half of the
                     raise ValueError("dpm_solver_b200: out2 must be dense and laid out like out")   # doubled CFG batch is)
                 d.out2 = a.out2.data_ptr()
-        self._launch(ref.device, self._lib.dpm_step, C.byref(d))
+        if a.ratio is not None:
+            r = a.ratio
+            if not r.is_cuda or r.dtype != torch.float32 or not r.is_contiguous() or r.device != ref.device:
+                raise TypeError("dpm_solver_b200: `ratio` must be a contiguous fp32 tensor on the tensors' device")
+            if a.per_sample <= 0 or ref.numel() % a.per_sample or r.numel() != ref.numel() // a.per_sample:
+                raise ValueError("dpm_solver_b200: `ratio` needs one value per sample")
+            # phi and 1 - phi (formed in double, as the python-float expression does), each rounded to fp32 once
+            self._launch(ref.device, self._lib.dpm_step_rescaled, C.byref(d), C.c_void_p(r.data_ptr()),
+                         C.c_float(a.phi), C.c_float(1.0 - a.phi))
+        else:
+            self._launch(ref.device, self._lib.dpm_step, C.byref(d))
         return m_out, out
+
+    def cfg_rescale_ratio(self, e_cond: torch.Tensor, e_uncond: torch.Tensor, guidance: float) -> torch.Tensor:
+        """Per-sample r = std(e_cond_b) / std(g_b), g = e_uncond + guidance*(e_cond - e_uncond), as fp32 [B] on the
+        device (dpm_cfg_rescale_ratio). Both halves keep a shared dense layout: a sample is one contiguous block
+        in row-major and in channels_last storage alike."""
+        n, dev = e_cond.numel(), e_cond.device
+        layout = self._layout(e_cond)
+        if layout is None or self._layout(e_uncond) != layout:
+            layout = "c"
+        ec = self._check(e_cond, "e_cond", dev, n, layout=layout)
+        eu = self._check(e_uncond, "e_uncond", dev, n, e_cond.dtype, layout)
+        nb = e_cond.shape[0]
+        per_sample = n // nb
+        r = torch.empty(nb, dtype=torch.float32, device=dev)
+        ws_bytes = int(self._lib.dpm_cfg_rescale_workspace(nb, per_sample))
+        ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev)
+        self._launch(dev, self._lib.dpm_cfg_rescale_ratio, C.c_void_p(r.data_ptr()), C.c_void_p(ec.data_ptr()),
+                     C.c_void_p(eu.data_ptr()), C.c_float(guidance), C.c_uint64(per_sample), C.c_uint64(n),
+                     C.c_int(_DTYPE_CODE[e_cond.dtype]), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
+        return r
 
     def _launch(self, device, fn, *args):
         """Call a C-ABI entry on torch's current stream of `device` (device guard only if needed)."""
@@ -413,8 +446,8 @@ class PreparedStep:
 
     @staticmethod
     def build(be: "CudaBackend", a: StepArgs) -> Optional["PreparedStep"]:
-        if a.thr is not None or a.raw_round or a.out is not None and a.out2 is None:
-            return None
+        if a.thr is not None or a.raw_round or a.ratio is not None or a.out is not None and a.out2 is None:
+            return None     # (a rescaled step reads a fresh ratio tensor every evaluation: never frozen)
         ref = a.reference_tensor()
         if not ref.is_contiguous():
             return None

@@ -19,6 +19,7 @@ from __future__ import annotations
 
 import dataclasses
 import inspect
+import math
 from dataclasses import dataclass
 from typing import List, Optional
 
@@ -45,6 +46,25 @@ class RawOutput:
     e_uncond: Optional[torch.Tensor]
     param: int
     guidance: float
+    phi: float = 0.0        # guidance rescale of the combine (model_wrapper's guidance_rescale); 0 = off
+
+
+def _cfg_ratio(be, raw: RawOutput) -> Optional[torch.Tensor]:
+    """Per-sample ratio std(out_c)/std(g) of a rescaled CFG evaluation (device fp32 [B]); None without rescale."""
+    if raw.phi == 0 or raw.e_uncond is None:
+        return None
+    fn = getattr(be, "cfg_rescale_ratio", None)
+    if fn is None:
+        raise RuntimeError("guidance_rescale needs an executor with cfg_rescale_ratio; {} has none".format(
+            getattr(be, "name", type(be).__name__)))
+    return fn(raw.e_cond, raw.e_uncond, raw.guidance)
+
+
+def _rescale_args(a: StepArgs, ratio: Optional[torch.Tensor], raw: RawOutput) -> StepArgs:
+    if ratio is not None:
+        a.ratio, a.phi = ratio, raw.phi
+        a.per_sample = a.e_cond.numel() // a.e_cond.shape[0]
+    return a
 
 
 class WrappedModel:
@@ -55,8 +75,9 @@ class WrappedModel:
     """
 
     def __init__(self, model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
-                 unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs):
+                 unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale=0.):
         self.model = model
+        self.guidance_rescale = guidance_rescale
         self.noise_schedule = noise_schedule
         self.model_type = model_type
         self.model_kwargs = model_kwargs
@@ -120,7 +141,7 @@ class WrappedModel:
                 x_in = ops.backend().duplicate(x)              # cat([x] * 2) :326 (the solver hands over a prebuilt one)
             t_in = None if t_input is not None else torch.cat([t_continuous] * 2)
             out_u, out_c = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(2)  # uncond first
-            return RawOutput(out_c, out_u, param, float(self.guidance_scale))
+            return RawOutput(out_c, out_u, param, float(self.guidance_scale), self.guidance_rescale)
         raise RuntimeError("raw() is not available with classifier guidance")
 
     def _alpha_sigma(self, t_continuous):
@@ -171,11 +192,13 @@ class WrappedModel:
         pairs = self._alpha_sigma(t_continuous) if r.param != PARAM_NOISE else [(1.0, 0.0)]
         needs_x = r.param in (PARAM_BY_NAME["x_start"], PARAM_BY_NAME["v"])
         xo = x.to(r.e_cond.dtype) if needs_x else None
+        ratio = _cfg_ratio(be, r)      # over the whole batch: each sample's ratio reads its own values only
 
         def convert(rows, alpha, sigma):
             a = StepArgs(form=FORM_NONE, n_model=2 if r.e_uncond is not None else 1, e_cond=r.e_cond[rows],
                          e_uncond=None if r.e_uncond is None else r.e_uncond[rows], param=r.param,
                          guidance=r.guidance, alpha_e=alpha, sigma_e=sigma, state_dtype=r.e_cond.dtype)
+            _rescale_args(a, None if ratio is None else ratio[rows], r)
             if needs_x:
                 a.xe = xo[rows]
             return be.step(a)[0]
@@ -184,14 +207,25 @@ class WrappedModel:
 
 def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, guidance_type="uncond",
                   condition=None, unconditional_condition=None, guidance_scale=1., classifier_fn=None,
-                  classifier_kwargs={}):
+                  classifier_kwargs={}, guidance_rescale=0.):
     """Wrap a network into `model_fn(x, t_continuous) -> noise`; same contract as the reference
     (:170-334): model_type in {noise, x_start, v, score}, guidance_type in {uncond, classifier,
-    classifier-free}."""
+    classifier-free}.
+
+    guidance_rescale=phi (classifier-free guidance only; not in the reference): guidance rescale of Lin et al.
+    2023 as diffusers' `rescale_noise_cfg` does it, in the network's output space (eps for a noise network, v for
+    a v network): g = out_u + s*(out_c - out_u), r_b = std(out_c_b)/std(g_b) per sample (unbiased),
+    g' = phi*(g*r_b) + (1 - phi)*g, then the parameterisation converts g'. It applies only when the combine
+    runs (scale != 1 and an unconditional condition); 0 (default) is plain CFG."""
     assert model_type in ["noise", "x_start", "v", "score"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
+    guidance_rescale = float(guidance_rescale)
+    if not math.isfinite(guidance_rescale):
+        raise ValueError("guidance_rescale must be finite, got {}".format(guidance_rescale))
+    if guidance_rescale != 0 and guidance_type != "classifier-free":
+        raise ValueError("guidance_rescale needs guidance_type='classifier-free', got '{}'".format(guidance_type))
     return WrappedModel(model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
-                        unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs)
+                        unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale)
 
 
 # =================================================================================================
@@ -256,6 +290,8 @@ class DPM_Solver:
         self.state_dtype = state_dtype
         self.plan_broadcast = bool(plan_broadcast)
         self.reference_rounding = bool(reference_rounding)
+        if self.reference_rounding and getattr(model_fn, "guidance_rescale", 0) != 0:
+            raise ValueError("guidance_rescale is not available with reference_rounding=True")
         self._rr_run = 0     # raw_round of the buffered values of the run in flight (reference_rounding)
         self._prep_cache = {}   # frozen launch descriptors of cached plan steps (ops.PreparedStep)
         self._prep_on = False
@@ -497,7 +533,8 @@ class DPM_Solver:
         be = ops.backend()
         pkey = None
         if slot is not None and self._prep_on:
-            pkey = (slot, raw.param, raw.guidance, raw.e_uncond is None, raw.e_cond.dtype, xe.dtype, xe.shape,
+            # (phi is part of the key: a rescaled evaluation is never served by a launch frozen without the rescale)
+            pkey = (slot, raw.param, raw.guidance, raw.phi, raw.e_uncond is None, raw.e_cond.dtype, xe.dtype, xe.shape,
                     want_m, dup_out)
             prep = self._prep_cache.get(pkey)
             if prep is not None:
@@ -514,6 +551,7 @@ class DPM_Solver:
         custom_fix = x0 and self.correcting_x0_fn is not None and not self._dynamic_thresholding
         code = self._rr_code(raw)
         rr = 0
+        ratio = _cfg_ratio(be, raw)     # guidance rescale: one streaming pass over both halves (+2 launches)
         if code:
             # reference-rounding mode (raw 16-bit NOISE outputs, fp32 state): bits 0-1 make the fused kernel take the
             # CFG combine in the network's type, three rounded ops (:329-330); for the eps-solver the buffered values
@@ -521,14 +559,16 @@ class DPM_Solver:
             rr = code
             if not x0:
                 rr = self._rr_run = code | 4
-            if raw.e_uncond is not None and x0 and self._dynamic_thresholding:
-                # the quantile kernels take the combine in fp32: give them (and the step) the reference's rounded
-                # noise, materialised once (values exactly representable in the network's type, held in fp32)
-                e = be.step(StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond,
-                                     param=PARAM_NOISE, guidance=raw.guidance, state_dtype=torch.float32,
-                                     raw_round=code))[0]
-                raw = RawOutput(e, None, PARAM_NOISE, 1.0)
-                rr = 0
+        if raw.e_uncond is not None and x0 and self._dynamic_thresholding and (code or ratio is not None):
+            # the quantile kernels take the plain fp32 combine: give them (and the step) the reference's rounded noise,
+            # or the rescaled network output, materialised once in fp32 and then treated as one network output (the
+            # parameterisation, which the quantile and the step apply, still converts it)
+            a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
+                         guidance=raw.guidance, state_dtype=torch.float32, raw_round=code)
+            e = be.step(_rescale_args(a, ratio, raw))[0]
+            raw = RawOutput(e, None, raw.param, 1.0)
+            rr = 0
+            ratio = None
         if (rr & 4) and co is not None:
             co = self._rr_coeffs(co, code)
         if not self._needs_conversion(raw, sd, x0):
@@ -536,7 +576,7 @@ class DPM_Solver:
             x_next = self._pure_update(co, x, m_new, m1, m2, rr=rr & 4 and rr, pkey=pkey if m_new is raw.e_cond else None) \
                 if co is not None else None
             return m_new, x_next
-        a = self._conv_args(raw, xe, alsig, sd, x0)
+        a = _rescale_args(self._conv_args(raw, xe, alsig, sd, x0), ratio, raw)
         if alsig is _DEV:
             if co is None or co.dev is None:
                 raise RuntimeError("device-side scalars need the coefficient block of the consuming launch")

@@ -256,6 +256,30 @@ DPM_API int dpm_adaptive_error(float* e_out, const void* x_higher, const void* x
                                uint64_t n, int dtype, void* workspace, size_t workspace_bytes,
                                dpm_stream_t stream);
 
+/* ---- guidance rescale (Lin et al. 2023, "Common Diffusion Noise Schedules and Sample Steps are Flawed") ------
+ * Classifier-free guidance with the guided prediction rescaled toward the standard deviation of the conditional one,
+ * in the network's output space (eps for a noise network, v for a v network):
+ *   g  = e_uncond + guidance*(e_cond - e_uncond)                       (:330, on the raw outputs)
+ *   r_b = fl32(std(e_cond_b)) / fl32(std(g_b))                          (per sample, unbiased, fp64 accumulation)
+ *   g' = phi*(g*r_b) + one_minus_phi*g                                  (each op rounded to fp32)
+ * then g' takes the place of the combined output in dpm_step (parameterisation :288-298, eps->x0, clamp, update).
+ *
+ * dpm_cfg_rescale_ratio: r -> ratio_out, fp32 [n/per_sample]. e_cond, e_uncond: n elements of model_dtype each.
+ *   One streaming pass with fp64 per-chunk moments and a final kernel that merges them in chunk order: the bits of
+ *   r_b depend on sample b's values only. A sample of one element gives NaN (unbiased std), a constant guided sample
+ *   inf or NaN; nothing is clamped. workspace: dpm_cfg_rescale_workspace(n/per_sample, per_sample) bytes of 8-byte
+ *   aligned device memory (contents irrelevant).
+ * dpm_step_rescaled: dpm_step with the rescale; desc->n_model == 2, desc->per_sample set (dividing n),
+ *   desc->raw_round == 0. ratio: device fp32 [n/per_sample] (from dpm_cfg_rescale_ratio, same guidance).
+ *   phi, one_minus_phi: fl32(phi) and fl32(1 - phi) with 1 - phi formed in double. Served by the direct vector
+ *   kernels (tails, unaligned views and dev_coef launches by the generic kernel); never by the TMA variant. */
+DPM_API size_t dpm_cfg_rescale_workspace(uint64_t n_samples, uint64_t per_sample);
+DPM_API int dpm_cfg_rescale_ratio(float* ratio_out, const void* e_cond, const void* e_uncond, float guidance,
+                                  uint64_t per_sample, uint64_t n, int model_dtype,
+                                  void* workspace, size_t workspace_bytes, dpm_stream_t stream);
+DPM_API int dpm_step_rescaled(const dpm_step_desc* desc, const float* ratio, float phi, float one_minus_phi,
+                              dpm_stream_t stream);
+
 /* ---- dpm_solver_adaptive with the controller on the device (:956-1010) -------------------------------------
  * Device buffers (caller-allocated, fp32): state[16] (s, lambda_s, lambda_0, h, t, nfe, done, accept, iterations as
  * int bit patterns where integral), coef[4][16] (one dpm_step_desc.dev_coef block per fused launch of an
