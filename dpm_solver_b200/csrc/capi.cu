@@ -231,13 +231,11 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale*
   bool body_done = false;
   if (p.npk > 0 && all_aligned(p, nd) && p.dev_coef == nullptr) {   // device-side scalars: generic kernel only
     int r = 1;
-    // small launches (a few tiles per SM) gain nothing from the ring; auto keeps them direct
-    // fp32 state: direct vector loads already sit near the HBM roofline (fewer instructions per
-    // byte); 16-bit state is issue-limited there and gains from the ring (measured on the first target GPU)
+    // auto: the direct variant for every launch. On H100 its one-tile-per-CTA grid streams the 16-bit steps
+    // faster than the ring (DESIGN.md §4); the ring runs when it is asked for
     const bool tma = p.raw_round == 0 &&   // reference-rounding mode: the direct variant's <RND> kernels
                      p.ratio == nullptr &&  // guidance rescale: the direct variant's <RS> kernels
-                     (t.variant == 1 || (t.variant == 2 && p.state_dtype != DPM_F32 &&
-                                         p.npk >= (uint32_t)sm_count() * 1024u));
+                     t.variant == 1;
     if (tma) r = launch_step_tma(p, t, stream);
     if (r == 1) r = launch_step_direct(p, t, stream);
     if (r < 0 || r > 1) return r;

@@ -79,8 +79,9 @@ static inline R pick_step(const KParams& p, Pick&& pick) {
 // Programmatic dependent launch (PDL): the step kernels call pdl_wait() after their prologue (barrier init, index
 // setup) and before touching global memory, and pdl_trigger() at entry; launched with the programmatic-stream-
 // serialization attribute, the CTAs of step i+1 become resident while step i drains and only their first global
-// access waits for its completion (and visibility). Without the attribute both are no-ops. Persistent one-wave grids
-// only, so an early dependent can never starve its primary.
+// access waits for its completion (and visibility). Without the attribute both are no-ops. The dependent grid starts
+// only once every CTA of the primary has run pdl_trigger(), i.e. once the primary's last wave is resident, so an
+// early dependent can never starve its primary, whatever the number of waves.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 bool pdl_enabled();   // DPM_PDL=0 turns the launch attribute off (A/B measurements)

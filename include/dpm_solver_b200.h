@@ -138,9 +138,9 @@ DPM_API int dpm_version(void);
 DPM_API const char* dpm_last_error(void);
 
 /* Tuning knobs (process-wide, read at launch): variant 0 = direct 128/256-bit global
- * loads, 1 = TMA (cp.async.bulk) shared-memory ring, 2 = auto (default: the ring for 16-bit state
- * tensors and launches of >= 1024 packets per SM, direct otherwise); threads per CTA; CTAs per SM for the persistent
- * grid; 0 keeps the built-in default. Returns DPM_ERR_ARG on invalid values. */
+ * loads, 1 = TMA (cp.async.bulk) shared-memory ring, 2 = auto (default: direct); threads per CTA; CTAs per SM of a
+ * persistent grid (0: the direct variant launches one CTA per tile, the ring its built-in shape); 0 keeps the built-in
+ * default. Returns DPM_ERR_ARG on invalid values. */
 DPM_API int dpm_set_tuning(int variant, int threads, int ctas_per_sm);
 DPM_API int dpm_get_tuning(int* variant, int* threads, int* ctas_per_sm);
 /* number of kernels launched by this library since load (all streams) */

@@ -21,7 +21,7 @@ dev = "cuda"
 g = torch.Generator(device=dev).manual_seed(0)
 mk = lambda n, dt=torch.float32: torch.randn(n, device=dev, generator=g).to(dt)
 co = dict(a=0.95, c0=-0.1, c1=0.05, c2=-0.01, w0=1.02, w1=0.98, w2=0.51, w3=0.5, w4=0.33)
-n = 8 * 148 * 1024 + 8 * 700 + 5          # > 1024 packets per SM so that auto picks the ring for 16-bit state
+n = 8 * 148 * 1024 + 8 * 700 + 5          # > 1024 packets per SM: many tiles per SM on both variants, and a tail
 for variant in (0, 1):
     be.set_tuning(variant, 0, 0)
     for dt in (torch.float32, torch.bfloat16):
