@@ -83,6 +83,8 @@ PROTOTYPES = {
     "dpm_cfg_rescale_workspace": (C.c_size_t, [_u64, _u64]),
     "dpm_cfg_rescale_ratio": (C.c_int, [_vp, _vp, _vp, _f, _u64, _u64, _i, _vp, C.c_size_t, _vp]),
     "dpm_step_rescaled": (C.c_int, [C.POINTER(StepDesc), _vp, _f, _f, _vp]),
+    "dpm_step_guided": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _f, _f, _vp]),
+    "dpm_cfg_rescale_ratio_guided": (C.c_int, [_vp, _vp, _vp, _vp, _u64, _u64, _i, _vp, C.c_size_t, _vp]),
 }
 
 _lib = None

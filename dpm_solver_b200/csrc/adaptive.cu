@@ -155,6 +155,7 @@ struct RParams {
   uint32_t chunks;       // per sample
   int32_t dtype;
   float guidance;
+  const float* gscale;   // per-sample scales [n_samples] in place of `guidance` (<PG = true> only)
 };
 
 // deterministic CTA sum of one double per thread (butterfly within the warps, then the warps in order)
@@ -170,7 +171,15 @@ __device__ __forceinline__ double cta_sum(double v, double* warp_part) {
   return s;
 }
 
-template <typename T, bool VEC>
+// the scale of the combine: the launch's, or with PG sample b's
+template <bool PG>
+__device__ __forceinline__ float ratio_scale(const RParams& p, uint64_t sample) {
+  if constexpr (PG) return __ldg(p.gscale + sample);
+  else return p.guidance;
+}
+
+// PG: per-sample guidance (dpm_cfg_rescale_ratio_guided): g = out_u + s_b*(out_c - out_u) with the sample's scale
+template <typename T, bool VEC, bool PG = false>
 __global__ void __launch_bounds__(kEThreads) k_cfg_ratio_partial(const __grid_constant__ RParams p) {
   __shared__ double warp_part[2][kEThreads / 32];
   const uint64_t sample = blockIdx.x / p.chunks;
@@ -203,7 +212,7 @@ __global__ void __launch_bounds__(kEThreads) k_cfg_ratio_partial(const __grid_co
         unpack(rc[u], fc[u]);
         unpack(ru[u], fu);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) fg[u][i] = fu[i] + p.guidance * (fc[u][i] - fu[i]);   // :330
+        for (int i = 0; i < 8; ++i) fg[u][i] = fu[i] + ratio_scale<PG>(p, sample) * (fc[u][i] - fu[i]);   // :330
       }
     }
   } else {
@@ -215,7 +224,7 @@ __global__ void __launch_bounds__(kEThreads) k_cfg_ratio_partial(const __grid_co
         if (k < cnt) {
           const float c = load_any(p.ec, p.dtype, e0 + k), uu = load_any(p.eu, p.dtype, e0 + k);
           fc[u][i] = c;
-          fg[u][i] = uu + p.guidance * (c - uu);   // :330
+          fg[u][i] = uu + ratio_scale<PG>(p, sample) * (c - uu);   // :330
         }
       }
     }
@@ -288,8 +297,10 @@ size_t cfg_rescale_workspace_bytes(uint64_t n_samples, uint64_t per_sample) {
 }
 
 int launch_cfg_rescale_ratio(float* ratio, const void* ec, const void* eu, float guidance, uint64_t per_sample,
-                             uint64_t n, int dtype, void* ws, size_t ws_bytes, cudaStream_t stream) {
+                             uint64_t n, int dtype, void* ws, size_t ws_bytes, cudaStream_t stream,
+                             const float* gscale) {
   RParams p;
+  p.gscale = gscale;
   p.ec = ec; p.eu = eu; p.ratio = ratio; p.per_sample = per_sample; p.n_samples = n / per_sample;
   p.chunks = (uint32_t)((per_sample + kEChunk - 1) / kEChunk);
   p.dtype = dtype; p.guidance = guidance;
@@ -305,6 +316,7 @@ int launch_cfg_rescale_ratio(float* ratio, const void* ec, const void* eu, float
   typedef void (*RKernel)(const RParams);
   RKernel k = with_packet_pair(dtype, dtype, [&](auto pair) -> RKernel {
     using T = typename decltype(pair)::TS;
+    if (gscale != nullptr) return vec ? k_cfg_ratio_partial<T, true, true> : k_cfg_ratio_partial<T, false, true>;
     return vec ? k_cfg_ratio_partial<T, true> : k_cfg_ratio_partial<T, false>;
   });
   k<<<(unsigned)(p.n_samples * p.chunks), kEThreads, 0, stream>>>(p);

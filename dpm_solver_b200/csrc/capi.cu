@@ -212,7 +212,9 @@ struct Rescale {
   float phi, psi;
 };
 
-static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale* rs = nullptr) {
+// gscale (optional): per-sample guidance of an n_model == 2 step, fp32 [n/per_sample]; rs then may be NULL
+static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale* rs = nullptr,
+                     const float* gscale = nullptr) {
   KParams p;
   Needs nd;
   if (d != nullptr && d->n == 0) return DPM_OK;  // empty tensors: nothing to do (pointers may be NULL)
@@ -226,6 +228,7 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale*
     }
     p.ratio = rs->ratio; p.phi = rs->phi; p.psi = rs->psi;
   }
+  p.gscale = gscale;
   Tuning t{g_variant.load(), g_threads.load(), g_ctas.load()};
 
   bool body_done = false;
@@ -235,6 +238,7 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale*
     // faster than the ring (DESIGN.md §4); the ring runs when it is asked for
     const bool tma = p.raw_round == 0 &&   // reference-rounding mode: the direct variant's <RND> kernels
                      p.ratio == nullptr &&  // guidance rescale: the direct variant's <RS> kernels
+                     p.gscale == nullptr &&  // per-sample guidance: the direct variant's <PG> kernels
                      t.variant == 1;
     if (tma) r = launch_step_tma(p, t, stream);
     if (r == 1) r = launch_step_direct(p, t, stream);
@@ -283,6 +287,19 @@ int dpm_step_rescaled(const dpm_step_desc* desc, const float* ratio, float phi, 
   return step_impl(desc, static_cast<cudaStream_t>(stream), &rs);
 }
 
+int dpm_step_guided(const dpm_step_desc* desc, const float* guidance, const float* ratio, float phi,
+                    float one_minus_phi, dpm_stream_t stream) {
+  if (desc != nullptr && desc->n == 0) return DPM_OK;
+  if (desc == nullptr || guidance == nullptr || desc->n_model != 2 || desc->raw_round != 0 || desc->per_sample == 0 ||
+      desc->n % desc->per_sample) {
+    set_error("guided step: needs guidance, n_model == 2, raw_round == 0 and per_sample dividing n");
+    return DPM_ERR_ARG;
+  }
+  if (ratio == nullptr) return step_impl(desc, static_cast<cudaStream_t>(stream), nullptr, guidance);
+  const Rescale rs{ratio, phi, one_minus_phi};
+  return step_impl(desc, static_cast<cudaStream_t>(stream), &rs, guidance);
+}
+
 size_t dpm_cfg_rescale_workspace(uint64_t n_samples, uint64_t per_sample) {
   return cfg_rescale_workspace_bytes(n_samples, per_sample);
 }
@@ -295,6 +312,16 @@ int dpm_cfg_rescale_ratio(float* ratio_out, const void* e_cond, const void* e_un
   if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) { set_error("cfg rescale: bad dtype or sizes"); return DPM_ERR_ARG; }
   return finish(launch_cfg_rescale_ratio(ratio_out, e_cond, e_uncond, guidance, per_sample, n, model_dtype, workspace,
                                          workspace_bytes, static_cast<cudaStream_t>(stream)));
+}
+
+int dpm_cfg_rescale_ratio_guided(float* ratio_out, const void* e_cond, const void* e_uncond, const float* guidance,
+                                 uint64_t per_sample, uint64_t n, int model_dtype, void* workspace,
+                                 size_t workspace_bytes, dpm_stream_t stream) {
+  if (n == 0) return DPM_OK;
+  if (!ratio_out || !e_cond || !e_uncond || !guidance) { set_error("cfg rescale: NULL tensor"); return DPM_ERR_ARG; }
+  if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) { set_error("cfg rescale: bad dtype or sizes"); return DPM_ERR_ARG; }
+  return finish(launch_cfg_rescale_ratio(ratio_out, e_cond, e_uncond, 0.f, per_sample, n, model_dtype, workspace,
+                                         workspace_bytes, static_cast<cudaStream_t>(stream), guidance));
 }
 
 static dpm_step_desc base_desc(void* out, const void* x, uint64_t n, int dtype, int form) {

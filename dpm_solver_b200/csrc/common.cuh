@@ -61,6 +61,9 @@ struct KParams {
   // host-rounded weights phi, psi = fl32(1 - phi). Only the <RS = true> instantiations read them.
   const float* ratio;
   float phi, psi;
+  // per-sample classifier-free guidance (dpm_step_guided): fp32 scale per sample [n/per_sample], in place of
+  // `guidance`. Only the <PG = true> instantiations read it; with it, `ratio` may be NULL (no rescale).
+  const float* gscale;
 };
 
 // ---- storage types ------------------------------------------------------------------------
@@ -281,18 +284,48 @@ __device__ __forceinline__ float rescale_value(const KParams& p, float g, float 
   return p.phi * (g * r) + p.psi * g;
 }
 
+// per-sample guidance with the sample's scale gs, in one of three kinds that are uniform over a sample (the caller
+// picks the kind once per packet, or per element with kPgAny):
+//   kPgBypass  gs == 1: the reference's bypass (:323), the converted conditional output alone (no combine, no rescale)
+//   kPgRescale p.ratio set: the rescaled combine of the RS path
+//   kPgCombine otherwise: the combine of the plain path
+enum { kPgAny = 1, kPgBypass = 2, kPgRescale = 3, kPgCombine = 4 };
+__host__ __device__ __forceinline__ int pg_kind(const KParams& p, float gs) {
+  return gs == 1.f ? kPgBypass : (p.ratio != nullptr ? kPgRescale : kPgCombine);
+}
+template <int K>
+__device__ __forceinline__ float guided_value(const KParams& p, float xe, float ec, float eu, float r, float gs) {
+  if constexpr (K == kPgAny) {
+    const int k = pg_kind(p, gs);
+    if (k == kPgBypass) return guided_value<kPgBypass>(p, xe, ec, eu, r, gs);
+    if (k == kPgRescale) return guided_value<kPgRescale>(p, xe, ec, eu, r, gs);
+    return guided_value<kPgCombine>(p, xe, ec, eu, r, gs);
+  } else if constexpr (K == kPgBypass) {
+    return convert_param(p.param, ec, xe, p.alpha_e, p.sigma_e);
+  } else if constexpr (K == kPgRescale) {
+    return convert_param(p.param, rescale_value(p, eu + gs * (ec - eu), r), xe, p.alpha_e, p.sigma_e);
+  } else {
+    const float epc = convert_param(p.param, ec, xe, p.alpha_e, p.sigma_e);
+    const float epu = convert_param(p.param, eu, xe, p.alpha_e, p.sigma_e);
+    return epu + gs * (epc - epu);  // :330
+  }
+}
+
 // RS: guidance rescale (NE == 2). The combine then runs on the raw outputs, the rescale follows, and the
 // parameterisation converts the rescaled prediction -- the order of a rescaling network wrapped by :288-298.
-template <int NE, bool RND = false, bool RS = false>
+// PG: per-sample guidance (NE == 2, guided_value<PG>) with the sample's scale gs; 0 = off, else the kind.
+template <int NE, bool RND = false, bool RS = false, int PG = 0>
 __device__ __forceinline__ float model_value(const KParams& p, float xe, float ec, float eu,
-                                             float thr, bool clamp, float r = 1.f) {
+                                             float thr, bool clamp, float r = 1.f, float gs = 1.f) {
   float eps;
-  if (RS) {
+  if constexpr (PG != 0) {
+    eps = guided_value<PG>(p, xe, ec, eu, r, gs);
+  } else if (RS) {
     eps = convert_param(p.param, rescale_value(p, eu + p.guidance * (ec - eu), r), xe, p.alpha_e, p.sigma_e);
   } else {
     eps = convert_param(p.param, ec, xe, p.alpha_e, p.sigma_e);
   }
-  if (NE == 2 && !RS) {
+  if (NE == 2 && !RS && !PG) {
     float epu = convert_param(p.param, eu, xe, p.alpha_e, p.sigma_e);
     if (RND && p.param == DPM_PARAM_NOISE) {
       const int dt = p.raw_round & 3;
@@ -370,12 +403,28 @@ __device__ __forceinline__ float update_value(const KParams& p, float x, float T
 // straight-line code over 8 elements. Callers guarantee: p.param == NOISE; p.fast_div when a division
 // is needed; a clamp threshold `s` that is uniform over the packet.
 // RS: guidance rescale with the sample's ratio r (uniform over the packet, like s).
-template <int NE, bool RS = false>
+// PG: per-sample guidance with the sample's scale gs (uniform over the packet): gs == 1 selects ec (the bypass),
+// else the combine, rescaled when p.ratio is set -- both branches uniform per packet.
+template <int NE, bool RS = false, bool PG = false>
 __device__ __forceinline__ void fast_model8(const KParams& p, const float (&xe)[8], const float (&ec)[8],
                                             const float (&eu)[8], bool clamp, float s, float (&T)[8],
-                                            float r = 1.f) {
+                                            float r = 1.f, float gs = 1.f) {
+  if constexpr (PG) {
+    if (gs == 1.f) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) T[i] = (NE == 2) ? eu[i] + p.guidance * (ec[i] - eu[i]) : ec[i];  // :330
+      for (int i = 0; i < 8; ++i) T[i] = ec[i];   // :323 (p.param == NOISE: the conversion is the identity)
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) T[i] = eu[i] + gs * (ec[i] - eu[i]);  // :330
+      if (p.ratio != nullptr) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) T[i] = rescale_value(p, T[i], r);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) T[i] = (NE == 2) ? eu[i] + p.guidance * (ec[i] - eu[i]) : ec[i];  // :330
+  }
   if (RS) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) T[i] = rescale_value(p, T[i], r);
@@ -433,7 +482,7 @@ __host__ __forceinline__ bool fast_path_ok(const KParams& p) {
   if (p.n_model == 0) return true;
   if (p.param != DPM_PARAM_NOISE) return false;
   if (p.predict_x0 && !p.fast_div) return false;
-  if ((p.thr != nullptr || p.ratio != nullptr) && p.pk_per_sample == 0) return false;
+  if ((p.thr != nullptr || p.ratio != nullptr || p.gscale != nullptr) && p.pk_per_sample == 0) return false;
   return true;
 }
 

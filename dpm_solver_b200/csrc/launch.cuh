@@ -124,6 +124,7 @@ int launch_adaptive_error(float* out, const void* xh, const void* xl, const void
                           uint64_t per_sample, uint64_t n, int dtype, void* ws, size_t ws_bytes, cudaStream_t stream);
 size_t cfg_rescale_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
 int launch_cfg_rescale_ratio(float* ratio, const void* ec, const void* eu, float guidance, uint64_t per_sample,
-                             uint64_t n, int dtype, void* ws, size_t ws_bytes, cudaStream_t stream);
+                             uint64_t n, int dtype, void* ws, size_t ws_bytes, cudaStream_t stream,
+                             const float* gscale = nullptr);
 
 }  // namespace dpm

@@ -19,7 +19,9 @@ constexpr int kMaxThreads = 512;
 // loads and stores.
 // RS (only with NE == 2 and RND = false): guidance rescale (dpm_step_rescaled) with the per-sample ratio p.ratio, read
 // like the per-sample thresholds.
-template <typename TE, typename TS, int NE, int FORM, bool FAST, bool RND = false, bool RS = false>
+// PG (only with NE == 2, RND = false and RS = false): per-sample guidance (dpm_step_guided) with the scale p.gscale
+// and, when p.ratio is set, the rescale -- one kernel family for rescale on and off.
+template <typename TE, typename TS, int NE, int FORM, bool FAST, bool RND = false, bool RS = false, bool PG = false>
 __global__ void __launch_bounds__(kMaxThreads)
     k_step_direct(const __grid_constant__ KParams p) {
   constexpr bool kX = form_reads(FORM).x, kM1 = form_reads(FORM).m1, kM2 = form_reads(FORM).m2;
@@ -78,12 +80,23 @@ __global__ void __launch_bounds__(kMaxThreads)
           unpack(rec[u], fec);
           if (NE == 2) unpack(reu[u], feu);
           const float s_thr = clamp ? __ldg(p.thr + (uint32_t)pk / p.pk_per_sample) : 1.f;   // packet index < 2^32 (npk)
-          const float r = RS ? __ldg(p.ratio + (uint32_t)pk / p.pk_per_sample) : 1.f;
-          if (sep_xe) {
-            unpack(rxe[u], fxe);
-            fast_model8<NE, RS>(p, fxe, fec, feu, clamp, s_thr, fT, r);
+          if constexpr (PG) {
+            const float r = p.ratio != nullptr ? __ldg(p.ratio + (uint32_t)pk / p.pk_per_sample) : 1.f;
+            const float gs = __ldg(p.gscale + (uint32_t)pk / p.pk_per_sample);
+            if (sep_xe) {
+              unpack(rxe[u], fxe);
+              fast_model8<NE, false, true>(p, fxe, fec, feu, clamp, s_thr, fT, r, gs);
+            } else {
+              fast_model8<NE, false, true>(p, fx, fec, feu, clamp, s_thr, fT, r, gs);   // fx: as below
+            }
           } else {
-            fast_model8<NE, RS>(p, fx, fec, feu, clamp, s_thr, fT, r);   // fx is only read when predict_x0 (then it is loaded)
+            const float r = RS ? __ldg(p.ratio + (uint32_t)pk / p.pk_per_sample) : 1.f;
+            if (sep_xe) {
+              unpack(rxe[u], fxe);
+              fast_model8<NE, RS>(p, fxe, fec, feu, clamp, s_thr, fT, r);
+            } else {
+              fast_model8<NE, RS>(p, fx, fec, feu, clamp, s_thr, fT, r);   // fx is only read when predict_x0 (then it is loaded)
+            }
           }
           Raw<TS> rmo;
           round_pack(rmo, fT);
@@ -101,37 +114,56 @@ __global__ void __launch_bounds__(kMaxThreads)
 #pragma unroll
             for (int i = 0; i < 8; ++i) fxe[i] = 0.f;
           }
-          float thr8[8];
-          const bool thr_uniform = p.pk_per_sample != 0;
-          if (clamp) {
-            if (thr_uniform) {
-              const float tpk = __ldg(p.thr + (uint32_t)(pk / p.pk_per_sample));
+          if constexpr (PG) {
+            // samples hold whole packets here (pick_direct): the sample's scale, ratio (when the launch is rescaled) and
+            // threshold are one scalar each per packet
+            const uint32_t b = (uint32_t)(pk / p.pk_per_sample);
+            const float gpk = __ldg(p.gscale + b), rpk = p.ratio != nullptr ? __ldg(p.ratio + b) : 1.f;
+            const float tpk = clamp ? __ldg(p.thr + b) : 1.f;
+            // the kind of the combine is uniform per packet: one branch per packet, straight-line code per element
+            auto guided8 = [&](auto kind) {
 #pragma unroll
-              for (int i = 0; i < 8; ++i) thr8[i] = tpk;
-            } else {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) thr8[i] = __ldg(p.thr + (e + i) / p.per_sample);
-            }
+              for (int i = 0; i < 8; ++i)
+                fT[i] = model_value<NE, false, false, decltype(kind)::value>(p, fxe[i], fec[i], feu[i], tpk, clamp,
+                                                                             rpk, gpk);
+            };
+            const int kind = pg_kind(p, gpk);
+            if (kind == kPgBypass) guided8(std::integral_constant<int, kPgBypass>{});
+            else if (kind == kPgRescale) guided8(std::integral_constant<int, kPgRescale>{});
+            else guided8(std::integral_constant<int, kPgCombine>{});
           } else {
+            float thr8[8];
+            const bool thr_uniform = p.pk_per_sample != 0;
+            if (clamp) {
+              if (thr_uniform) {
+                const float tpk = __ldg(p.thr + (uint32_t)(pk / p.pk_per_sample));
 #pragma unroll
-            for (int i = 0; i < 8; ++i) thr8[i] = 1.f;
-          }
-          float r8[8];
+                for (int i = 0; i < 8; ++i) thr8[i] = tpk;
+              } else {
 #pragma unroll
-          for (int i = 0; i < 8; ++i) r8[i] = 1.f;
-          if (RS) {
-            if (thr_uniform) {
-              const float rpk = __ldg(p.ratio + (uint32_t)(pk / p.pk_per_sample));
-#pragma unroll
-              for (int i = 0; i < 8; ++i) r8[i] = rpk;
+                for (int i = 0; i < 8; ++i) thr8[i] = __ldg(p.thr + (e + i) / p.per_sample);
+              }
             } else {
 #pragma unroll
-              for (int i = 0; i < 8; ++i) r8[i] = __ldg(p.ratio + (e + i) / p.per_sample);
+              for (int i = 0; i < 8; ++i) thr8[i] = 1.f;
             }
-          }
+            float r8[8];
 #pragma unroll
-          for (int i = 0; i < 8; ++i)
-            fT[i] = model_value<NE, RND, RS>(p, fxe[i], fec[i], NE == 2 ? feu[i] : 0.f, thr8[i], clamp, r8[i]);
+            for (int i = 0; i < 8; ++i) r8[i] = 1.f;
+            if (RS) {
+              if (thr_uniform) {
+                const float rpk = __ldg(p.ratio + (uint32_t)(pk / p.pk_per_sample));
+#pragma unroll
+                for (int i = 0; i < 8; ++i) r8[i] = rpk;
+              } else {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) r8[i] = __ldg(p.ratio + (e + i) / p.per_sample);
+              }
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+              fT[i] = model_value<NE, RND, RS>(p, fxe[i], fec[i], NE == 2 ? feu[i] : 0.f, thr8[i], clamp, r8[i]);
+          }
           Raw<TS> rmo;
           round_pack(rmo, fT);
           if (gmo != nullptr) stg_pk(gmo + e, rmo);
@@ -161,7 +193,8 @@ __global__ void __launch_bounds__(kMaxThreads)
 // RND = true: reference-rounding mode (common.cuh) for the launches the <RND> vector kernels do not serve:
 // unaligned views, tails and fp32 network outputs.
 // RS = true: guidance rescale (n_model == 2) for unaligned views, tails and dev_coef launches.
-template <bool RND, bool RS = false>
+// PG = true: per-sample guidance (n_model == 2; rescale iff p.ratio is set), likewise.
+template <bool RND, bool RS = false, bool PG = false>
 __global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KParams pc) {
   KParams p = pc;
   if (pc.dev_coef != nullptr) {
@@ -188,7 +221,11 @@ __global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KPa
       float eu = p.n_model == 2 ? load_any(p.eu, md, i) : 0.f;
       float thr = clamp ? p.thr[(i + p.elem_offset) / p.per_sample] : 1.f;
       float mv;
-      if (RS) {
+      if constexpr (PG) {
+        const uint64_t b = (i + p.elem_offset) / p.per_sample;
+        mv = model_value<2, false, false, kPgAny>(p, xe, ec, eu, thr, clamp, p.ratio != nullptr ? p.ratio[b] : 1.f,
+                                                  p.gscale[b]);
+      } else if (RS) {
         mv = model_value<2, false, true>(p, xe, ec, eu, thr, clamp, p.ratio[(i + p.elem_offset) / p.per_sample]);
       } else {
         mv = p.n_model == 2 ? model_value<2, RND>(p, xe, ec, eu, thr, clamp)
@@ -221,12 +258,21 @@ typedef void (*StepKernel)(const KParams);
 // RND: an fp32 state with raw network outputs in bf16 / f16 (NE >= 1), or fp32 buffers holding such raw outputs
 // (NE == 0, differences rounded).
 // RS: guidance rescale, NE == 2 only (the C-ABI rejects it together with raw_round).
+// PG: per-sample guidance, NE == 2 only; serves rescaled and plain launches alike (so it is tested before RS).
 static StepKernel pick_direct(const KParams& p) {
-  const bool fast = fast_path_ok(p), rnd = p.raw_round != 0, rs = p.ratio != nullptr;
+  const bool fast = fast_path_ok(p), rnd = p.raw_round != 0, rs = p.ratio != nullptr, pg = p.gscale != nullptr;
+  if (pg && p.pk_per_sample == 0) return nullptr;
   return pick_step<StepKernel>(p, [&](auto pair, auto ne, auto form) -> StepKernel {
     using TE = typename decltype(pair)::TE;
     using TS = typename decltype(pair)::TS;
     constexpr int NE = decltype(ne)::value, FORM = decltype(form)::value;
+    if (pg) {   // samples that do not hold whole packets: the generic kernel (k_step_scalar<PG>)
+      if constexpr (NE == 2)
+        return fast ? k_step_direct<TE, TS, 2, FORM, true, false, false, true>
+                    : k_step_direct<TE, TS, 2, FORM, false, false, false, true>;
+      else
+        return nullptr;
+    }
     if (rs) {
       if constexpr (NE == 2)
         return fast ? k_step_direct<TE, TS, 2, FORM, true, false, true> : k_step_direct<TE, TS, 2, FORM, false, false, true>;
@@ -272,6 +318,7 @@ int launch_step_scalar(const KParams& p, cudaStream_t stream) {
   uint64_t cap = (uint64_t)sm_count() * 8;
   uint32_t grid = (uint32_t)(blocks < cap ? blocks : cap);
   if (p.raw_round) k_step_scalar<true><<<grid, threads, 0, stream>>>(p);
+  else if (p.gscale) k_step_scalar<false, false, true><<<grid, threads, 0, stream>>>(p);
   else if (p.ratio) k_step_scalar<false, true><<<grid, threads, 0, stream>>>(p);
   else k_step_scalar<false><<<grid, threads, 0, stream>>>(p);
   count_launch();

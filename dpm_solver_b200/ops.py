@@ -60,6 +60,9 @@ class StepArgs:
     # guidance rescale (dpm_step_rescaled; n_model == 2, per_sample set): fp32 [B] from cfg_rescale_ratio, and phi
     ratio: Optional[torch.Tensor] = None
     phi: float = 0.0
+    # per-sample classifier-free guidance (dpm_step_guided; n_model == 2, per_sample set): fp32 [B] on the device, in
+    # place of `guidance`. With `ratio` the step is also rescaled.
+    guidance_b: Optional[torch.Tensor] = None
 
     def state_tensors(self):
         return [t for t in (self.x, self.xe, self.m0, self.m1, self.m2) if t is not None]
@@ -204,23 +207,31 @@ class CudaBackend:
                 if self._layout(a.out2) != layout:      # dense, laid out like `out` (a channels_last half of the
                     raise ValueError("dpm_solver_b200: out2 must be dense and laid out like out")   # doubled CFG batch is)
                 d.out2 = a.out2.data_ptr()
-        if a.ratio is not None:
-            r = a.ratio
-            if not r.is_cuda or r.dtype != torch.float32 or not r.is_contiguous() or r.device != ref.device:
-                raise TypeError("dpm_solver_b200: `ratio` must be a contiguous fp32 tensor on the tensors' device")
-            if a.per_sample <= 0 or ref.numel() % a.per_sample or r.numel() != ref.numel() // a.per_sample:
-                raise ValueError("dpm_solver_b200: `ratio` needs one value per sample")
+        for v, what in ((a.ratio, "ratio"), (a.guidance_b, "guidance_b")):
+            if v is None:
+                continue
+            if not v.is_cuda or v.dtype != torch.float32 or not v.is_contiguous() or v.device != ref.device:
+                raise TypeError(f"dpm_solver_b200: `{what}` must be a contiguous fp32 tensor on the tensors' device")
+            if a.per_sample <= 0 or ref.numel() % a.per_sample or v.numel() != ref.numel() // a.per_sample:
+                raise ValueError(f"dpm_solver_b200: `{what}` needs one value per sample")
+        if a.guidance_b is not None:
+            # (phi and 1 - phi as below; ignored without a ratio)
+            self._launch(ref.device, self._lib.dpm_step_guided, C.byref(d), C.c_void_p(a.guidance_b.data_ptr()),
+                         C.c_void_p(None if a.ratio is None else a.ratio.data_ptr()), C.c_float(a.phi),
+                         C.c_float(1.0 - a.phi))
+        elif a.ratio is not None:
             # phi and 1 - phi (formed in double, as the python-float expression does), each rounded to fp32 once
-            self._launch(ref.device, self._lib.dpm_step_rescaled, C.byref(d), C.c_void_p(r.data_ptr()),
+            self._launch(ref.device, self._lib.dpm_step_rescaled, C.byref(d), C.c_void_p(a.ratio.data_ptr()),
                          C.c_float(a.phi), C.c_float(1.0 - a.phi))
         else:
             self._launch(ref.device, self._lib.dpm_step, C.byref(d))
         return m_out, out
 
-    def cfg_rescale_ratio(self, e_cond: torch.Tensor, e_uncond: torch.Tensor, guidance: float) -> torch.Tensor:
+    def cfg_rescale_ratio(self, e_cond: torch.Tensor, e_uncond: torch.Tensor, guidance) -> torch.Tensor:
         """Per-sample r = std(e_cond_b) / std(g_b), g = e_uncond + guidance*(e_cond - e_uncond), as fp32 [B] on the
         device (dpm_cfg_rescale_ratio). Both halves keep a shared dense layout: a sample is one contiguous block
-        in row-major and in channels_last storage alike."""
+        in row-major and in channels_last storage alike. `guidance` may be a contiguous fp32 device tensor of B
+        per-sample scales (dpm_cfg_rescale_ratio_guided)."""
         n, dev = e_cond.numel(), e_cond.device
         layout = self._layout(e_cond)
         if layout is None or self._layout(e_uncond) != layout:
@@ -232,6 +243,16 @@ class CudaBackend:
         r = torch.empty(nb, dtype=torch.float32, device=dev)
         ws_bytes = int(self._lib.dpm_cfg_rescale_workspace(nb, per_sample))
         ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev)
+        if torch.is_tensor(guidance):
+            if not guidance.is_cuda or guidance.dtype != torch.float32 or not guidance.is_contiguous() \
+                    or guidance.device != dev or guidance.numel() != nb:
+                raise ValueError("dpm_solver_b200: per-sample guidance must be a contiguous fp32 [B] tensor on the "
+                                 "tensors' device")
+            self._launch(dev, self._lib.dpm_cfg_rescale_ratio_guided, C.c_void_p(r.data_ptr()),
+                         C.c_void_p(ec.data_ptr()), C.c_void_p(eu.data_ptr()), C.c_void_p(guidance.data_ptr()),
+                         C.c_uint64(per_sample), C.c_uint64(n), C.c_int(_DTYPE_CODE[e_cond.dtype]),
+                         C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
+            return r
         self._launch(dev, self._lib.dpm_cfg_rescale_ratio, C.c_void_p(r.data_ptr()), C.c_void_p(ec.data_ptr()),
                      C.c_void_p(eu.data_ptr()), C.c_float(guidance), C.c_uint64(per_sample), C.c_uint64(n),
                      C.c_int(_DTYPE_CODE[e_cond.dtype]), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
@@ -252,6 +273,9 @@ class CudaBackend:
         """Per-sample s_b = max(quantile(|x0_b|, q), max_val) -> fp32 [B].
         return_stats=True also returns the pipeline's per-sample header words (int32 [B, 8]:
         lo key, hi key, #below, #inside, path (1 bracket / 2 exact fallback), ...) for diagnostics."""
+        if a.guidance_b is not None:
+            raise ValueError("dpm_solver_b200: the quantile takes one guidance scale; materialise a per-sample "
+                             "combine first")
         d, keep, ref, _, _ = self._fill(a)
         if a.per_sample <= 0 or ref.numel() % a.per_sample:
             raise ValueError("dpm_solver_b200: per_sample must divide numel")
@@ -446,8 +470,11 @@ class PreparedStep:
 
     @staticmethod
     def build(be: "CudaBackend", a: StepArgs) -> Optional["PreparedStep"]:
-        if a.thr is not None or a.raw_round or a.ratio is not None or a.out is not None and a.out2 is None:
-            return None     # (a rescaled step reads a fresh ratio tensor every evaluation: never frozen)
+        if a.thr is not None or a.raw_round or a.ratio is not None or a.guidance_b is not None \
+                or a.out is not None and a.out2 is None:
+            # (a rescaled step reads a fresh ratio tensor every evaluation, a guided one a scales tensor the
+            # descriptor does not carry: never frozen)
+            return None
         ref = a.reference_tensor()
         if not ref.is_contiguous():
             return None

@@ -47,6 +47,7 @@ class RawOutput:
     param: int
     guidance: float
     phi: float = 0.0        # guidance rescale of the combine (model_wrapper's guidance_rescale); 0 = off
+    guidance_b: Optional[torch.Tensor] = None   # per-sample scales, fp32 [B] (then `guidance` is not read)
 
 
 def _cfg_ratio(be, raw: RawOutput) -> Optional[torch.Tensor]:
@@ -57,14 +58,31 @@ def _cfg_ratio(be, raw: RawOutput) -> Optional[torch.Tensor]:
     if fn is None:
         raise RuntimeError("guidance_rescale needs an executor with cfg_rescale_ratio; {} has none".format(
             getattr(be, "name", type(be).__name__)))
-    return fn(raw.e_cond, raw.e_uncond, raw.guidance)
+    return fn(raw.e_cond, raw.e_uncond, raw.guidance if raw.guidance_b is None else raw.guidance_b)
 
 
-def _rescale_args(a: StepArgs, ratio: Optional[torch.Tensor], raw: RawOutput) -> StepArgs:
+def _guidance_args(a: StepArgs, ratio: Optional[torch.Tensor], raw: RawOutput, rows=None) -> StepArgs:
+    """The rescale ratio and the per-sample scales (rows `rows` of them) of `raw` on a CFG step."""
     if ratio is not None:
         a.ratio, a.phi = ratio, raw.phi
+    if raw.guidance_b is not None and a.n_model == 2:
+        a.guidance_b = raw.guidance_b if rows is None else raw.guidance_b[rows]
+    if a.ratio is not None or a.guidance_b is not None:
         a.per_sample = a.e_cond.numel() // a.e_cond.shape[0]
     return a
+
+
+def _scale_vector(guidance_scale, guidance_type):
+    """model_wrapper's guidance_scale as per-sample scales (a 1-D tensor, or None for one scale). A python number, a
+    0-dim or a one-element tensor is one scale, as before; any other tensor must be 1-D."""
+    s = guidance_scale
+    if not torch.is_tensor(s) or s.numel() == 1:
+        return None
+    if s.dim() != 1:
+        raise ValueError("a per-sample guidance_scale must be 1-D, got shape {}".format(tuple(s.shape)))
+    if guidance_type == "classifier":
+        raise ValueError("a per-sample guidance_scale needs guidance_type='classifier-free'")
+    return s
 
 
 class WrappedModel:
@@ -84,10 +102,14 @@ class WrappedModel:
         self.guidance_type = guidance_type
         self.condition = condition
         self.unconditional_condition = unconditional_condition
+        if isinstance(guidance_scale, (list, tuple)):
+            guidance_scale = torch.tensor(list(guidance_scale), dtype=torch.float32)   # each value rounded once
         self.guidance_scale = guidance_scale
         self.classifier_fn = classifier_fn
         self.classifier_kwargs = classifier_kwargs
         self._c_in = None
+        self._scale_vec = _scale_vector(guidance_scale, guidance_type)
+        self._gs = None
 
     # -- pieces of the reference closure ----------------------------------------------------
     def get_model_input_time(self, t_continuous):
@@ -104,9 +126,29 @@ class WrappedModel:
         return self.model(x, t_input, cond, **self.model_kwargs)
 
     @property
+    def per_sample_guidance(self) -> bool:
+        """True when classifier-free guidance runs with one scale per sample (other guidance types ignore the scale)."""
+        return self._scale_vec is not None and self.guidance_type == "classifier-free"
+
+    @property
     def uses_cfg(self) -> bool:
-        return (self.guidance_type == "classifier-free" and self.guidance_scale != 1.
-                and self.unconditional_condition is not None)
+        return (self.guidance_type == "classifier-free" and self.unconditional_condition is not None
+                and (self._scale_vec is not None or self.guidance_scale != 1.))
+
+    def _scales(self, x) -> torch.Tensor:
+        """The per-sample scales as the kernels read them: fp32 [B] on x's device. A contiguous fp32 tensor already
+        there is read in place (so values written into it between graph replays take effect); any other form is
+        converted once per (tensor, version, device). Never reads the values on the host."""
+        s = self._scale_vec
+        if s.numel() != x.shape[0]:
+            raise ValueError("guidance_scale has {} values for a batch of {}".format(s.numel(), x.shape[0]))
+        if s.device == x.device and s.dtype == torch.float32 and s.is_contiguous():
+            return s
+        key = (id(s), s._version, str(x.device))
+        if self._gs is None or self._gs[0] != key:
+            # the source is kept alive next to the key so that its id cannot be recycled
+            self._gs = (key, s.detach().to(device=x.device, dtype=torch.float32).contiguous(), s)
+        return self._gs[1]
 
     @property
     def fusable(self) -> bool:
@@ -135,12 +177,15 @@ class WrappedModel:
         if self.guidance_type == "uncond":
             return RawOutput(self._call_model(x, t_continuous, t_input=t_input), None, param, 1.0)
         if self.guidance_type == "classifier-free":
+            gb = self._scales(x) if self._scale_vec is not None else None     # (checked before the network runs)
             if not self.uses_cfg:
                 return RawOutput(self._call_model(x, t_continuous, cond=self.condition, t_input=t_input), None, param, 1.0)
             if x_in is None:
                 x_in = ops.backend().duplicate(x)              # cat([x] * 2) :326 (the solver hands over a prebuilt one)
             t_in = None if t_input is not None else torch.cat([t_continuous] * 2)
             out_u, out_c = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(2)  # uncond first
+            if gb is not None:
+                return RawOutput(out_c, out_u, param, 1.0, self.guidance_rescale, gb)
             return RawOutput(out_c, out_u, param, float(self.guidance_scale), self.guidance_rescale)
         raise RuntimeError("raw() is not available with classifier guidance")
 
@@ -198,7 +243,7 @@ class WrappedModel:
             a = StepArgs(form=FORM_NONE, n_model=2 if r.e_uncond is not None else 1, e_cond=r.e_cond[rows],
                          e_uncond=None if r.e_uncond is None else r.e_uncond[rows], param=r.param,
                          guidance=r.guidance, alpha_e=alpha, sigma_e=sigma, state_dtype=r.e_cond.dtype)
-            _rescale_args(a, None if ratio is None else ratio[rows], r)
+            _guidance_args(a, None if ratio is None else ratio[rows], r, rows)
             if needs_x:
                 a.xe = xo[rows]
             return be.step(a)[0]
@@ -216,7 +261,14 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     2023 as diffusers' `rescale_noise_cfg` does it, in the network's output space (eps for a noise network, v for
     a v network): g = out_u + s*(out_c - out_u), r_b = std(out_c_b)/std(g_b) per sample (unbiased),
     g' = phi*(g*r_b) + (1 - phi)*g, then the parameterisation converts g'. It applies only when the combine
-    runs (scale != 1 and an unconditional condition); 0 (default) is plain CFG."""
+    runs (scale != 1 and an unconditional condition); 0 (default) is plain CFG.
+
+    guidance_scale (classifier-free guidance) may also hold one scale per sample of x: a 1-D tensor, list or tuple of
+    B numbers (not in the reference). Row b of every result is then that of the same call with
+    guidance_scale=float(s[b]), each scale rounded to fp32 once; a row with s[b] == 1 gets the conditional output alone,
+    as the reference's bypass does, although the network still sees the doubled batch. A contiguous fp32 tensor on
+    x's device is read in place by the kernels (a captured graph sees values written into it); other forms are
+    converted once and cached. A python number, a 0-dim or a one-element tensor is one scale, as before."""
     assert model_type in ["noise", "x_start", "v", "score"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
     guidance_rescale = float(guidance_rescale)
@@ -292,6 +344,8 @@ class DPM_Solver:
         self.reference_rounding = bool(reference_rounding)
         if self.reference_rounding and getattr(model_fn, "guidance_rescale", 0) != 0:
             raise ValueError("guidance_rescale is not available with reference_rounding=True")
+        if self.reference_rounding and getattr(model_fn, "per_sample_guidance", False):
+            raise ValueError("a per-sample guidance_scale is not available with reference_rounding=True")
         self._rr_run = 0     # raw_round of the buffered values of the run in flight (reference_rounding)
         self._prep_cache = {}   # frozen launch descriptors of cached plan steps (ops.PreparedStep)
         self._prep_on = False
@@ -534,8 +588,9 @@ class DPM_Solver:
         pkey = None
         if slot is not None and self._prep_on:
             # (phi is part of the key: a rescaled evaluation is never served by a launch frozen without the rescale)
-            pkey = (slot, raw.param, raw.guidance, raw.phi, raw.e_uncond is None, raw.e_cond.dtype, xe.dtype, xe.shape,
-                    want_m, dup_out)
+            # (and so is a per-sample scale: a guided evaluation never meets a launch frozen with one scale)
+            pkey = (slot, raw.param, raw.guidance, raw.phi, raw.guidance_b is None, raw.e_uncond is None,
+                    raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out)
             prep = self._prep_cache.get(pkey)
             if prep is not None:
                 r = prep.launch((x, xe, raw.e_cond, m1, m2, raw.e_cond, raw.e_uncond))
@@ -559,14 +614,28 @@ class DPM_Solver:
             rr = code
             if not x0:
                 rr = self._rr_run = code | 4
-        if raw.e_uncond is not None and x0 and self._dynamic_thresholding and (code or ratio is not None):
-            # the quantile kernels take the plain fp32 combine: give them (and the step) the reference's rounded noise,
-            # or the rescaled network output, materialised once in fp32 and then treated as one network output (the
-            # parameterisation, which the quantile and the step apply, still converts it)
-            a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
-                         guidance=raw.guidance, state_dtype=torch.float32, raw_round=code)
-            e = be.step(_rescale_args(a, ratio, raw))[0]
-            raw = RawOutput(e, None, raw.param, 1.0)
+        if raw.e_uncond is not None and x0 and self._dynamic_thresholding and (
+                code or ratio is not None or raw.guidance_b is not None):
+            # the quantile kernels take the plain fp32 combine with one scale: give them (and the step) the reference's
+            # rounded noise, or the rescaled network output, materialised once in fp32 and then treated as one network
+            # output (the parameterisation, which the quantile and the step apply, still converts it) -- or, with
+            # per-sample scales and no rescale, the guided noise: each half parameterised, then combined with its
+            # sample's scale, as the reference orders it (+1 launch)
+            if ratio is None and raw.guidance_b is not None:
+                a = self._conv_args(raw, xe, alsig, torch.float32, False)
+                if a.xe is not None and a.xe.dtype != torch.float32:
+                    a.xe = a.xe.float()
+                if alsig is _DEV:
+                    if co is None or co.dev is None:
+                        raise RuntimeError("device-side scalars need the coefficient block of the consuming launch")
+                    a.coef_dev = co.dev
+                e = be.step(_guidance_args(a, None, raw))[0]
+                raw = RawOutput(e, None, PARAM_NOISE, 1.0)
+            else:
+                a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
+                             guidance=raw.guidance, state_dtype=torch.float32, raw_round=code)
+                e = be.step(_guidance_args(a, ratio, raw))[0]
+                raw = RawOutput(e, None, raw.param, 1.0)
             rr = 0
             ratio = None
         if (rr & 4) and co is not None:
@@ -576,7 +645,7 @@ class DPM_Solver:
             x_next = self._pure_update(co, x, m_new, m1, m2, rr=rr & 4 and rr, pkey=pkey if m_new is raw.e_cond else None) \
                 if co is not None else None
             return m_new, x_next
-        a = _rescale_args(self._conv_args(raw, xe, alsig, sd, x0), ratio, raw)
+        a = _guidance_args(self._conv_args(raw, xe, alsig, sd, x0), ratio, raw)
         if alsig is _DEV:
             if co is None or co.dev is None:
                 raise RuntimeError("device-side scalars need the coefficient block of the consuming launch")

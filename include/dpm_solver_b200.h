@@ -280,6 +280,23 @@ DPM_API int dpm_cfg_rescale_ratio(float* ratio_out, const void* e_cond, const vo
 DPM_API int dpm_step_rescaled(const dpm_step_desc* desc, const float* ratio, float phi, float one_minus_phi,
                               dpm_stream_t stream);
 
+/* ---- per-sample classifier-free guidance ------------------------------------------------------------------
+ * The scale of the CFG combine (:330) as a device fp32 array guidance[n/per_sample], one value per sample, in place
+ * of desc->guidance (ignored by both entries). Sample b with guidance[b] == 1 gets the reference's bypass (:323): the
+ * converted conditional output alone, with no combine and no rescale. The values are read on the device only, so a
+ * captured graph picks up new values written into the array between replays.
+ * dpm_step_guided: dpm_step with the per-sample scale; ratio NULL = plain CFG, else the guidance rescale of
+ *   dpm_step_rescaled with that ratio (from dpm_cfg_rescale_ratio_guided) and phi, one_minus_phi.
+ *   Needs desc->n_model == 2, desc->raw_round == 0, desc->per_sample != 0 dividing n and a non-NULL guidance;
+ *   DPM_ERR_ARG otherwise. Served by the direct vector kernels (tails, unaligned views and dev_coef launches by the
+ *   generic kernel); never by the TMA variant.
+ * dpm_cfg_rescale_ratio_guided: dpm_cfg_rescale_ratio with g_b = e_uncond + guidance[b]*(e_cond - e_uncond). */
+DPM_API int dpm_step_guided(const dpm_step_desc* desc, const float* guidance, const float* ratio, float phi,
+                            float one_minus_phi, dpm_stream_t stream);
+DPM_API int dpm_cfg_rescale_ratio_guided(float* ratio_out, const void* e_cond, const void* e_uncond,
+                                         const float* guidance, uint64_t per_sample, uint64_t n, int model_dtype,
+                                         void* workspace, size_t workspace_bytes, dpm_stream_t stream);
+
 /* ---- dpm_solver_adaptive with the controller on the device (:956-1010) -------------------------------------
  * Device buffers (caller-allocated, fp32): state[16] (s, lambda_s, lambda_0, h, t, nfe, done, accept, iterations as
  * int bit patterns where integral), coef[4][16] (one dpm_step_desc.dev_coef block per fused launch of an
