@@ -241,8 +241,8 @@ __device__ __forceinline__ void div_const8(float (&x)[8], float d, float r) {
   for (int i = 0; i < 8; ++i) x[i] = q[i];
 }
 __host__ __device__ __forceinline__ bool recip_div_ok(float d) {
-  // |d| within 2^-20 .. 2^20 (so that with 1e-25 < |x| < 1e30 neither the quotient nor the residual
-  // of div_const can overflow or reach the denormal range), significand not all ones
+  // |d| in [2^-20, 2^21), biased exponent 107..147 (so that with 1e-25 < |x| < 1e30 neither the quotient nor
+  // the residual of div_const can overflow or reach the denormal range), significand not all ones
 #ifdef __CUDA_ARCH__
   const uint32_t b = __float_as_uint(d);
 #else

@@ -730,6 +730,10 @@ class DPM_Solver:
 
     def noise_prediction_fn(self, x, t):
         """Return the noise prediction model (:427-431)."""
+        if self.reference_rounding:
+            # the conversion launch, so that a 16-bit CFG combine is rounded as the reference rounds it (:329-330)
+            xs = self._state(x)
+            return self._post_model(self._evaluate(xs, t), xs, t, P._cpu(t)[:1], x0=False)[0]
         return self.model(x, t)
 
     def data_prediction_fn(self, x, t):

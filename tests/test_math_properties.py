@@ -89,11 +89,13 @@ def _rn32(fr):
 
 def test_two_step_constant_division_is_correctly_rounded():
     """q0 = RN(x*r), then twice: e = x - q*d (one FMA), q = RN(q + e*r), with r = RN(1/d): equals RN(x/d) for every
-    divisor the kernels accept (recip_div_ok: |d| in 2^-20..2^20, significand not all ones). After the first
-    refinement the quotient is faithful, so the second residual is EXACT (asserted) -- the premise of Markstein's
-    theorem. Random and adversarial pairs: quotients next to rounding midpoints, divisors one ulp from a power of
-    two or from the excluded all-ones pattern."""
+    divisor the kernels accept (recip_div_ok: |d| in [2^-20, 2^21), biased exponent 107..147, significand not all
+    ones). After the first refinement the quotient is faithful, so the second residual is EXACT (asserted) -- the
+    premise of Markstein's theorem. Random and adversarial pairs over the whole admitted range: every exponent,
+    quotients next to rounding midpoints, divisors one ulp from a power of two or from the excluded all-ones pattern,
+    numerators within a few ulps of the range guard (1e-25, 1e30), there too with quotients next to a midpoint."""
     from fractions import Fraction
+    from step_edges import from_bits, nudge, recip_div_ok
     rng = np.random.default_rng(7)
     ds = []
     for _ in range(300):
@@ -101,11 +103,14 @@ def test_two_step_constant_division_is_correctly_rounded():
     for e in (-19, -3, 0, 1, 7, 18):
         base = np.float32(2.0 ** e)
         ds += [base, np.nextafter(base, np.float32(np.inf)), np.nextafter(np.nextafter(base, np.float32(0)), np.float32(0))]
+    for e in range(-20, 21):                          # biased exponents 107..147
+        all_ones = from_bits(((e + 127) << 23) | 0x7fffff)
+        ds += [np.float32(rng.uniform(1.0, 2.0) * 2.0 ** e), nudge(all_ones, -1), nudge(all_ones, 1),
+               from_bits((e + 127) << 23)]
     checked = 0
     for d in ds:
-        bits = int(np.float32(d).view(np.uint32))
-        if (bits & 0x7fffff) == 0x7fffff:
-            continue                                  # excluded on the host (IEEE path)
+        if not recip_div_ok(d):
+            continue                                  # refused on the host (IEEE path)
         d = np.float32(d)
         r = np.float32(1.0) / d                       # numpy's fp32 division is correctly rounded
         assert _rn32(Fraction(1) / Fraction(float(d))) == r
@@ -115,6 +120,14 @@ def test_two_step_constant_division_is_correctly_rounded():
             mid = (Fraction(float(q)) + Fraction(float(np.nextafter(q, np.float32(np.inf))))) / 2
             x0 = _rn32(mid * Fraction(float(d)))
             xs += [x0, np.nextafter(x0, np.float32(np.inf)), np.nextafter(x0, np.float32(-np.inf))]
+        for g in (1e-25, 1e30):                       # at the guard: x a few ulps from it, and midpoint quotients
+            xs += [nudge(g, k) for k in range(-3, 4)]
+            q = _rn32(Fraction(float(np.float32(g))) / Fraction(float(d)))
+            for k in (-1, 0, 1):
+                qk = nudge(q, k)
+                mid = (Fraction(float(qk)) + Fraction(float(np.nextafter(qk, np.float32(np.inf))))) / 2
+                x0 = _rn32(mid * Fraction(float(d)))
+                xs += [x0, nudge(x0, 1), nudge(x0, -1)]
         for x in xs:
             x = np.float32(x) * np.float32(rng.choice([-1.0, 1.0]))
             if not (1e-25 < abs(float(x)) < 1e30):
