@@ -47,6 +47,7 @@ class AdaptiveCtl(C.Structure):
         ("discrete_time_input", C.c_int32), ("order", C.c_int32), ("predict_x0", C.c_int32), ("taylor", C.c_int32),
         ("t_0", C.c_float), ("theta", C.c_float), ("t_err", C.c_float),
         ("state", C.c_void_p), ("coef", C.c_void_p), ("times", C.c_void_p), ("error", C.c_void_p),
+        ("beta_0_sq", C.c_float),
     ]
 
 

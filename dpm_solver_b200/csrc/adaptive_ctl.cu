@@ -17,10 +17,14 @@
 // The host enqueues a fixed-length chunk of iterations and reads `done`/`nfe` back once per chunk. After `done`
 // the plan kernel emits identity coefficients at t_0, so the surplus iterations of a chunk leave x untouched.
 //
-// Schedule scalars use correctly rounded exp/log/expm1 (fp64, rounded once); the host's differ in the last ulp of
-// some arguments: results
-// agree with the reference to the north-star tolerance (like the reference itself run on CUDA vs CPU), the
-// accept/reject sequence -- hence NFE -- is identical unless E lands within ~1e-6 of 1 (tests/test_adaptive.py).
+// Contract: the reference's fp32 operation order (plan.py / schedule.py and the host controller's update), with
+// exp/log/expm1/log1p evaluated in fp64 and rounded once -- correctly rounded fp32 -- and float_power(E, -1/order)
+// rounded to fp64 and then to fp32 as the reference does. tests/adaptive_oracle.py evaluates exactly that (mpmath
+// for the transcendentals) and tests/test_gpu_adaptive_controller.py requires every word these kernels write to be
+// bit-identical to it; only where the exact value lies within the fp64 libm's error (1 ulp, 2 for pow) of an fp32
+// rounding boundary is either neighbour accepted. The host's fp32 libm differs in the last ulp of some arguments,
+// so end to end the sample agrees with the reference to the north-star tolerance and the accept/reject sequence --
+// hence NFE -- is identical unless E lands within ~1e-6 of 1 (tests/test_adaptive.py).
 #include <math.h>
 
 #include "common.cuh"
@@ -37,6 +41,7 @@ struct SchedDev {
   const float* la_f;       // [K] flipped log alpha (ascending)
   const float* t_f;        // [K] flipped t
   float beta_0, beta_d;    // linear: beta_0, fl(beta_1 - beta_0)
+  float beta_0_sq;         // linear: fl(beta_0**2), squared in double like the reference's python float (:162)
   float inv_N;             // fl(1 / total_N) (model-input time of discrete-time networks :278)
   int32_t discrete_input;  // 1: network takes (t - 1/N)*1000, 0: t itself
 };
@@ -86,7 +91,7 @@ __device__ float log_alpha_of(const SchedDev& ns, float t) {
 __device__ float inverse_lambda(const SchedDev& ns, float lamb) {
   if (ns.kind == 1) {                                                            // :161-163
     const float tmp = (2.f * ns.beta_d) * logaddexp0(-2.f * lamb);
-    const float Delta = ns.beta_0 * ns.beta_0 + tmp;
+    const float Delta = ns.beta_0_sq + tmp;
     return tmp / (sqrtf(Delta) + ns.beta_0) / ns.beta_d;
   }
   const float la = -0.5f * logaddexp0(-2.f * lamb);                             // :165
@@ -215,9 +220,12 @@ __global__ void k_adapt_decide(const AdaptCfg c) {
     st[ST_LAM_S] = marg(c.ns, st[ST_T]).lam;
   }
   // h = min(theta * h * float_power(E, -1/order).float(), lambda_0 - lambda_s)   :1007
+  // torch.min propagates NaN (E = 0 with h = 0 gives 0 * inf): fminf would drop it and jump to lambda_0 - lambda_s
   const float grow = (float)pow((double)E, -1.0 / (double)c.order);
-  st[ST_H] = fminf((c.theta * st[ST_H]) * grow, st[ST_LAM_0] - st[ST_LAM_S]);
+  const float h = min_nan((c.theta * st[ST_H]) * grow, st[ST_LAM_0] - st[ST_LAM_S]);
+  st[ST_H] = h;
   st[ST_NFE] = __int_as_float(__float_as_int(st[ST_NFE]) + c.order);           // :1008
+  if (h != h) st[ST_DONE] = __int_as_float(2);   // NaN step: every later estimate is NaN, stop now, the host raises
   if (fabsf(st[ST_S] - c.t_0) <= c.t_err) st[ST_DONE] = __int_as_float(1);     // while |s - t_0| > t_err :983
 }
 
@@ -252,7 +260,8 @@ static int fill_cfg(AdaptCfg* c, const dpm_adaptive_ctl* a) {
   memset(c, 0, sizeof(*c));
   c->ns.kind = a->schedule_kind; c->ns.K = a->table_len;
   c->ns.t = a->t_array; c->ns.la = a->log_alpha_array; c->ns.la_f = a->log_alpha_flipped; c->ns.t_f = a->t_flipped;
-  c->ns.beta_0 = a->beta_0; c->ns.beta_d = a->beta_1_minus_beta_0; c->ns.inv_N = a->inv_total_N;
+  c->ns.beta_0 = a->beta_0; c->ns.beta_d = a->beta_1_minus_beta_0; c->ns.beta_0_sq = a->beta_0_sq;
+  c->ns.inv_N = a->inv_total_N;
   c->ns.discrete_input = a->discrete_time_input;
   c->order = a->order; c->pp = a->predict_x0; c->taylor = a->taylor;
   c->t_0 = a->t_0; c->theta = a->theta; c->t_err = a->t_err;

@@ -264,6 +264,10 @@ __device__ __forceinline__ float clamp_sym(float x0, float s) {
 __device__ __forceinline__ float max_nan(float a, float b) {
   return (a != a) ? a : ((b != b) ? b : fmaxf(a, b));
 }
+// torch.min(a, b) / torch.minimum: NaN wins; otherwise std::min's `b < a ? b : a`
+__device__ __forceinline__ float min_nan(float a, float b) {
+  return (a != a) ? a : ((b != b) ? b : (b < a ? b : a));
+}
 // model_wrapper.noise_pred_fn :288-298
 __device__ __forceinline__ float convert_param(int param, float out, float xe, float alpha,
                                                float sigma) {

@@ -416,6 +416,7 @@ class AdaptiveController:
         else:
             c.schedule_kind, c.table_len = 1, 0
             c.beta_0, c.beta_1_minus_beta_0 = ns.beta_0, ns.beta_1 - ns.beta_0
+            c.beta_0_sq = ns.beta_0 ** 2          # squared in double, rounded once (inverse_lambda :162)
             c.inv_total_N = 1. / ns.total_N
         c.discrete_time_input = int(bool(discrete_input))
         c.order, c.predict_x0, c.taylor = order, int(bool(predict_x0)), int(bool(taylor))

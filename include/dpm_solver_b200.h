@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 100 /* 0.1.0 */
+#define DPM_B200_VERSION 101 /* 0.1.1: dpm_adaptive_ctl.beta_0_sq */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -330,6 +330,7 @@ typedef struct dpm_adaptive_ctl {
   float* coef;                 /* device [4][16] */
   float* times;                /* device [6] */
   const float* error;          /* device [1] */
+  float beta_0_sq;             /* linear: fl32(beta_0**2) with the square taken in double (reference :162) */
 } dpm_adaptive_ctl;
 
 DPM_API int dpm_adaptive_init(const dpm_adaptive_ctl* ctl, float t_T, float h_init, dpm_stream_t stream);

@@ -21,7 +21,9 @@ def test_header_declares_the_expected_entry_points():
         assert s in syms
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_the_declared_symbols_and_version():
+    """Every declared symbol is exported and bound, and dpm_version() is the header's DPM_B200_VERSION -- at least
+    101, the first version whose dpm_adaptive_ctl carries beta_0_sq (a caller built against 100 leaves it unset)."""
     from dpm_solver_b200 import _lib
     from dpm_solver_b200.build import build
     build()
@@ -29,8 +31,10 @@ def test_library_exports_every_declared_symbol():
     for s in declared_symbols():
         assert hasattr(handle, s), s
     assert set(declared_symbols()) == set(_lib.PROTOTYPES)
+    src = open(os.path.join(ROOT, "include", "dpm_solver_b200.h")).read()
+    header_version = int(re.search(r"#define\s+DPM_B200_VERSION\s+(\d+)", src).group(1))
     L = _lib.lib()
-    assert L.dpm_version() == 100
+    assert L.dpm_version() == header_version >= 101
 
 
 def test_argument_validation_needs_no_gpu():
