@@ -86,7 +86,11 @@ PROTOTYPES = {
     "dpm_step_rescaled": (C.c_int, [C.POINTER(StepDesc), _vp, _f, _f, _vp]),
     "dpm_step_guided": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _f, _f, _vp]),
     "dpm_cfg_rescale_ratio_guided": (C.c_int, [_vp, _vp, _vp, _vp, _u64, _u64, _i, _vp, C.c_size_t, _vp]),
+    "dpm_step_multi": (C.c_int, [C.POINTER(StepDesc), C.POINTER(_vp), C.POINTER(_f), _i, C.POINTER(_vp), _vp]),
+    "dpm_replicate": (C.c_int, [_vp, _vp, _u64, _i, _i, _vp]),
 }
+
+MAX_CONDITIONS = 4      # DPM_MAX_CONDITIONS
 
 _lib = None
 

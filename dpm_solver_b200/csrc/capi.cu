@@ -253,6 +253,63 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale*
   return finish(rc);
 }
 
+// multi-condition guidance: the tensors of MultiParams beyond KParams, shifted like `shifted`
+static MultiParams shifted_multi(const MultiParams& mp, uint64_t elems) {
+  MultiParams t = mp;
+  t.k = shifted(mp.k, elems);
+  for (int k = 0; k < mp.n_cond; ++k) {
+    t.ec[k] = off(mp.ec[k], mp.k.model_dtype, elems);
+    t.rep[k] = off(mp.rep[k], mp.k.state_dtype, elems);
+  }
+  return t;
+}
+
+static int step_multi_impl(const dpm_step_desc* desc, const void* const* e_conds, const float* scales, int n_cond,
+                           void* const* replicas, cudaStream_t stream) {
+  if (desc == nullptr || e_conds == nullptr || scales == nullptr || n_cond < 2 || n_cond > kMaxCond ||
+      desc->n_model != 2 || desc->raw_round != 0) {
+    set_error("multi-condition step: needs desc, e_conds, scales, 2 <= n_cond <= %d, n_model == 2 and raw_round == 0",
+              kMaxCond);
+    return DPM_ERR_ARG;
+  }
+  for (int k = 0; k < n_cond; ++k) {
+    if (e_conds[k] == nullptr || (replicas != nullptr && replicas[k] == nullptr)) {
+      set_error("multi-condition step: conditional output or replica %d is NULL", k);
+      return DPM_ERR_ARG;
+    }
+  }
+  if (desc->n == 0) return DPM_OK;
+  dpm_step_desc d = *desc;
+  d.e_cond = e_conds[0];   // (checked for NULL by build_params like any conditional output; the kernels read mp.ec)
+  d.out2 = nullptr;
+  MultiParams mp;
+  memset(&mp, 0, sizeof(mp));
+  Needs nd;
+  int rc = build_params(&d, &mp.k, &nd, false);
+  if (rc != DPM_OK) return rc;
+  mp.n_cond = n_cond;
+  bool aligned_all = all_aligned(mp.k, nd);
+  for (int k = 0; k < n_cond; ++k) {
+    mp.ec[k] = e_conds[k];
+    mp.s[k] = scales[k];
+    mp.rep[k] = (replicas != nullptr && d.form != DPM_FORM_NONE) ? replicas[k] : nullptr;
+    aligned_all = aligned_all && aligned(mp.ec[k], d.model_dtype) && (mp.rep[k] == nullptr || aligned(mp.rep[k], d.state_dtype));
+  }
+  Tuning t{g_variant.load(), g_threads.load(), g_ctas.load()};
+  bool body_done = false;
+  if (mp.k.npk > 0 && aligned_all && mp.k.dev_coef == nullptr) {   // device-side scalars: generic kernel only
+    const int r = launch_step_multi(mp, t, stream);
+    if (r < 0 || r > 1) return r;
+    body_done = (r == 0);
+  }
+  if (!body_done) {
+    rc = launch_step_multi_scalar(mp, stream);
+  } else if (mp.k.n % kPacket) {
+    rc = launch_step_multi_scalar(shifted_multi(mp, (uint64_t)mp.k.npk * kPacket), stream);   // tail
+  }
+  return finish(rc);
+}
+
 }  // namespace dpm
 
 using namespace dpm;
@@ -411,6 +468,29 @@ int dpm_duplicate(void* out, const void* x, uint64_t n, int dtype, dpm_stream_t 
     cudaError_t e = cudaMemcpyAsync(out, x, bytes, cudaMemcpyDeviceToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(static_cast<char*>(out) + bytes, x, bytes, cudaMemcpyDeviceToDevice, st);
     return e != cudaSuccess ? launch_error("duplicate", e) : DPM_OK;
+  }
+  return finish(r);
+}
+
+int dpm_step_multi(const dpm_step_desc* desc, const void* const* e_conds, const float* scales, int n_cond,
+                   void* const* replicas, dpm_stream_t stream) {
+  return step_multi_impl(desc, e_conds, scales, n_cond, replicas, static_cast<cudaStream_t>(stream));
+}
+
+int dpm_replicate(void* out, const void* x, uint64_t n, int copies, int dtype, dpm_stream_t stream) {
+  if (copies < 1 || out == nullptr || x == nullptr || !valid_dtype(dtype)) {
+    set_error("replicate: NULL tensor, bad dtype or copies < 1");
+    return DPM_ERR_ARG;
+  }
+  if (n == 0) return DPM_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const uint64_t bytes = n * (uint64_t)esize(dtype);
+  int r = launch_replicate(out, x, bytes, copies, st);
+  if (r == 1) {   // unaligned views: plain device-to-device copies
+    cudaError_t e = cudaSuccess;
+    for (int c = 0; c < copies && e == cudaSuccess; ++c)
+      e = cudaMemcpyAsync(static_cast<char*>(out) + (uint64_t)c * bytes, x, bytes, cudaMemcpyDeviceToDevice, st);
+    return e != cudaSuccess ? launch_error("replicate", e) : DPM_OK;
   }
   return finish(r);
 }

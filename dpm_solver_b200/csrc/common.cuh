@@ -66,6 +66,19 @@ struct KParams {
   const float* gscale;
 };
 
+// multi-condition classifier-free guidance (dpm_step_multi): eps = eps_u; eps = eps + s[k]*(eps_k - eps_u) for k < n_cond,
+// each output converted by the parameterisation first. `k.eu` is the unconditional output; `k.ec` and `k.out2` are not
+// read. rep[k] (optional) receives x_t again: block k + 1 of the [(n_cond + 1)B, ...] network input. KParams itself is
+// left as it is, so the kernels that take it keep their code.
+constexpr int kMaxCond = DPM_MAX_CONDITIONS;
+struct MultiParams {
+  KParams k;
+  const void* ec[kMaxCond];
+  void* rep[kMaxCond];
+  float s[kMaxCond];
+  int32_t n_cond;
+};
+
 // ---- storage types ------------------------------------------------------------------------
 template <typename T> struct Raw;  // one packet as loaded (still packed)
 template <> struct Raw<float> { uint32_t r[8]; };

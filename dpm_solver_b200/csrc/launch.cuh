@@ -116,6 +116,9 @@ int launch_adaptive_plan(const dpm_adaptive_ctl* a, cudaStream_t stream);
 int launch_adaptive_decide(const dpm_adaptive_ctl* a, cudaStream_t stream);
 int launch_select_copy(void* dst, const void* src, const float* state, uint64_t bytes, cudaStream_t stream);
 int launch_duplicate(void* dst, const void* src, uint64_t bytes, cudaStream_t stream);
+int launch_step_multi(const MultiParams& mp, const Tuning& t, cudaStream_t stream);
+int launch_step_multi_scalar(const MultiParams& mp, cudaStream_t stream);
+int launch_replicate(void* dst, const void* src, uint64_t bytes, int copies, cudaStream_t stream);
 int launch_quantile(float* s_out, const KParams& p, uint64_t n_samples, float q, float max_val,
                     void* workspace, size_t workspace_bytes, cudaStream_t stream);
 size_t quantile_workspace_bytes(uint64_t n_samples, uint64_t per_sample);

@@ -63,6 +63,12 @@ class StepArgs:
     # per-sample classifier-free guidance (dpm_step_guided; n_model == 2, per_sample set): fp32 [B] on the device, in
     # place of `guidance`. With `ratio` the step is also rescaled.
     guidance_b: Optional[torch.Tensor] = None
+    # multi-condition classifier-free guidance (dpm_step_multi; n_model == 2): the K >= 2 conditional outputs, in place
+    # of `e_cond` (which holds the first of them), their K fp32-rounded python-float scales, in place of `guidance`, and
+    # optionally K tensors that receive x_t again (blocks 1..K of the next network input; `out2` is not used)
+    e_conds: Optional[Tuple[torch.Tensor, ...]] = None
+    scales: Optional[Tuple[float, ...]] = None
+    replicas: Optional[Tuple[torch.Tensor, ...]] = None
 
     def state_tensors(self):
         return [t for t in (self.x, self.xe, self.m0, self.m1, self.m2) if t is not None]
@@ -214,7 +220,9 @@ class CudaBackend:
                 raise TypeError(f"dpm_solver_b200: `{what}` must be a contiguous fp32 tensor on the tensors' device")
             if a.per_sample <= 0 or ref.numel() % a.per_sample or v.numel() != ref.numel() // a.per_sample:
                 raise ValueError(f"dpm_solver_b200: `{what}` needs one value per sample")
-        if a.guidance_b is not None:
+        if a.e_conds is not None:
+            self._step_multi(a, d, ref, sdt, layout, keep)
+        elif a.guidance_b is not None:
             # (phi and 1 - phi as below; ignored without a ratio)
             self._launch(ref.device, self._lib.dpm_step_guided, C.byref(d), C.c_void_p(a.guidance_b.data_ptr()),
                          C.c_void_p(None if a.ratio is None else a.ratio.data_ptr()), C.c_float(a.phi),
@@ -226,6 +234,46 @@ class CudaBackend:
         else:
             self._launch(ref.device, self._lib.dpm_step, C.byref(d))
         return m_out, out
+
+    def _step_multi(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
+        """dpm_step_multi: the K conditional outputs and scales of a multi-condition CFG step (d already filled)."""
+        K = len(a.e_conds)
+        if not 2 <= K <= _lib.MAX_CONDITIONS or a.scales is None or len(a.scales) != K or a.n_model != 2:
+            raise ValueError("dpm_solver_b200: a multi-condition step takes 2..{} conditional outputs, one scale each, "
+                             "and n_model == 2".format(_lib.MAX_CONDITIONS))
+        if a.replicas is not None and len(a.replicas) != K:
+            raise ValueError("dpm_solver_b200: a multi-condition step takes one replica per condition")
+        n, mdt = ref.numel(), a.e_cond.dtype
+        ecs = [self._check(e, "e_conds[%d]" % k, ref.device, n, mdt, layout) for k, e in enumerate(a.e_conds)]
+        keep.extend(ecs)
+        reps = None
+        if a.replicas is not None and a.form != FORM_NONE:
+            for k, r in enumerate(a.replicas):
+                self._check(r, "replicas[%d]" % k, ref.device, n, sdt)
+                if self._layout(r) != layout:
+                    raise ValueError("dpm_solver_b200: replicas must be dense and laid out like out")
+            reps = (C.c_void_p * K)(*[r.data_ptr() for r in a.replicas])
+        d.out2 = None
+        self._launch(ref.device, self._lib.dpm_step_multi, C.byref(d),
+                     (C.c_void_p * K)(*[e.data_ptr() for e in ecs]), (C.c_float * K)(*a.scales), C.c_int(K), reps)
+
+    def replicate(self, x: torch.Tensor, copies: int) -> torch.Tensor:
+        """torch.cat([x] * copies) -- one read, `copies` writes (dpm_replicate); layout of x kept."""
+        if x.dtype not in _DTYPE_CODE:
+            raise TypeError(f"dpm_solver_b200: unsupported dtype {x.dtype} for replicate")
+        layout = self._layout(x)
+        if layout is None:
+            x, layout = x.contiguous(), "c"
+        shape = (copies * x.shape[0],) + tuple(x.shape[1:])
+        if layout == "cl":
+            out = torch.empty(shape, dtype=x.dtype, device=x.device,
+                              memory_format=torch.channels_last if x.dim() == 4 else torch.channels_last_3d)
+        else:
+            out = torch.empty(shape, dtype=x.dtype, device=x.device)
+        self._check(x, "x", x.device, x.numel(), layout=layout)
+        self._launch(x.device, self._lib.dpm_replicate, C.c_void_p(out.data_ptr()), C.c_void_p(x.data_ptr()),
+                     C.c_uint64(x.numel()), C.c_int(copies), C.c_int(_DTYPE_CODE[x.dtype]))
+        return out
 
     def cfg_rescale_ratio(self, e_cond: torch.Tensor, e_uncond: torch.Tensor, guidance) -> torch.Tensor:
         """Per-sample r = std(e_cond_b) / std(g_b), g = e_uncond + guidance*(e_cond - e_uncond), as fp32 [B] on the
@@ -273,9 +321,9 @@ class CudaBackend:
         """Per-sample s_b = max(quantile(|x0_b|, q), max_val) -> fp32 [B].
         return_stats=True also returns the pipeline's per-sample header words (int32 [B, 8]:
         lo key, hi key, #below, #inside, path (1 bracket / 2 exact fallback), ...) for diagnostics."""
-        if a.guidance_b is not None:
+        if a.guidance_b is not None or a.e_conds is not None:
             raise ValueError("dpm_solver_b200: the quantile takes one guidance scale; materialise a per-sample "
-                             "combine first")
+                             "or multi-condition combine first")
         d, keep, ref, _, _ = self._fill(a)
         if a.per_sample <= 0 or ref.numel() % a.per_sample:
             raise ValueError("dpm_solver_b200: per_sample must divide numel")
@@ -472,9 +520,9 @@ class PreparedStep:
     @staticmethod
     def build(be: "CudaBackend", a: StepArgs) -> Optional["PreparedStep"]:
         if a.thr is not None or a.raw_round or a.ratio is not None or a.guidance_b is not None \
-                or a.out is not None and a.out2 is None:
+                or a.e_conds is not None or a.out is not None and a.out2 is None:
             # (a rescaled step reads a fresh ratio tensor every evaluation, a guided one a scales tensor the
-            # descriptor does not carry: never frozen)
+            # descriptor does not carry, a multi-condition one K outputs and scales it does not carry: never frozen)
             return None
         ref = a.reference_tensor()
         if not ref.is_contiguous():

@@ -48,6 +48,37 @@ class RawOutput:
     guidance: float
     phi: float = 0.0        # guidance rescale of the combine (model_wrapper's guidance_rescale); 0 = off
     guidance_b: Optional[torch.Tensor] = None   # per-sample scales, fp32 [B] (then `guidance` is not read)
+    # multi-condition guidance (K >= 2 conditions): the K conditional outputs in condition order (`e_cond` is the first)
+    # and their fp32-rounded scales; `guidance` is then not read
+    e_conds: Optional[tuple] = None
+    scales: Optional[tuple] = None
+
+
+def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale):
+    """model_wrapper's list or tuple of conditions -> (condition, guidance_scale, per-condition scales or None).
+    One condition is the tensor form (its scale as one python float); K >= 2 conditions keep their K scales, each read
+    on the host once and rounded to fp32 once."""
+    K = len(condition)
+    if not 1 <= K <= ops._lib.MAX_CONDITIONS:
+        raise ValueError("classifier-free guidance takes 1 to {} conditions, got {}".format(ops._lib.MAX_CONDITIONS, K))
+    s = guidance_scale
+    if not isinstance(s, (list, tuple)) and not (torch.is_tensor(s) and s.dim() >= 1):
+        raise ValueError("a list of {} conditions needs a list, tuple or 1-D tensor of {} guidance scales, got a "
+                         "single scale".format(K, K))
+    s = torch.as_tensor(s.detach().cpu() if torch.is_tensor(s) else list(s), dtype=torch.float32)
+    if s.dim() != 1:
+        raise ValueError("a list of conditions takes one guidance scale per condition (shape [{}]); per-sample scales "
+                         "are not available with several conditions, got shape {}".format(K, tuple(s.shape)))
+    if s.numel() != K:
+        raise ValueError("{} guidance scales for {} conditions".format(s.numel(), K))
+    scales = tuple(s.tolist())
+    if K == 1:
+        return condition[0], scales[0], None
+    if unconditional_condition is None:
+        raise ValueError("classifier-free guidance with {} conditions needs an unconditional_condition".format(K))
+    if guidance_rescale != 0:
+        raise ValueError("guidance_rescale is not available with several conditions")
+    return tuple(condition), scales, scales
 
 
 def _cfg_ratio(be, raw: RawOutput) -> Optional[torch.Tensor]:
@@ -67,6 +98,9 @@ def _guidance_args(a: StepArgs, ratio: Optional[torch.Tensor], raw: RawOutput, r
         a.ratio, a.phi = ratio, raw.phi
     if raw.guidance_b is not None and a.n_model == 2:
         a.guidance_b = raw.guidance_b if rows is None else raw.guidance_b[rows]
+    if raw.e_conds is not None and a.n_model == 2:
+        a.e_conds = raw.e_conds if rows is None else tuple(e[rows] for e in raw.e_conds)
+        a.scales = raw.scales
     if a.ratio is not None or a.guidance_b is not None:
         a.per_sample = a.e_cond.numel() // a.e_cond.shape[0]
     return a
@@ -100,15 +134,19 @@ class WrappedModel:
         self.model_type = model_type
         self.model_kwargs = model_kwargs
         self.guidance_type = guidance_type
+        self.cond_scales = None     # K >= 2 conditions: their K scales (python floats, fp32-rounded)
+        if guidance_type == "classifier-free" and isinstance(condition, (list, tuple)):
+            condition, guidance_scale, self.cond_scales = _multi_condition(
+                condition, unconditional_condition, guidance_scale, guidance_rescale)
         self.condition = condition
         self.unconditional_condition = unconditional_condition
-        if isinstance(guidance_scale, (list, tuple)):
+        if isinstance(guidance_scale, (list, tuple)) and self.cond_scales is None:
             guidance_scale = torch.tensor(list(guidance_scale), dtype=torch.float32)   # each value rounded once
         self.guidance_scale = guidance_scale
         self.classifier_fn = classifier_fn
         self.classifier_kwargs = classifier_kwargs
         self._c_in = None
-        self._scale_vec = _scale_vector(guidance_scale, guidance_type)
+        self._scale_vec = None if self.cond_scales is not None else _scale_vector(guidance_scale, guidance_type)
         self._gs = None
 
     # -- pieces of the reference closure ----------------------------------------------------
@@ -131,9 +169,21 @@ class WrappedModel:
         return self._scale_vec is not None and self.guidance_type == "classifier-free"
 
     @property
+    def n_cond(self) -> int:
+        """Number of conditions of a multi-condition run (K >= 2), else 0."""
+        return 0 if self.cond_scales is None else len(self.cond_scales)
+
+    @property
     def uses_cfg(self) -> bool:
+        # (several conditions: guidance_scale is their tuple of scales, never equal to 1 -- always combined, no bypass)
         return (self.guidance_type == "classifier-free" and self.unconditional_condition is not None
                 and (self._scale_vec is not None or self.guidance_scale != 1.))
+
+    def input_copies(self) -> int:
+        """How many copies of x the network input holds: K + 1 with K >= 2 conditions, 2 under CFG (:326), else 1."""
+        if self.cond_scales is not None:
+            return len(self.cond_scales) + 1
+        return 2 if self.uses_cfg else 1
 
     def _scales(self, x) -> torch.Tensor:
         """The per-sample scales as the kernels read them: fp32 [B] on x's device. A contiguous fp32 tensor already
@@ -156,12 +206,19 @@ class WrappedModel:
         return self.guidance_type != "classifier"
 
     def input_rows(self, batch: int) -> int:
-        """Length of the time vector the network receives for a batch (doubled under CFG :327)."""
-        return 2 * batch if self.uses_cfg else batch
+        """Length of the time vector the network receives for a batch (doubled under CFG :327, (K+1)-fold with K >= 2
+        conditions)."""
+        return self.input_copies() * batch
 
     def _cond_in(self):
-        """cat([unconditional_condition, condition]) (:328); constant over a run, so built once."""
+        """cat([unconditional_condition, condition]) (:328), or cat([uc, c1, ..., cK]) with several conditions;
+        constant over a run, so built once."""
         uc, c = self.unconditional_condition, self.condition
+        if self.cond_scales is not None:
+            key = tuple((id(v), getattr(v, "_version", 0)) for v in (uc,) + c)
+            if self._c_in is None or self._c_in[0] != key:
+                self._c_in = (key, torch.cat([uc, *c]), (uc, c))
+            return self._c_in[1]
         key = (id(uc), getattr(uc, "_version", 0), id(c), getattr(c, "_version", 0))
         if self._c_in is None or self._c_in[0] != key:
             # the pair is kept alive next to the key so that neither id can be recycled
@@ -176,6 +233,13 @@ class WrappedModel:
         param = PARAM_BY_NAME[self.model_type]
         if self.guidance_type == "uncond":
             return RawOutput(self._call_model(x, t_continuous, t_input=t_input), None, param, 1.0)
+        if self.guidance_type == "classifier-free" and self.cond_scales is not None:
+            n = len(self.cond_scales) + 1
+            if x_in is None:
+                x_in = ops.backend().replicate(x, n)              # cat([x] * (K+1)) (the solver hands over a prebuilt one)
+            t_in = None if t_input is not None else torch.cat([t_continuous] * n)
+            outs = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(n)   # uncond first
+            return RawOutput(outs[1], outs[0], param, 1.0, e_conds=tuple(outs[1:]), scales=self.cond_scales)
         if self.guidance_type == "classifier-free":
             gb = self._scales(x) if self._scale_vec is not None else None     # (checked before the network runs)
             if not self.uses_cfg:
@@ -268,7 +332,16 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     guidance_scale=float(s[b]), each scale rounded to fp32 once; a row with s[b] == 1 gets the conditional output alone,
     as the reference's bypass does, although the network still sees the doubled batch. A contiguous fp32 tensor on
     x's device is read in place by the kernels (a captured graph sees values written into it); other forms are
-    converted once and cached. A python number, a 0-dim or a one-element tensor is one scale, as before."""
+    converted once and cached. A python number, a 0-dim or a one-element tensor is one scale, as before.
+
+    condition (classifier-free guidance) may also be a list or tuple of K conditions, 1 <= K <= 4 (composable prompts,
+    Liu et al. 2022; not in the reference, whose cat([uc, c]) refuses a list). guidance_scale then holds exactly K
+    scales (a list, tuple or 1-D tensor), read on the host once here and rounded to fp32 once. The network runs once
+    per evaluation on cat([x] * (K+1)) with cat([uc, c1, ..., cK]); every output block is converted by the
+    parameterisation, then eps = eps_u + s1*(eps_1 - eps_u) + ... + sK*(eps_K - eps_u), left to right in fp32, as
+    torch's eager ops compute it. Every output is combined, whatever the scales (no bypass). One condition in a list is
+    exactly the tensor form. With K >= 2: unconditional_condition is required, and guidance_rescale, per-sample scales
+    and DPM_Solver(reference_rounding=True) are not available (ValueError)."""
     assert model_type in ["noise", "x_start", "v", "score"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
     guidance_rescale = float(guidance_rescale)
@@ -346,6 +419,8 @@ class DPM_Solver:
             raise ValueError("guidance_rescale is not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "per_sample_guidance", False):
             raise ValueError("a per-sample guidance_scale is not available with reference_rounding=True")
+        if self.reference_rounding and getattr(model_fn, "n_cond", 0) >= 2:
+            raise ValueError("several conditions are not available with reference_rounding=True")
         self._rr_run = 0     # raw_round of the buffered values of the run in flight (reference_rounding)
         self._prep_cache = {}   # frozen launch descriptors of cached plan steps (ops.PreparedStep)
         self._prep_on = False
@@ -431,19 +506,22 @@ class DPM_Solver:
         return RawOutput(self.model(x, t_dev), None, PARAM_NOISE, 1.0)
 
     def _dup_target(self, x):
-        """Under CFG the network consumes cat([x]*2) (:326). When nothing can touch x between the
-        update and the next evaluation, the update kernel writes x_t straight into both halves of a
-        [2B, ...] buffer: returns (x_in, first half, second half) or None."""
+        """Under CFG the network consumes cat([x]*2) (:326), cat([x]*(K+1)) with K >= 2 conditions. When nothing can
+        touch x between the update and the next evaluation, the update kernel writes x_t straight into every block of
+        a [copies*B, ...] buffer: returns (x_in, block 0, block 1, ...) or None."""
         w = self._wrapped
         if self.correcting_xt_fn is not None or not (isinstance(w, WrappedModel) and w.fusable and w.uses_cfg):
             return None
-        shape = (2 * x.shape[0],) + tuple(x.shape[1:])
+        B, n = x.shape[0], 2 if w.cond_scales is None else len(w.cond_scales) + 1
+        shape = (n * B,) + tuple(x.shape[1:])
         if ops.CudaBackend._layout(x) == "cl":      # keep a channels_last network's layout
             x_in = torch.empty(shape, dtype=x.dtype, device=x.device,
                                memory_format=torch.channels_last if x.dim() == 4 else torch.channels_last_3d)
         else:
             x_in = torch.empty(shape, dtype=x.dtype, device=x.device)
-        return x_in, x_in[:x.shape[0]], x_in[x.shape[0]:]
+        if n == 2:
+            return x_in, x_in[:B], x_in[B:]
+        return (x_in,) + tuple(x_in[i * B:(i + 1) * B] for i in range(n))
 
     _CACHE_MAX = 16
 
@@ -589,8 +667,10 @@ class DPM_Solver:
         if slot is not None and self._prep_on:
             # (phi is part of the key: a rescaled evaluation is never served by a launch frozen without the rescale)
             # (and so is a per-sample scale: a guided evaluation never meets a launch frozen with one scale)
+            # (and so are the scales of several conditions: such a step is never frozen, and a key with them cannot
+            # meet a launch frozen for one condition)
             pkey = (slot, raw.param, raw.guidance, raw.phi, raw.guidance_b is None, raw.e_uncond is None,
-                    raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out)
+                    raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, raw.scales)
             prep = self._prep_cache.get(pkey)
             if prep is not None:
                 r = prep.launch((x, xe, raw.e_cond, m1, m2, raw.e_cond, raw.e_uncond))
@@ -606,6 +686,7 @@ class DPM_Solver:
         custom_fix = x0 and self.correcting_x0_fn is not None and not self._dynamic_thresholding
         code = self._rr_code(raw)
         rr = 0
+        q_raw = None        # what the quantile reads, when not `raw` itself
         ratio = _cfg_ratio(be, raw)     # guidance rescale: one streaming pass over both halves (+2 launches)
         if code:
             # reference-rounding mode (raw 16-bit NOISE outputs, fp32 state): bits 0-1 make the fused kernel take the
@@ -615,13 +696,14 @@ class DPM_Solver:
             if not x0:
                 rr = self._rr_run = code | 4
         if raw.e_uncond is not None and x0 and self._dynamic_thresholding and (
-                code or ratio is not None or raw.guidance_b is not None):
+                code or ratio is not None or raw.guidance_b is not None or raw.e_conds is not None):
             # the quantile kernels take the plain fp32 combine with one scale: give them (and the step) the reference's
             # rounded noise, or the rescaled network output, materialised once in fp32 and then treated as one network
             # output (the parameterisation, which the quantile and the step apply, still converts it) -- or, with
             # per-sample scales and no rescale, the guided noise: each half parameterised, then combined with its
-            # sample's scale, as the reference orders it (+1 launch)
-            if ratio is None and raw.guidance_b is not None:
+            # sample's scale, as the reference orders it (+1 launch) -- or, with several conditions, their combined
+            # noise, each block parameterised first (+1 launch)
+            if ratio is None and (raw.guidance_b is not None or raw.e_conds is not None):
                 a = self._conv_args(raw, xe, alsig, torch.float32, False)
                 if a.xe is not None and a.xe.dtype != torch.float32:
                     a.xe = a.xe.float()
@@ -630,7 +712,12 @@ class DPM_Solver:
                         raise RuntimeError("device-side scalars need the coefficient block of the consuming launch")
                     a.coef_dev = co.dev
                 e = be.step(_guidance_args(a, None, raw))[0]
-                raw = RawOutput(e, None, PARAM_NOISE, 1.0)
+                if raw.e_conds is not None:
+                    # several conditions: the quantile reads the materialised noise; the step then recomputes the same
+                    # fp32 combine from the K+1 outputs, so that it can also write the K+1 blocks of the next input
+                    q_raw = RawOutput(e, None, PARAM_NOISE, 1.0)
+                else:
+                    raw = RawOutput(e, None, PARAM_NOISE, 1.0)
             else:
                 a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
                              guidance=raw.guidance, state_dtype=torch.float32, raw_round=code)
@@ -652,7 +739,11 @@ class DPM_Solver:
             a.coef_dev = co.dev
         if x0 and self._dynamic_thresholding:
             a.per_sample = xe.numel() // xe.shape[0]
-            a.thr = be.dynamic_threshold(a, float(self.dynamic_thresholding_ratio),
+            qa = a
+            if q_raw is not None:
+                qa = self._conv_args(q_raw, xe, alsig, sd, x0)
+                qa.per_sample, qa.coef_dev = a.per_sample, a.coef_dev
+            a.thr = be.dynamic_threshold(qa, float(self.dynamic_thresholding_ratio),
                                          float(self.thresholding_max_val))
         if custom_fix or co is None:
             a.form = FORM_NONE
@@ -667,11 +758,14 @@ class DPM_Solver:
         a.raw_round = rr
         dup = self._dup_target(x) if dup_out else None
         if dup is not None:
-            a.out, a.out2 = dup[1], dup[2]
+            if a.e_conds is not None:
+                a.out, a.replicas = dup[1], dup[2:]     # blocks 1..K of the next network input
+            else:
+                a.out, a.out2 = dup[1], dup[2]
         m_new, x_next = be.step(a)
         if dup is not None:
             self._xin_pair = (x_next, dup[0])
-        if pkey is not None and not a.per_sample:
+        if pkey is not None and not a.per_sample and a.e_conds is None:
             self._remember(pkey, a, dup)
         return m_new, x_next
 

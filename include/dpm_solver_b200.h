@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 101 /* 0.1.1: dpm_adaptive_ctl.beta_0_sq */
+#define DPM_B200_VERSION 102 /* 0.1.2: dpm_step_multi, dpm_replicate */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -296,6 +296,25 @@ DPM_API int dpm_step_guided(const dpm_step_desc* desc, const float* guidance, co
 DPM_API int dpm_cfg_rescale_ratio_guided(float* ratio_out, const void* e_cond, const void* e_uncond,
                                          const float* guidance, uint64_t per_sample, uint64_t n, int model_dtype,
                                          void* workspace, size_t workspace_bytes, dpm_stream_t stream);
+
+/* ---- multi-condition classifier-free guidance (composable prompts, Liu et al. 2022) ----------------------------
+ * The network runs once on cat([x] * (n_cond + 1)) with the conditions cat([uc, c_1, ..., c_n]) and returns
+ * n_cond + 1 blocks: desc->e_uncond (eps_u) and e_conds[0 .. n_cond-1]. Each block is converted by the
+ * parameterisation (:288-298), then
+ *   eps = eps_u;  eps = eps + scales[k]*(eps_k - eps_u),  k = 0 .. n_cond-1      (each op rounded to fp32)
+ * takes the place of the combined output in dpm_step (eps->x0, clamp, update). No scale is bypassed.
+ * dpm_step_multi: dpm_step with that combine; desc->n_model == 2, desc->raw_round == 0; desc->e_cond and desc->out2 are
+ *   ignored. scales: HOST array of n_cond floats, copied into the launch (capturable). replicas: NULL, or n_cond
+ *   device pointers that receive x_t again (blocks 1..n_cond of the next network input; block 0 is `out`). Returns
+ *   DPM_ERR_ARG for n_cond outside 2..DPM_MAX_CONDITIONS, raw_round != 0, n_model != 2, or a NULL output, scale array
+ *   or replica pointer, before any launch. Served by the packet kernels for the five dtype pairs (tails, unaligned
+ *   views, other pairs and dev_coef launches by the generic kernel).
+ * dpm_replicate: torch.cat([x] * copies), out holds copies*n elements; x is read once. It serves the first evaluation
+ *   of a run (inside the loop dpm_step_multi's replicas do this for free). */
+#define DPM_MAX_CONDITIONS 4
+DPM_API int dpm_step_multi(const dpm_step_desc* desc, const void* const* e_conds, const float* scales, int n_cond,
+                           void* const* replicas, dpm_stream_t stream);
+DPM_API int dpm_replicate(void* out, const void* x, uint64_t n, int copies, int dtype, dpm_stream_t stream);
 
 /* ---- dpm_solver_adaptive with the controller on the device (:956-1010) -------------------------------------
  * Device buffers (caller-allocated, fp32): state[16] (s, lambda_s, lambda_0, h, t, nfe, done, accept, iterations as
