@@ -483,8 +483,11 @@ class AdaptiveController:
 
     def select_copy(self, dst: torch.Tensor, src: torch.Tensor) -> None:
         """dst <- src iff the last decide() accepted the step."""
-        if dst.shape != src.shape or dst.dtype != src.dtype or not dst.is_contiguous() or not src.is_contiguous():
-            raise ValueError("select_copy: dense tensors of one shape and dtype")
+        if dst.shape != src.shape or dst.dtype != src.dtype or CudaBackend._layout(dst) is None:
+            raise ValueError("select_copy: tensors of one shape and dtype, the destination dense")
+        if src.stride() != dst.stride():
+            # (a channels_last network under a row-major x_T, or the reverse: the byte copy below needs dst's order)
+            src = torch.empty_like(dst).copy_(src)
         self.be._launch(self.dev, self.be._lib.dpm_select_copy, C.c_void_p(dst.data_ptr()), C.c_void_p(src.data_ptr()),
                         C.c_void_p(self.state.data_ptr()), C.c_uint64(dst.numel() * dst.element_size()))
 
@@ -520,9 +523,10 @@ class PreparedStep:
     @staticmethod
     def build(be: "CudaBackend", a: StepArgs) -> Optional["PreparedStep"]:
         if a.thr is not None or a.raw_round or a.ratio is not None or a.guidance_b is not None \
-                or a.e_conds is not None or a.out is not None and a.out2 is None:
+                or a.e_conds is not None or a.coef_dev is not None or a.out is not None and a.out2 is None:
             # (a rescaled step reads a fresh ratio tensor every evaluation, a guided one a scales tensor the
-            # descriptor does not carry, a multi-condition one K outputs and scales it does not carry: never frozen)
+            # descriptor does not carry, a multi-condition one K outputs and scales it does not carry, one with device
+            # coefficients a block the descriptor would point into without owning it: never frozen)
             return None
         ref = a.reference_tensor()
         if not ref.is_contiguous():

@@ -148,6 +148,7 @@ class WrappedModel:
         self._c_in = None
         self._scale_vec = None if self.cond_scales is not None else _scale_vector(guidance_scale, guidance_type)
         self._gs = None
+        self._gs1 = None
 
     # -- pieces of the reference closure ----------------------------------------------------
     def get_model_input_time(self, t_continuous):
@@ -173,11 +174,23 @@ class WrappedModel:
         """Number of conditions of a multi-condition run (K >= 2), else 0."""
         return 0 if self.cond_scales is None else len(self.cond_scales)
 
+    def _one_scale(self):
+        """The single guidance scale as the host reads it. A 0-dim or one-element tensor is read once per (tensor,
+        version), not at every evaluation: on the device that read is a host synchronisation, which a steady-state
+        loop must not pay and a graph capture cannot contain."""
+        s = self.guidance_scale
+        if not torch.is_tensor(s):
+            return s
+        key = (id(s), s._version)
+        if self._gs1 is None or self._gs1[0] != key:
+            self._gs1 = (key, float(s), s)          # (the tensor is kept alive so that its id cannot be recycled)
+        return self._gs1[1]
+
     @property
     def uses_cfg(self) -> bool:
         # (several conditions: guidance_scale is their tuple of scales, never equal to 1 -- always combined, no bypass)
         return (self.guidance_type == "classifier-free" and self.unconditional_condition is not None
-                and (self._scale_vec is not None or self.guidance_scale != 1.))
+                and (self._scale_vec is not None or self._one_scale() != 1.))
 
     def input_copies(self) -> int:
         """How many copies of x the network input holds: K + 1 with K >= 2 conditions, 2 under CFG (:326), else 1."""
@@ -250,7 +263,7 @@ class WrappedModel:
             out_u, out_c = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(2)  # uncond first
             if gb is not None:
                 return RawOutput(out_c, out_u, param, 1.0, self.guidance_rescale, gb)
-            return RawOutput(out_c, out_u, param, float(self.guidance_scale), self.guidance_rescale)
+            return RawOutput(out_c, out_u, param, float(self._one_scale()), self.guidance_rescale)
         raise RuntimeError("raw() is not available with classifier guidance")
 
     def _alpha_sigma(self, t_continuous):
@@ -332,7 +345,8 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     guidance_scale=float(s[b]), each scale rounded to fp32 once; a row with s[b] == 1 gets the conditional output alone,
     as the reference's bypass does, although the network still sees the doubled batch. A contiguous fp32 tensor on
     x's device is read in place by the kernels (a captured graph sees values written into it); other forms are
-    converted once and cached. A python number, a 0-dim or a one-element tensor is one scale, as before.
+    converted once and cached. A python number, a 0-dim or a one-element tensor is one scale, as before; such a tensor is
+    read on the host once per (tensor, version), so a steady-state loop does not synchronise on it.
 
     condition (classifier-free guidance) may also be a list or tuple of K conditions, 1 <= K <= 4 (composable prompts,
     Liu et al. 2022; not in the reference, whose cat([uc, c]) refuses a list). guidance_scale then holds exactly K
@@ -669,8 +683,9 @@ class DPM_Solver:
             # (and so is a per-sample scale: a guided evaluation never meets a launch frozen with one scale)
             # (and so are the scales of several conditions: such a step is never frozen, and a key with them cannot
             # meet a launch frozen for one condition)
+            # (and so is dynamic thresholding: a launch frozen without the clamp never serves a solver switched to it)
             pkey = (slot, raw.param, raw.guidance, raw.phi, raw.guidance_b is None, raw.e_uncond is None,
-                    raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, raw.scales)
+                    raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, raw.scales, self._dynamic_thresholding)
             prep = self._prep_cache.get(pkey)
             if prep is not None:
                 r = prep.launch((x, xe, raw.e_cond, m1, m2, raw.e_cond, raw.e_uncond))

@@ -277,6 +277,32 @@ def test_diffedit_corrector_matches_the_notebook_on_the_host_executor(oracle_bac
         np.testing.assert_array_equal(got.numpy(), want.numpy())
 
 
+def test_diffedit_corrector_reused_with_other_times_on_the_host_executor(oracle_backend):
+    """One corrector called again with the same step numbers at other times (another `steps` or `t_end` of the solver
+    holding it), then with another `time_fn`: (alpha, sigma) follow the time, never the step number."""
+    import adapters as A
+    import dpm_solver_b200 as new
+    mod = A.load_sd_adapter(A.reference_solver("sd"), "diffedit_ref", "cpu")
+    sampler = mod.DPMSolverSampler(A.StubLatentDiffusion("cpu"))
+    x0, x = seeded((1, 4, 16, 16), 3), seeded((1, 4, 16, 16), 4)
+    mask = (seeded((16, 16), 5) > 0).float()
+    ns = new.NoiseScheduleVP("discrete", alphas_cumprod=sampler.alphas_cumprod)
+    fused = new.DiffEditCorrector(ns, x0, mask, time_fn=lambda t: sampler.ratio_to_time(sampler.time_to_ratio(t)))
+    ref_fn = _notebook_corrector(sampler, x0, mask)
+    labels = [torch.tensor(v) for v in (0.9, 0.5, 0.05, 0.8, 0.3, 0.02)]      # kept alive, as a solver's tables are
+    for n, t in enumerate(labels + labels):
+        torch.manual_seed(200 + n)
+        want = ref_fn(x, t, n % 3)
+        torch.manual_seed(200 + n)
+        np.testing.assert_array_equal(fused(x, t, n % 3).numpy(), want.numpy())
+    fused.time_fn = None                    # the same label and step again, re-noised to the label's own level now
+    te = labels[1].reshape(1)
+    torch.manual_seed(300)
+    inter = ns.marginal_alpha(te) * x0 + ns.marginal_std(te) * torch.randn((1, *x0.shape))[0]
+    torch.manual_seed(300)
+    np.testing.assert_array_equal(fused(x, labels[1], 1).numpy(), (x * mask + (1 - mask) * inter).numpy())
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape,times", [((2, 4, 64, 64), [0.5]), ((3, 3, 17, 5), [0.3, 0.8, 0.05]), ((700, 4, 64, 64), [0.6])])
 def test_add_noise_draws_torch_randn_in_the_kernel(cuda_backend, shape, times):
