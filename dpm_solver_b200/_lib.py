@@ -15,9 +15,10 @@ LIB_PATH = _PKG / "lib" / "libdpmsolver_b200.so"
 # enums (mirror include/dpm_solver_b200.h)
 DPM_F32, DPM_BF16, DPM_F16 = 0, 1, 2
 FORM_NONE, FORM_LIN1, FORM_LIN2, FORM_LIN3, FORM_DIFF2, FORM_MS3, FORM_SS3T = range(7)
-PARAM_NOISE, PARAM_X_START, PARAM_V, PARAM_SCORE = range(4)
+PARAM_NOISE, PARAM_X_START, PARAM_V, PARAM_SCORE, PARAM_FLOW = range(5)
 
-PARAM_BY_NAME = {"noise": PARAM_NOISE, "x_start": PARAM_X_START, "v": PARAM_V, "score": PARAM_SCORE}
+PARAM_BY_NAME = {"noise": PARAM_NOISE, "x_start": PARAM_X_START, "v": PARAM_V, "score": PARAM_SCORE,
+                 "flow": PARAM_FLOW}
 
 
 class StepDesc(C.Structure):
@@ -48,6 +49,7 @@ class AdaptiveCtl(C.Structure):
         ("t_0", C.c_float), ("theta", C.c_float), ("t_err", C.c_float),
         ("state", C.c_void_p), ("coef", C.c_void_p), ("times", C.c_void_p), ("error", C.c_void_p),
         ("beta_0_sq", C.c_float),
+        ("flow_shift", C.c_float), ("flow_shift_minus_1", C.c_float), ("flow_time_scale", C.c_float),
     ]
 
 

@@ -32,9 +32,9 @@
 
 namespace dpm {
 
-// device view of NoiseScheduleVP
+// device view of NoiseScheduleVP / NoiseScheduleFlow
 struct SchedDev {
-  int32_t kind;            // 0 discrete (tables), 1 linear
+  int32_t kind;            // 0 discrete (tables), 1 linear, 2 flow
   int32_t K;               // table length
   const float* t;          // [K] ascending
   const float* la;         // [K] log alpha (descending in value)
@@ -43,7 +43,9 @@ struct SchedDev {
   float beta_0, beta_d;    // linear: beta_0, fl(beta_1 - beta_0)
   float beta_0_sq;         // linear: fl(beta_0**2), squared in double like the reference's python float (:162)
   float inv_N;             // fl(1 / total_N) (model-input time of discrete-time networks :278)
-  int32_t discrete_input;  // 1: network takes (t - 1/N)*1000, 0: t itself
+  int32_t discrete_input;  // 1: network takes (t - 1/N)*1000, 0: t itself (kinds 0 and 1)
+  float shift, shift_m1;   // flow: fl(shift), fl(shift - 1)
+  float time_scale;        // flow: the network takes time_scale * sigma_t
 };
 
 struct AdaptCfg {
@@ -88,7 +90,13 @@ __device__ float log_alpha_of(const SchedDev& ns, float t) {
   if (ns.kind == 0) return interp(ns.t, ns.la, ns.K, t);                       // :129
   return -0.25f * (t * t) * ns.beta_d - 0.5f * t * ns.beta_0;                  // :134
 }
+// NoiseScheduleFlow (schedule.py): sigma_t = (shift*t) / (1 + (shift-1)*t)
+__device__ float flow_sigma(const SchedDev& ns, float t) { return (ns.shift * t) / (1.f + ns.shift_m1 * t); }
 __device__ float inverse_lambda(const SchedDev& ns, float lamb) {
+  if (ns.kind == 2) {                                                            // NoiseScheduleFlow.inverse_lambda
+    const float sigma = 1.f / (1.f + exp_cr(lamb));
+    return sigma / (ns.shift - ns.shift_m1 * sigma);
+  }
   if (ns.kind == 1) {                                                            // :161-163
     const float tmp = (2.f * ns.beta_d) * logaddexp0(-2.f * lamb);
     const float Delta = ns.beta_0_sq + tmp;
@@ -97,15 +105,26 @@ __device__ float inverse_lambda(const SchedDev& ns, float lamb) {
   const float la = -0.5f * logaddexp0(-2.f * lamb);                             // :165
   return interp(ns.la_f, ns.t_f, ns.K, la);                                     // :166
 }
-struct Marg { float t, la, sigma, lam, alpha; };
+// alpha: exp(log alpha), as the update formulas form it (:567); alpha_e: marginal_alpha(t), what the conversion of a
+// network output takes (the same number on a VP schedule, 1 - sigma on the flow schedule)
+struct Marg { float t, la, sigma, lam, alpha, alpha_e; };
 __device__ Marg marg(const SchedDev& ns, float t) {
   Marg m;
   m.t = t;
+  if (ns.kind == 2) {                       // NoiseScheduleFlow.marginals
+    m.sigma = flow_sigma(ns, t);
+    m.alpha_e = 1.f - m.sigma;
+    m.la = log_cr(m.alpha_e);
+    m.lam = m.la - log_cr(m.sigma);
+    m.alpha = exp_cr(m.la);
+    return m;
+  }
   m.la = log_alpha_of(ns, t);
   const float e2 = 1.f - exp_cr(2.f * m.la);
   m.sigma = sqrtf(e2);                    // :146
   m.lam = m.la - 0.5f * log_cr(e2);         // :153-154
   m.alpha = exp_cr(m.la);                   // :140
+  m.alpha_e = m.alpha;
   return m;
 }
 
@@ -123,6 +142,12 @@ __device__ void first_update(bool pp, const Marg& ms, const Marg& mt, float& a, 
   else { a = exp_cr(mt.la - ms.la); c0 = -(mt.sigma * expm1_cr(h)); }
 }
 
+// the time the network receives for the label t: get_model_input_time :278, or time_scale*sigma_t on the flow schedule
+__device__ float input_time(const SchedDev& ns, float t) {
+  if (ns.kind == 2) return ns.time_scale * flow_sigma(ns, t);
+  return ns.discrete_input ? (t - ns.inv_N) * 1000.f : t;
+}
+
 __global__ void k_adapt_plan(const AdaptCfg c) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   float* st = c.state;
@@ -131,10 +156,10 @@ __global__ void k_adapt_plan(const AdaptCfg c) {
   if (__float_as_int(st[ST_DONE]) != 0) {
     // finished: identity updates at t_0 for the rest of the chunk (x_lower = x_higher = x)
     const Marg m0 = marg(c.ns, c.t_0);
-    for (int l = 0; l < 4; ++l) put(co + l * CO_WORDS, 1.f, 0.f, 0.f, 0.f, 1.f, 1.f, 1.f, 1.f, 1.f, m0.alpha, m0.sigma);
+    for (int l = 0; l < 4; ++l) put(co + l * CO_WORDS, 1.f, 0.f, 0.f, 0.f, 1.f, 1.f, 1.f, 1.f, 1.f, m0.alpha_e, m0.sigma);
     for (int j = 0; j < 3; ++j) {
       c.times[j] = c.t_0;
-      c.times[3 + j] = c.ns.discrete_input ? (c.t_0 - c.ns.inv_N) * 1000.f : c.t_0;
+      c.times[3 + j] = input_time(c.ns, c.t_0);
     }
     return;
   }
@@ -148,7 +173,7 @@ __global__ void k_adapt_plan(const AdaptCfg c) {
     // lower: first update s -> t (launch 0, consumes the evaluation at s)
     float a, c0;
     first_update(pp, ms, mt, a, c0);
-    put(co + 0 * CO_WORDS, a, c0, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, ms.alpha, ms.sigma);
+    put(co + 0 * CO_WORDS, a, c0, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, ms.alpha_e, ms.sigma);
     // higher: singlestep second update, r1 = 0.5 (:613-669): launch 1 = x -> x_s1 (pure), launch 2 = final
     const float r1 = 0.5f;
     const float s1 = inverse_lambda(c.ns, ms.lam + r1 * h);
@@ -166,8 +191,8 @@ __global__ void k_adapt_plan(const AdaptCfg c) {
       af = exp_cr(mt.la - ms.la); bf = mt.sigma * phi_1;
       c1f = c.taylor ? -((1.f / r1) * (mt.sigma * (phi_1 / h - 1.f))) : -((0.5f / r1) * bf);
     }
-    put(co + 1 * CO_WORDS, a1, c01, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, ms.alpha, ms.sigma);
-    put(co + 2 * CO_WORDS, af, -bf, c1f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, m1.alpha, m1.sigma);
+    put(co + 1 * CO_WORDS, a1, c01, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, ms.alpha_e, ms.sigma);
+    put(co + 2 * CO_WORDS, af, -bf, c1f, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, m1.alpha_e, m1.sigma);
   } else {
     // lower: singlestep second update with r1 = 1/3; higher: singlestep third update r1 = 1/3, r2 = 2/3 (:697-789)
     const float r1 = (float)(1.0 / 3.0), r2 = (float)(2.0 / 3.0);
@@ -194,15 +219,15 @@ __global__ void k_adapt_plan(const AdaptCfg c) {
       c1fin = -((1.f / r2) * (mt.sigma * phi_2));
       c1tay = -(mt.sigma * phi_2); c2fin = -(mt.sigma * phi_3);
     }
-    put(co + 0 * CO_WORDS, a1, c01, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, ms.alpha, ms.sigma);              // eval s: x -> x_s1
-    put(co + 1 * CO_WORDS, at, -bt, c1low, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, m1.alpha, m1.sigma);            // eval s1: lower final
-    put(co + 2 * CO_WORDS, a2, c02, c12, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, m1.alpha, m1.sigma);              // pure: x -> x_s2
-    if (c.taylor) put(co + 3 * CO_WORDS, at, -bt, c1tay, c2fin, 1.f / r1, 1.f / r2, r2, r1, r2 - r1, m2.alpha, m2.sigma);
-    else put(co + 3 * CO_WORDS, at, -bt, c1fin, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, m2.alpha, m2.sigma);       // eval s2: higher final
+    put(co + 0 * CO_WORDS, a1, c01, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, ms.alpha_e, ms.sigma);              // eval s: x -> x_s1
+    put(co + 1 * CO_WORDS, at, -bt, c1low, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, m1.alpha_e, m1.sigma);            // eval s1: lower final
+    put(co + 2 * CO_WORDS, a2, c02, c12, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, m1.alpha_e, m1.sigma);              // pure: x -> x_s2
+    if (c.taylor) put(co + 3 * CO_WORDS, at, -bt, c1tay, c2fin, 1.f / r1, 1.f / r2, r2, r1, r2 - r1, m2.alpha_e, m2.sigma);
+    else put(co + 3 * CO_WORDS, at, -bt, c1fin, 0.f, 1.f, 0.f, 0.f, 0.f, 0.f, m2.alpha_e, m2.sigma);       // eval s2: higher final
   }
   for (int j = 0; j < 3; ++j) {
     c.times[j] = tt[j];
-    c.times[3 + j] = c.ns.discrete_input ? (tt[j] - c.ns.inv_N) * 1000.f : tt[j];   // get_model_input_time :278
+    c.times[3 + j] = input_time(c.ns, tt[j]);
   }
 }
 
@@ -256,13 +281,14 @@ static int fill_cfg(AdaptCfg* c, const dpm_adaptive_ctl* a) {
   if (a->schedule_kind == 0 && (a->table_len < 2 || !a->t_array || !a->log_alpha_array || !a->log_alpha_flipped || !a->t_flipped)) {
     set_error("adaptive controller: discrete schedule needs its four tables"); return DPM_ERR_ARG;
   }
-  if (a->schedule_kind != 0 && a->schedule_kind != 1) { set_error("adaptive controller: schedule must be discrete (0) or linear (1)"); return DPM_ERR_UNSUPPORTED; }
+  if (a->schedule_kind < 0 || a->schedule_kind > 2) { set_error("adaptive controller: schedule must be discrete (0), linear (1) or flow (2)"); return DPM_ERR_UNSUPPORTED; }
   memset(c, 0, sizeof(*c));
   c->ns.kind = a->schedule_kind; c->ns.K = a->table_len;
   c->ns.t = a->t_array; c->ns.la = a->log_alpha_array; c->ns.la_f = a->log_alpha_flipped; c->ns.t_f = a->t_flipped;
   c->ns.beta_0 = a->beta_0; c->ns.beta_d = a->beta_1_minus_beta_0; c->ns.beta_0_sq = a->beta_0_sq;
   c->ns.inv_N = a->inv_total_N;
   c->ns.discrete_input = a->discrete_time_input;
+  c->ns.shift = a->flow_shift; c->ns.shift_m1 = a->flow_shift_minus_1; c->ns.time_scale = a->flow_time_scale;
   c->order = a->order; c->pp = a->predict_x0; c->taylor = a->taylor;
   c->t_0 = a->t_0; c->theta = a->theta; c->t_err = a->t_err;
   c->state = a->state; c->coef = a->coef; c->times = a->times; c->E = a->error;

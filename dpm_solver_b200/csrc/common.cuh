@@ -281,15 +281,27 @@ __device__ __forceinline__ float max_nan(float a, float b) {
 __device__ __forceinline__ float min_nan(float a, float b) {
   return (a != a) ? a : ((b != b) ? b : (b < a ? b : a));
 }
-// model_wrapper.noise_pred_fn :288-298
-__device__ __forceinline__ float convert_param(int param, float out, float xe, float alpha,
-                                               float sigma) {
-  switch (param) {
+// DPM_PARAM_FLOW: the velocity of a flow-matching model, converted straight into the solver's space (no division)
+__device__ __forceinline__ float flow_value(bool x0, float out, float xe, float alpha, float sigma) {
+  return x0 ? xe - sigma * out : xe + alpha * out;
+}
+// model_wrapper.noise_pred_fn :288-298. FLOW returns x0 when p.predict_x0 and eps otherwise (finish_x0 then skips :439).
+__device__ __forceinline__ float convert_param(const KParams& p, float out, float xe) {
+  const float alpha = p.alpha_e, sigma = p.sigma_e;
+  switch (p.param) {
     case DPM_PARAM_X_START: return (xe - alpha * out) / sigma;   // :292
     case DPM_PARAM_V: return alpha * out + sigma * xe;           // :295
     case DPM_PARAM_SCORE: return (-sigma) * out;                 // :298
+    case DPM_PARAM_FLOW: return flow_value(p.predict_x0 != 0, out, xe, alpha, sigma);
     default: return out;                                         // :289
   }
+}
+// converted and combined prediction -> buffered model value: eps, or x0 (:439, the thresholding clamp :424)
+__device__ __forceinline__ float finish_x0(const KParams& p, float eps, float xe, float thr, bool clamp) {
+  if (!p.predict_x0) return eps;
+  float x0 = p.param == DPM_PARAM_FLOW ? eps : (xe - p.sigma_e * eps) / p.alpha_e;  // data_prediction_fn :439
+  if (clamp) x0 = clamp_sym(x0, thr) / thr;  // dynamic_thresholding_fn :424
+  return x0;
 }
 
 // raw network output(s) -> buffered model value (eps, or x0 for dpmsolver++)
@@ -318,12 +330,12 @@ __device__ __forceinline__ float guided_value(const KParams& p, float xe, float 
     if (k == kPgRescale) return guided_value<kPgRescale>(p, xe, ec, eu, r, gs);
     return guided_value<kPgCombine>(p, xe, ec, eu, r, gs);
   } else if constexpr (K == kPgBypass) {
-    return convert_param(p.param, ec, xe, p.alpha_e, p.sigma_e);
+    return convert_param(p, ec, xe);
   } else if constexpr (K == kPgRescale) {
-    return convert_param(p.param, rescale_value(p, eu + gs * (ec - eu), r), xe, p.alpha_e, p.sigma_e);
+    return convert_param(p, rescale_value(p, eu + gs * (ec - eu), r), xe);
   } else {
-    const float epc = convert_param(p.param, ec, xe, p.alpha_e, p.sigma_e);
-    const float epu = convert_param(p.param, eu, xe, p.alpha_e, p.sigma_e);
+    const float epc = convert_param(p, ec, xe);
+    const float epu = convert_param(p, eu, xe);
     return epu + gs * (epc - epu);  // :330
   }
 }
@@ -338,12 +350,12 @@ __device__ __forceinline__ float model_value(const KParams& p, float xe, float e
   if constexpr (PG != 0) {
     eps = guided_value<PG>(p, xe, ec, eu, r, gs);
   } else if (RS) {
-    eps = convert_param(p.param, rescale_value(p, eu + p.guidance * (ec - eu), r), xe, p.alpha_e, p.sigma_e);
+    eps = convert_param(p, rescale_value(p, eu + p.guidance * (ec - eu), r), xe);
   } else {
-    eps = convert_param(p.param, ec, xe, p.alpha_e, p.sigma_e);
+    eps = convert_param(p, ec, xe);
   }
   if (NE == 2 && !RS && !PG) {
-    float epu = convert_param(p.param, eu, xe, p.alpha_e, p.sigma_e);
+    float epu = convert_param(p, eu, xe);
     if (RND && p.param == DPM_PARAM_NOISE) {
       const int dt = p.raw_round & 3;
       const float d = round_any(dt, eps - epu);
@@ -352,12 +364,7 @@ __device__ __forceinline__ float model_value(const KParams& p, float xe, float e
       eps = epu + p.guidance * (eps - epu);  // model_wrapper.model_fn :330
     }
   }
-  if (p.predict_x0) {
-    float x0 = (xe - p.sigma_e * eps) / p.alpha_e;  // data_prediction_fn :439
-    if (clamp) x0 = clamp_sym(x0, thr) / thr;  // dynamic_thresholding_fn :424
-    return x0;
-  }
-  return eps;
+  return finish_x0(p, eps, xe, thr, clamp);
 }
 
 // round a packet to its storage type once: returns the packed words and rewrites f[] with the
@@ -415,21 +422,57 @@ __device__ __forceinline__ float update_value(const KParams& p, float x, float T
   return 0.f;
 }
 
-// ---- the fast path: noise-parameterised networks (the common case), exact constant division ------
+// ---- the fast path: noise- and flow-parameterised networks, exact constant division ------
 // Launch-uniform switches are taken once per PACKET (uniform branches), every loop below is
-// straight-line code over 8 elements. Callers guarantee: p.param == NOISE; p.fast_div when a division
-// is needed; a clamp threshold `s` that is uniform over the packet.
+// straight-line code over 8 elements. Callers guarantee: p.param == NOISE or FLOW; p.fast_div when a division
+// is needed (a FLOW conversion has none); a clamp threshold `s` that is uniform over the packet.
+// FLOW converts each output first (flow8: one multiply and one add per element, in the solver's space) and combines the
+// converted values; a rescaled combine runs on the raw outputs and is converted afterwards. ec and eu are overwritten.
+__device__ __forceinline__ void flow8(const KParams& p, const float (&xe)[8], float (&v)[8]) {
+  if (p.predict_x0) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) v[i] = xe[i] - p.sigma_e * v[i];
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) v[i] = xe[i] + p.alpha_e * v[i];
+  }
+}
+// combined prediction T -> buffered model value: eps -> x0 (:439; a FLOW value is x0 already) and the clamp (:424)
+__device__ __forceinline__ void fast_finish8(const KParams& p, const float (&xe)[8], bool clamp, float s, float (&T)[8]) {
+  if (!p.predict_x0) return;
+  if (p.param != DPM_PARAM_FLOW) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) T[i] = xe[i] - p.sigma_e * T[i];
+    div_const8(T, p.alpha_e, p.r_alpha);  // :439
+  }
+  if (clamp) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) T[i] = clamp_sym(T[i], s);
+    if (recip_div_ok(s)) {
+      div_const8(T, s, __frcp_rn(s));  // :424
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) T[i] = div_ieee_cold(T[i], s);
+    }
+  }
+}
 // RS: guidance rescale with the sample's ratio r (uniform over the packet, like s).
 // PG: per-sample guidance with the sample's scale gs (uniform over the packet): gs == 1 selects ec (the bypass),
 // else the combine, rescaled when p.ratio is set -- both branches uniform per packet.
 template <int NE, bool RS = false, bool PG = false>
-__device__ __forceinline__ void fast_model8(const KParams& p, const float (&xe)[8], const float (&ec)[8],
-                                            const float (&eu)[8], bool clamp, float s, float (&T)[8],
+__device__ __forceinline__ void fast_model8(const KParams& p, const float (&xe)[8], float (&ec)[8],
+                                            float (&eu)[8], bool clamp, float s, float (&T)[8],
                                             float r = 1.f, float gs = 1.f) {
+  const bool flow = p.param == DPM_PARAM_FLOW;
+  const bool raw_combine = RS || (PG && p.ratio != nullptr);   // rescaled: combine the raw outputs, convert after
+  if (flow && !raw_combine) {
+    flow8(p, xe, ec);
+    if (NE == 2) flow8(p, xe, eu);
+  }
   if constexpr (PG) {
     if (gs == 1.f) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) T[i] = ec[i];   // :323 (p.param == NOISE: the conversion is the identity)
+      for (int i = 0; i < 8; ++i) T[i] = ec[i];   // :323 (NOISE: the conversion is the identity; FLOW: done above or below)
     } else {
 #pragma unroll
       for (int i = 0; i < 8; ++i) T[i] = eu[i] + gs * (ec[i] - eu[i]);  // :330
@@ -446,20 +489,8 @@ __device__ __forceinline__ void fast_model8(const KParams& p, const float (&xe)[
 #pragma unroll
     for (int i = 0; i < 8; ++i) T[i] = rescale_value(p, T[i], r);
   }
-  if (!p.predict_x0) return;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) T[i] = xe[i] - p.sigma_e * T[i];
-  div_const8(T, p.alpha_e, p.r_alpha);  // :439
-  if (clamp) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) T[i] = clamp_sym(T[i], s);
-    if (recip_div_ok(s)) {
-      div_const8(T, s, __frcp_rn(s));  // :424
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) T[i] = div_ieee_cold(T[i], s);
-    }
-  }
+  if (flow && raw_combine) flow8(p, xe, T);
+  fast_finish8(p, xe, clamp, s, T);
 }
 
 template <int FORM>
@@ -497,8 +528,8 @@ __device__ __forceinline__ void fast_update8(const KParams& p, const float (&x)[
 __host__ __forceinline__ bool fast_path_ok(const KParams& p) {
   if (p.form == DPM_FORM_SS3T && !p.fast_div) return false;
   if (p.n_model == 0) return true;
-  if (p.param != DPM_PARAM_NOISE) return false;
-  if (p.predict_x0 && !p.fast_div) return false;
+  if (p.param != DPM_PARAM_NOISE && p.param != DPM_PARAM_FLOW) return false;
+  if (p.param == DPM_PARAM_NOISE && p.predict_x0 && !p.fast_div) return false;   // FLOW: no division by alpha_e
   if ((p.thr != nullptr || p.ratio != nullptr || p.gscale != nullptr) && p.pk_per_sample == 0) return false;
   return true;
 }

@@ -95,7 +95,7 @@ __global__ void __launch_bounds__(kMaxThreads)
               unpack(rxe[u], fxe);
               fast_model8<NE, RS>(p, fxe, fec, feu, clamp, s_thr, fT, r);
             } else {
-              fast_model8<NE, RS>(p, fx, fec, feu, clamp, s_thr, fT, r);   // fx is only read when predict_x0 (then it is loaded)
+              fast_model8<NE, RS>(p, fx, fec, feu, clamp, s_thr, fT, r);   // fx is only read when the conversion needs it (then it is loaded)
             }
           }
           Raw<TS> rmo;

@@ -17,8 +17,9 @@ namespace dpm {
 constexpr int kMultiUnroll = 2;
 constexpr int kMultiThreads = 256;
 
-// FAST: param == NOISE (the conversion is the identity), exact constant division, a clamp threshold uniform per packet
-// (fast_path_ok). FAST = false: every parameterisation, per-element thresholds, IEEE division.
+// FAST: param == NOISE (the conversion is the identity) or FLOW (each block converted by flow8, one uniform branch per
+// packet, no division), exact constant division, a clamp threshold uniform per packet (fast_path_ok). FAST = false:
+// every parameterisation, per-element thresholds, IEEE division.
 template <typename TE, typename TS, int FORM, bool FAST>
 __global__ void __launch_bounds__(kMultiThreads) k_step_multi(const __grid_constant__ MultiParams mp) {
   const KParams& p = mp.k;
@@ -79,6 +80,8 @@ __global__ void __launch_bounds__(kMultiThreads) k_step_multi(const __grid_const
         }
         unpack(reu[u], fu);
         if (FAST) {
+          const bool flow = p.param == DPM_PARAM_FLOW;
+          if (flow) flow8(p, fxe, fu);
 #pragma unroll
           for (int i = 0; i < 8; ++i) g[i] = fu[i];
 #pragma unroll
@@ -86,17 +89,20 @@ __global__ void __launch_bounds__(kMultiThreads) k_step_multi(const __grid_const
             if (k < nc) {
               float fc[8];
               unpack(rec[u][k], fc);
+              if (flow) flow8(p, fxe, fc);
               const float s = mp.s[k];
 #pragma unroll
               for (int i = 0; i < 8; ++i) g[i] = g[i] + s * (fc[i] - fu[i]);
             }
           }
           const float s_thr = clamp ? __ldg(p.thr + (uint32_t)pk / p.pk_per_sample) : 1.f;
-          fast_model8<1>(p, fxe, g, g, clamp, s_thr, fT);   // NE == 1: T = g, then eps->x0 and the clamp
+#pragma unroll
+          for (int i = 0; i < 8; ++i) fT[i] = g[i];
+          fast_finish8(p, fxe, clamp, s_thr, fT);   // eps->x0 (a FLOW value is x0 already) and the clamp
         } else {
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
-            fu[i] = convert_param(p.param, fu[i], fxe[i], p.alpha_e, p.sigma_e);
+            fu[i] = convert_param(p, fu[i], fxe[i]);
             g[i] = fu[i];
           }
 #pragma unroll
@@ -106,7 +112,7 @@ __global__ void __launch_bounds__(kMultiThreads) k_step_multi(const __grid_const
               unpack(rec[u][k], fc);
               const float s = mp.s[k];
 #pragma unroll
-              for (int i = 0; i < 8; ++i) g[i] = g[i] + s * (convert_param(p.param, fc[i], fxe[i], p.alpha_e, p.sigma_e) - fu[i]);
+              for (int i = 0; i < 8; ++i) g[i] = g[i] + s * (convert_param(p, fc[i], fxe[i]) - fu[i]);
             }
           }
           float thr8[8];
@@ -121,15 +127,7 @@ __global__ void __launch_bounds__(kMultiThreads) k_step_multi(const __grid_const
             }
           }
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            if (p.predict_x0) {
-              float x0 = (fxe[i] - p.sigma_e * g[i]) / p.alpha_e;  // data_prediction_fn :439
-              if (clamp) x0 = clamp_sym(x0, thr8[i]) / thr8[i];  // dynamic_thresholding_fn :424
-              fT[i] = x0;
-            } else {
-              fT[i] = g[i];
-            }
-          }
+          for (int i = 0; i < 8; ++i) fT[i] = finish_x0(p, g[i], fxe[i], clamp ? thr8[i] : 1.f, clamp);
         }
         Raw<TS> rmo;
         round_pack(rmo, fT);
@@ -172,18 +170,11 @@ __global__ void __launch_bounds__(256) k_step_multi_scalar(const __grid_constant
     const float m1 = reads.m1 ? load_any(p.m1, sd, i) : 0.f;
     const float m2 = reads.m2 ? load_any(p.m2, sd, i) : 0.f;
     const float xe = p.use_xe ? ((reads.x && p.xe_is_x) ? x : load_any(p.xe, sd, i)) : 0.f;
-    const float eu = convert_param(p.param, load_any(p.eu, md, i), xe, p.alpha_e, p.sigma_e);
+    const float eu = convert_param(p, load_any(p.eu, md, i), xe);
     float eps = eu;
     for (int k = 0; k < nc; ++k)
-      eps = eps + mpc.s[k] * (convert_param(p.param, load_any(mpc.ec[k], md, i), xe, p.alpha_e, p.sigma_e) - eu);
-    float mv = eps;
-    if (p.predict_x0) {
-      mv = (xe - p.sigma_e * eps) / p.alpha_e;  // :439
-      if (clamp) {
-        const float thr = p.thr[(i + p.elem_offset) / p.per_sample];
-        mv = clamp_sym(mv, thr) / thr;  // :424
-      }
-    }
+      eps = eps + mpc.s[k] * (convert_param(p, load_any(mpc.ec[k], md, i), xe) - eu);
+    const float mv = finish_x0(p, eps, xe, clamp ? p.thr[(i + p.elem_offset) / p.per_sample] : 1.f, clamp);
     if (p.m_out) store_any(p.m_out, sd, i, mv);
     const float T0 = round_any(sd, mv);
     float o;

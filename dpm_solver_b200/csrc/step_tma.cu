@@ -200,7 +200,7 @@ __global__ void __launch_bounds__(kTmaMaxThreads)
             unpack(rxe[u], fxe);
             fast_model8<NE>(p, fxe, fec, feu, false, 1.f, fT);
           } else {
-            fast_model8<NE>(p, fx, fec, feu, false, 1.f, fT);   // fx is only read when predict_x0 (then has_x)
+            fast_model8<NE>(p, fx, fec, feu, false, 1.f, fT);   // fx is only read when the conversion needs it (then has_x)
           }
           Raw<TS> rmo;
           round_pack(rmo, fT);

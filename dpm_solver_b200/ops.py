@@ -441,12 +441,12 @@ class AdaptiveController:
     tiny kernels that advance them (dpm_adaptive_init / _plan / _decide) and the conditional commit
     (dpm_select_copy). `read()` is the only host synchronisation."""
 
-    SUPPORTED = ("discrete", "linear")
+    SUPPORTED = ("discrete", "linear", "flow")
 
     def __init__(self, be: "CudaBackend", ns, device, order: int, predict_x0: bool, taylor: bool, t_0: float,
                  theta: float, t_err: float, discrete_input: bool):
         if ns.schedule not in self.SUPPORTED:
-            raise ValueError("the device controller supports the 'discrete' and 'linear' schedules")
+            raise ValueError("the device controller supports the 'discrete', 'linear' and 'flow' schedules")
         self.be, self.dev = be, torch.device(device)
         f32 = dict(dtype=torch.float32, device=self.dev)
         self.state = torch.zeros(16, **f32)
@@ -460,6 +460,11 @@ class AdaptiveController:
             self._keep = [t.to(torch.float32).contiguous() for t in tabs]
             c.schedule_kind, c.table_len = 0, self._keep[0].numel()
             c.t_array, c.log_alpha_array, c.log_alpha_flipped, c.t_flipped = (t.data_ptr() for t in self._keep)
+            c.inv_total_N = 1. / ns.total_N
+        elif ns.schedule == "flow":
+            c.schedule_kind, c.table_len = 2, 0
+            # shift - 1 in double, each scalar rounded to fp32 once, as torch rounds the python-float operands
+            c.flow_shift, c.flow_shift_minus_1, c.flow_time_scale = ns.shift, ns.shift - 1., ns.time_scale
             c.inv_total_N = 1. / ns.total_N
         else:
             c.schedule_kind, c.table_len = 1, 0

@@ -58,7 +58,7 @@ def _f(v: Number, i: int = 0) -> float:
 
 
 class Marginals:
-    """log(alpha), alpha, sigma, lambda of a vector of times (one vectorised pass; the expressions
+    """log(alpha), alpha, sigma, lambda of a vector of times (one vectorised pass; for a VP schedule the expressions
     are those of marginal_log_mean_coeff / marginal_std / marginal_lambda / marginal_alpha,
     :127-154, sharing the single evaluation of log(alpha))."""
 
@@ -66,15 +66,23 @@ class Marginals:
         if t is None:
             return
         self.t = t
+        own = getattr(ns, "marginals", None)      # a schedule that is not VP supplies the four itself (NoiseScheduleFlow)
+        if own is not None:
+            # alpha_e = marginal_alpha(t) converts network outputs (:438); the update formulas take exp(log alpha) (:567)
+            self.log_alpha, self.sigma, self.lam, self.alpha_e = own(t)
+            self.alpha = torch.exp(self.log_alpha)
+            return
         self.log_alpha = ns.marginal_log_mean_coeff(t)
         e2 = 1. - torch.exp(2. * self.log_alpha)
         self.sigma = torch.sqrt(e2)                           # :146
         self.lam = self.log_alpha - 0.5 * torch.log(e2)       # :153-154
         self.alpha = torch.exp(self.log_alpha)                # :140
+        self.alpha_e = self.alpha
 
     def __getitem__(self, i) -> "Marginals":
         m = Marginals(None, None)
         m.t, m.log_alpha, m.sigma, m.lam, m.alpha = self.t[i], self.log_alpha[i], self.sigma[i], self.lam[i], self.alpha[i]
+        m.alpha_e = self.alpha_e[i]
         return m
 
 

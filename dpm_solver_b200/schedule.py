@@ -1,4 +1,5 @@
-"""VP noise schedule scalars: log(alpha_t), alpha_t, sigma_t, lambda_t and lambda^-1.
+"""Noise schedule scalars: log(alpha_t), alpha_t, sigma_t, lambda_t and lambda^-1, for the reference's VP schedules
+(`NoiseScheduleVP`) and for flow-matching models on the linear path (`NoiseScheduleFlow`).
 
 API-compatible with `NoiseScheduleVP` of the reference (dpm_solver_pytorch.py:6-167) -- same
 constructor, attributes and methods -- but every method is a handful of vectorised ops: the
@@ -11,7 +12,7 @@ from __future__ import annotations
 
 import torch
 
-__all__ = ["NoiseScheduleVP", "interpolate_fn", "expand_dims"]
+__all__ = ["NoiseScheduleVP", "NoiseScheduleFlow", "interpolate_fn", "expand_dims"]
 
 
 def _piecewise_linear(x: torch.Tensor, xp: torch.Tensor, yp: torch.Tensor) -> torch.Tensor:
@@ -143,3 +144,66 @@ class NoiseScheduleVP:
             t_fn = lambda la: torch.arccos(torch.exp(la + self.cosine_log_alpha_0)) * 2. \
                 * (1. + self.cosine_s) / math.pi - self.cosine_s
             return t_fn(log_alpha)
+
+
+class NoiseScheduleFlow:
+    """Flow-matching (rectified-flow) schedule: x_t = alpha_t*x0 + sigma_t*eps on the linear path alpha_t + sigma_t = 1,
+    with the time shift of SD3 / FLUX (not in the reference; `schedule == "flow"` is the tag other code switches on):
+
+        sigma_t = shift*t / (1 + (shift - 1)*t),    alpha_t = 1 - sigma_t,    lambda_t = log(alpha_t) - log(sigma_t).
+
+    `model_wrapper(..., model_type="flow")` wraps a network that predicts the velocity v = eps - x0; it receives
+    `time_scale * sigma_t` (SD3's convention; time_scale=1 for a network that takes sigma itself). lambda(1) = -inf, so
+    sampling starts at T = 1 - 1/total_N and, by default, ends at 1/total_N.
+
+    Every method is fp32 torch arithmetic on `t` with the python floats `shift`, `shift - 1` (formed in double) and
+    `time_scale` as scalar operands, in exactly this order (the device controller of the adaptive solver and the tests
+    restate it):
+
+        sigma  = (shift * t) / (1. + (shift - 1.) * t)          # shift == 1: (1*t) / (1 + 0*t) == t exactly
+        alpha  = 1. - sigma
+        log_alpha = log(alpha);   lambda = log_alpha - log(sigma)
+        inverse_lambda: sigma = 1. / (1. + exp(lambda));   t = sigma / (shift - (shift - 1.) * sigma)
+        model input time = time_scale * sigma
+    """
+
+    schedule = "flow"
+
+    def __init__(self, shift=1.0, time_scale=1000.0, total_N=1000):
+        shift, time_scale = float(shift), float(time_scale)
+        if not shift > 0 or shift == float("inf"):
+            raise ValueError("NoiseScheduleFlow: shift must be a positive finite number, got {}".format(shift))
+        if int(total_N) != total_N or total_N < 2:
+            raise ValueError("NoiseScheduleFlow: total_N must be an integer >= 2, got {}".format(total_N))
+        self.shift = shift
+        self.time_scale = time_scale
+        self.total_N = int(total_N)
+        self.T = 1. - 1. / self.total_N
+
+    def marginal_std(self, t):
+        return (self.shift * t) / (1. + (self.shift - 1.) * t)
+
+    def marginal_alpha(self, t):
+        return 1. - self.marginal_std(t)
+
+    def marginal_log_mean_coeff(self, t):
+        return torch.log(self.marginal_alpha(t))
+
+    def marginal_lambda(self, t):
+        return self.marginals(t)[2]
+
+    def marginals(self, t):
+        """(log_alpha, sigma, lambda, alpha) of a vector of times in one pass (plan.Marginals). The update formulas take
+        exp(log_alpha) where the reference's do (:567); alpha itself converts the network output."""
+        sigma = self.marginal_std(t)
+        alpha = 1. - sigma
+        log_alpha = torch.log(alpha)
+        return log_alpha, sigma, log_alpha - torch.log(sigma), alpha
+
+    def inverse_lambda(self, lamb):
+        sigma = 1. / (1. + torch.exp(lamb))
+        return sigma / (self.shift - (self.shift - 1.) * sigma)
+
+    def model_input_time(self, t):
+        """What the network receives for the continuous label t: time_scale * sigma_t."""
+        return self.time_scale * self.marginal_std(t)

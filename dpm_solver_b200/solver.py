@@ -27,7 +27,7 @@ import torch
 import torch.distributed as dist
 
 from . import ops, plan as P
-from ._lib import FORM_LIN1, FORM_NONE, FORM_SS3T, PARAM_BY_NAME, PARAM_NOISE
+from ._lib import FORM_LIN1, FORM_NONE, FORM_SS3T, PARAM_BY_NAME, PARAM_FLOW, PARAM_NOISE
 from .ops import StepArgs
 
 __all__ = ["model_wrapper", "DPM_Solver", "WrappedModel"]
@@ -52,6 +52,7 @@ class RawOutput:
     # and their fp32-rounded scales; `guidance` is then not read
     e_conds: Optional[tuple] = None
     scales: Optional[tuple] = None
+    is_x0: bool = False     # `e_cond` is a materialised x0 (a guided flow prediction): it is only clamped, not converted
 
 
 def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale):
@@ -155,6 +156,8 @@ class WrappedModel:
         """[1/N, 1] -> [0, 1000*(N-1)/N] for discrete-time models (:271-280)."""
         if self.noise_schedule.schedule == 'discrete':
             return (t_continuous - 1. / self.noise_schedule.total_N) * 1000.
+        if self.noise_schedule.schedule == 'flow':
+            return self.noise_schedule.model_input_time(t_continuous)     # time_scale * sigma_t
         return t_continuous
 
     def _call_model(self, x, t_continuous, cond=None, t_input=None):
@@ -312,7 +315,7 @@ class WrappedModel:
         if r.e_uncond is None and r.param == PARAM_NOISE:
             return r.e_cond
         pairs = self._alpha_sigma(t_continuous) if r.param != PARAM_NOISE else [(1.0, 0.0)]
-        needs_x = r.param in (PARAM_BY_NAME["x_start"], PARAM_BY_NAME["v"])
+        needs_x = r.param in (PARAM_BY_NAME["x_start"], PARAM_BY_NAME["v"], PARAM_FLOW)
         xo = x.to(r.e_cond.dtype) if needs_x else None
         ratio = _cfg_ratio(be, r)      # over the whole batch: each sample's ratio reads its own values only
 
@@ -333,6 +336,13 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     """Wrap a network into `model_fn(x, t_continuous) -> noise`; same contract as the reference
     (:170-334): model_type in {noise, x_start, v, score}, guidance_type in {uncond, classifier,
     classifier-free}.
+
+    model_type="flow" (not in the reference; needs a `NoiseScheduleFlow`): the network predicts the velocity
+    v = eps - x0 of a flow-matching model. The solver converts it straight into its own space, x0 = x - sigma_t*v for
+    dpmsolver++ and eps = x + alpha_t*v for dpmsolver (this callable returns the latter), two rounded ops and no
+    division. Under classifier-free guidance in any form each output is converted first and the converted values are
+    combined; guidance_rescale combines and rescales the raw velocities, then converts. A NoiseScheduleFlow also takes
+    "noise" and "x_start" networks; "v" and "score" (VP formulas) and guidance_type="classifier" are rejected.
 
     guidance_rescale=phi (classifier-free guidance only; not in the reference): guidance rescale of Lin et al.
     2023 as diffusers' `rescale_noise_cfg` does it, in the network's output space (eps for a noise network, v for
@@ -356,8 +366,16 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     torch's eager ops compute it. Every output is combined, whatever the scales (no bypass). One condition in a list is
     exactly the tensor form. With K >= 2: unconditional_condition is required, and guidance_rescale, per-sample scales
     and DPM_Solver(reference_rounding=True) are not available (ValueError)."""
-    assert model_type in ["noise", "x_start", "v", "score"]
+    assert model_type in ["noise", "x_start", "v", "score", "flow"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
+    flow_schedule = getattr(noise_schedule, "schedule", None) == "flow"
+    if model_type == "flow" and not flow_schedule:
+        raise ValueError("model_type='flow' needs a NoiseScheduleFlow")
+    if flow_schedule and model_type in ("v", "score"):
+        raise ValueError("model_type='{}' is defined for variance-preserving schedules; a NoiseScheduleFlow takes "
+                         "'flow', 'noise' or 'x_start'".format(model_type))
+    if flow_schedule and guidance_type == "classifier":
+        raise ValueError("classifier guidance is not available with a NoiseScheduleFlow")
     guidance_rescale = float(guidance_rescale)
     if not math.isfinite(guidance_rescale):
         raise ValueError("guidance_rescale must be finite, got {}".format(guidance_rescale))
@@ -429,6 +447,8 @@ class DPM_Solver:
         self.state_dtype = state_dtype
         self.plan_broadcast = bool(plan_broadcast)
         self.reference_rounding = bool(reference_rounding)
+        if self.reference_rounding and getattr(noise_schedule, "schedule", None) == "flow":
+            raise ValueError("reference_rounding=True reproduces the reference, which has no flow schedule")
         if self.reference_rounding and getattr(model_fn, "guidance_rescale", 0) != 0:
             raise ValueError("guidance_rescale is not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "per_sample_guidance", False):
@@ -554,7 +574,7 @@ class DPM_Solver:
                     self.__dict__.pop(name, None)
             return ("discrete", id(la), la._version, id(ta), ta._version, ns.total_N)
         return (getattr(ns, "schedule", None), getattr(ns, "beta_0", None), getattr(ns, "beta_1", None),
-                getattr(ns, "T", None))
+                getattr(ns, "T", None), getattr(ns, "shift", None), getattr(ns, "time_scale", None))
 
     def _plan_id(self, key):
         """Hashable identity of a cached plan (schedule + algorithm + sampling arguments): prepared launches are
@@ -619,7 +639,7 @@ class DPM_Solver:
         """[n_evals, rows] device matrix of model-input times for a whole run (one tiny kernel per
         sample() instead of two per model call); None when the model takes t_continuous itself."""
         w = self._wrapped
-        if not (isinstance(w, WrappedModel) and w.fusable and w.noise_schedule.schedule == 'discrete'):
+        if not (isinstance(w, WrappedModel) and w.fusable and w.noise_schedule.schedule in ('discrete', 'flow')):
             return None
         t_in = self._upload(w.get_model_input_time(t_host.reshape(-1)), device)   # (t - 1/N) * 1000, fp32, :278
         return t_in[:, None].expand(t_in.shape[0], w.input_rows(batch)).contiguous()
@@ -627,6 +647,10 @@ class DPM_Solver:
     def _conv_args(self, raw: RawOutput, xe, alsig, sdtype, x0: bool) -> StepArgs:
         """StepArgs fields that turn `raw` into the buffered model value at time t (x0 if `x0`, else
         eps). `alsig` is (alpha_t, sigma_t) from the plan, or the host time tensor to derive them."""
+        if raw.is_x0:
+            # identity on the materialised x0, for every value: x0 = (-0) - (-1)*e_cond (then the clamp)
+            return StepArgs(n_model=1, e_cond=raw.e_cond, param=PARAM_FLOW, predict_x0=True, alpha_e=1.0, sigma_e=-1.0,
+                            xe=torch.full_like(xe, -0.0), state_dtype=sdtype)
         a = StepArgs(n_model=2 if raw.e_uncond is not None else 1, e_cond=raw.e_cond,
                      e_uncond=raw.e_uncond, param=raw.param, guidance=raw.guidance,
                      predict_x0=x0, state_dtype=sdtype)
@@ -719,7 +743,9 @@ class DPM_Solver:
             # sample's scale, as the reference orders it (+1 launch) -- or, with several conditions, their combined
             # noise, each block parameterised first (+1 launch)
             if ratio is None and (raw.guidance_b is not None or raw.e_conds is not None):
-                a = self._conv_args(raw, xe, alsig, torch.float32, False)
+                # (a flow network's outputs are converted to x0 directly and combined as x0: no eps -> x0 follows)
+                flow = raw.param == PARAM_FLOW
+                a = self._conv_args(raw, xe, alsig, torch.float32, flow)
                 if a.xe is not None and a.xe.dtype != torch.float32:
                     a.xe = a.xe.float()
                 if alsig is _DEV:
@@ -730,9 +756,9 @@ class DPM_Solver:
                 if raw.e_conds is not None:
                     # several conditions: the quantile reads the materialised noise; the step then recomputes the same
                     # fp32 combine from the K+1 outputs, so that it can also write the K+1 blocks of the next input
-                    q_raw = RawOutput(e, None, PARAM_NOISE, 1.0)
+                    q_raw = RawOutput(e, None, PARAM_NOISE, 1.0, is_x0=flow)
                 else:
-                    raw = RawOutput(e, None, PARAM_NOISE, 1.0)
+                    raw = RawOutput(e, None, PARAM_NOISE, 1.0, is_x0=flow)
             else:
                 a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
                              guidance=raw.guidance, state_dtype=torch.float32, raw_round=code)
@@ -1094,7 +1120,8 @@ class DPM_Solver:
         block the plan kernel wrote; `adaptive_chunk` iterations are enqueued per read of the `done` flag."""
         be, ns = ops.backend(), self.noise_schedule
         w = self._wrapped
-        discrete_in = isinstance(w, WrappedModel) and w.noise_schedule.schedule == 'discrete'
+        # (the network's time input differs from the label: the controller writes it next to the label)
+        discrete_in = isinstance(w, WrappedModel) and w.noise_schedule.schedule in ('discrete', 'flow')
         ctl = be.adaptive_controller(ns, x.device, order=order, predict_x0=self._pp, taylor=solver_type == 'taylor',
                                      t_0=t_0, theta=theta, t_err=t_err, discrete_input=discrete_in)
         ctl.init(t_T, h_init)
@@ -1258,7 +1285,7 @@ class DPM_Solver:
                     plan = P.multistep_plan(ns, self.algorithm_type, solver_type, ts, order, lower_order_final,
                                             marginals=marg)
                     # (alpha_t, sigma_t) per grid point: scalars of the eps->x0 / parameterisation step
-                    return ts, plan, list(zip(marg.alpha.tolist(), marg.sigma.tolist()))
+                    return ts, plan, list(zip(marg.alpha_e.tolist(), marg.sigma.tolist()))
 
                 ts, plan, alsig = self._host_plan(key, build)
                 plan = self._sync_plan(plan, key)
@@ -1325,7 +1352,7 @@ class DPM_Solver:
                     all_times = torch.cat([tt.reshape(-1) for sp in plans for tt in sp.times])
                     marg = P.Marginals(ns, all_times)
                     return (torch.cat([all_times, timesteps_outer.reshape(-1)]), plans,
-                            list(zip(marg.alpha.tolist(), marg.sigma.tolist())))
+                            list(zip(marg.alpha_e.tolist(), marg.sigma.tolist())))
 
                 packed, plans, alsig = self._host_plan(key, build)
                 if self.plan_broadcast and plans:

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 102 /* 0.1.2: dpm_step_multi, dpm_replicate */
+#define DPM_B200_VERSION 103 /* 0.1.3: DPM_PARAM_FLOW, dpm_adaptive_ctl.schedule_kind 2 (flow) */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -75,12 +75,20 @@ typedef enum dpm_form {
   DPM_FORM_SS3T = 6
 } dpm_form;
 
-/* Parameterisation of the network output, model_wrapper.noise_pred_fn :288-298 */
+/* Parameterisation of the network output, model_wrapper.noise_pred_fn :288-298.
+ * DPM_PARAM_FLOW (not in the reference): the velocity v = eps - x0 of a flow-matching model on the linear path
+ * x_t = alpha_t*x0 + sigma_t*eps with alpha_t + sigma_t = 1. Its conversion lands directly in the solver's space, two
+ * separately rounded ops and no division:
+ *   predict_x0 == 1 : x0  = xe - sigma_e*out      (the eps -> x0 division :439 is skipped; the clamp follows)
+ *   predict_x0 == 0 : eps = xe + alpha_e*out
+ * Classifier-free guidance in every form converts each output so and combines the converted values
+ * (T = T_u + s*(T_c - T_u)); a rescaled step combines and rescales the raw outputs, then converts. */
 typedef enum dpm_param {
   DPM_PARAM_NOISE = 0,   /* eps = out                         :289 */
   DPM_PARAM_X_START = 1, /* eps = (xe - alpha*out)/sigma      :292 */
   DPM_PARAM_V = 2,       /* eps = alpha*out + sigma*xe        :295 */
-  DPM_PARAM_SCORE = 3    /* eps = (-sigma)*out                :298 */
+  DPM_PARAM_SCORE = 3,   /* eps = (-sigma)*out                :298 */
+  DPM_PARAM_FLOW = 4     /* x0 = xe - sigma*out  or  eps = xe + alpha*out (see above) */
 } dpm_param;
 
 /* One fused solver step. With n_model == 0 this is a pure update on buffered model values.
@@ -112,7 +120,7 @@ typedef struct dpm_step_desc {
   int32_t form;        /* dpm_form                                                         */
   int32_t n_model;     /* 0, 1 or 2 raw network outputs                                    */
   int32_t param;       /* dpm_param                                                        */
-  int32_t predict_x0;  /* 1: buffered value is x0 = (xe - sigma_e*eps)/alpha_e :439         */
+  int32_t predict_x0;  /* 1: buffered value is x0 = (xe - sigma_e*eps)/alpha_e :439 (DPM_PARAM_FLOW: see there) */
   int32_t c0_on_old;   /* DIFF2 only                                                       */
   int32_t raw_round;   /* 0 (default). Reference-rounding mode for networks that return 16-bit NOISE into an
                           fp32 state: bits 0-1 = DPM_BF16 / DPM_F16, the type the raw outputs arrived in --
@@ -321,7 +329,8 @@ DPM_API int dpm_replicate(void* out, const void* x, uint64_t n, int copies, int 
  * int bit patterns where integral), coef[4][16] (one dpm_step_desc.dev_coef block per fused launch of an
  * iteration), times[6] (evaluation times s, s1, s2, then the model-input times the network receives), error[1]
  * (written by dpm_adaptive_error). Schedule: discrete (tables as NoiseScheduleVP holds them, plus their flipped
- * copies, all on the device) or the continuous linear VPSDE.
+ * copies, all on the device), the continuous linear VPSDE, or the flow schedule (NoiseScheduleFlow's closed forms:
+ * sigma_t = shift*t/(1 + (shift-1)*t), alpha_t = 1 - sigma_t; the network then receives time_scale*sigma_t).
  *   dpm_adaptive_init   : s = t_T, lambda_s, lambda_0, h = h_init                                      :972-977
  *   dpm_adaptive_plan   : t = lambda^-1(lambda_s + h) and every coefficient block / time label of the
  *                         lower- and higher-order updates of this iteration                             :984-992
@@ -333,7 +342,7 @@ DPM_API int dpm_replicate(void* out, const void* x, uint64_t n, int copies, int 
  * dpm_solver_b200/solver.py). After `done` the plan emits identity coefficients, so a fixed-length chunk of
  * iterations can be enqueued (or graph-captured) and `done` read back once per chunk. */
 typedef struct dpm_adaptive_ctl {
-  int32_t schedule_kind;       /* 0 discrete, 1 linear */
+  int32_t schedule_kind;       /* 0 discrete, 1 linear, 2 flow */
   int32_t table_len;
   const float* t_array;        /* device, [table_len] */
   const float* log_alpha_array;
@@ -350,6 +359,9 @@ typedef struct dpm_adaptive_ctl {
   float* times;                /* device [6] */
   const float* error;          /* device [1] */
   float beta_0_sq;             /* linear: fl32(beta_0**2) with the square taken in double (reference :162) */
+  float flow_shift;            /* flow: fl32(shift) */
+  float flow_shift_minus_1;    /* flow: fl32(shift - 1), the difference taken in double */
+  float flow_time_scale;       /* flow: the network takes fl32(time_scale)*sigma_t (discrete_time_input is not read) */
 } dpm_adaptive_ctl;
 
 DPM_API int dpm_adaptive_init(const dpm_adaptive_ctl* ctl, float t_T, float h_init, dpm_stream_t stream);
