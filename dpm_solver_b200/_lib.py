@@ -39,6 +39,14 @@ class StepDesc(C.Structure):
     ]
 
 
+class UniDesc(C.Structure):
+    """struct dpm_unipc_desc"""
+    _fields_ = [
+        ("m3", C.c_void_p), ("out_c", C.c_void_p), ("pc", C.c_int32), ("pp", C.c_int32),
+        ("cd", C.c_float * 2), ("ct", C.c_float), ("a", C.c_float), ("c0", C.c_float), ("cp", C.c_float * 2),
+    ]
+
+
 class AdaptiveCtl(C.Structure):
     """struct dpm_adaptive_ctl"""
     _fields_ = [
@@ -90,6 +98,7 @@ PROTOTYPES = {
     "dpm_cfg_rescale_ratio_guided": (C.c_int, [_vp, _vp, _vp, _vp, _u64, _u64, _i, _vp, C.c_size_t, _vp]),
     "dpm_step_multi": (C.c_int, [C.POINTER(StepDesc), C.POINTER(_vp), C.POINTER(_f), _i, C.POINTER(_vp), _vp]),
     "dpm_replicate": (C.c_int, [_vp, _vp, _u64, _i, _i, _vp]),
+    "dpm_step_unipc": (C.c_int, [C.POINTER(StepDesc), C.POINTER(UniDesc), _vp]),
 }
 
 MAX_CONDITIONS = 4      # DPM_MAX_CONDITIONS

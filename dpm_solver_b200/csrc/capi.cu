@@ -312,6 +312,65 @@ static int step_multi_impl(const dpm_step_desc* desc, const void* const* e_conds
   return finish(rc);
 }
 
+static int step_unipc_impl(const dpm_step_desc* desc, const dpm_unipc_desc* u, cudaStream_t stream) {
+  if (desc == nullptr || u == nullptr) { set_error("UniPC step: desc or u is NULL"); return DPM_ERR_ARG; }
+  if (u->pc < 0 || u->pc > 3 || u->pp < 0 || u->pp > 3 || (u->pc == 0 && u->pp == 0)) {
+    set_error("UniPC step: corrector order %d and predictor order %d must lie in 0..3, not both 0", u->pc, u->pp);
+    return DPM_ERR_ARG;
+  }
+  if (desc->raw_round != 0 || desc->dev_coef != nullptr) {
+    set_error("UniPC step: raw_round and dev_coef are not available");
+    return DPM_ERR_ARG;
+  }
+  const UniReads rd = uni_reads(u->pc, u->pp);
+  if ((rd.m1 && desc->m1 == nullptr) || (rd.m2 && desc->m2 == nullptr) || (rd.m3 && u->m3 == nullptr) ||
+      (u->pp == 0 && u->out_c == nullptr) || (u->pp > 0 && desc->out == nullptr)) {
+    set_error("UniPC step: a buffer or output required by corrector order %d / predictor order %d is NULL", u->pc, u->pp);
+    return DPM_ERR_ARG;
+  }
+  if (desc->n == 0) return DPM_OK;
+  // validated as a LIN1 step on x~ (x read, the conversion evaluated at x); its out stands in for out_c when pp == 0
+  dpm_step_desc d = *desc;
+  d.form = DPM_FORM_LIN1;
+  d.xe = nullptr;
+  d.m1 = d.m2 = nullptr;
+  if (u->pp == 0) { d.out = u->out_c; d.out2 = nullptr; }
+  UniParams up;
+  memset(&up, 0, sizeof(up));
+  Needs nd;
+  int rc = build_params(&d, &up.k, &nd, false);
+  if (rc != DPM_OK) return rc;
+  KParams& p = up.k;
+  p.m1 = desc->m1; p.m2 = desc->m2;
+  if (u->pp == 0) p.out = nullptr;
+  up.m3 = u->m3; up.out_c = u->out_c;
+  up.pc = u->pc; up.pp = u->pp;
+  up.cd[0] = u->cd[0]; up.cd[1] = u->cd[1]; up.ct = u->ct;
+  up.a = u->a; up.c0 = u->c0; up.cp[0] = u->cp[0]; up.cp[1] = u->cp[1];
+  const int sd = p.state_dtype;
+  nd.m1 = rd.m1; nd.m2 = rd.m2;
+  const bool aligned_all = all_aligned(p, nd) && (!rd.m3 || aligned(up.m3, sd)) &&
+                           (up.out_c == nullptr || aligned(up.out_c, sd));
+  Tuning t{g_variant.load(), g_threads.load(), g_ctas.load()};
+  bool body_done = false;
+  if (p.npk > 0 && aligned_all) {
+    const int r = launch_step_unipc(up, t, stream);
+    if (r < 0 || r > 1) return r;
+    body_done = (r == 0);
+  }
+  if (!body_done) {
+    rc = launch_step_unipc_scalar(up, stream);
+  } else if (p.n % kPacket) {
+    UniParams tail = up;
+    const uint64_t el = (uint64_t)p.npk * kPacket;
+    tail.k = shifted(p, el);
+    tail.m3 = off(up.m3, sd, el);
+    tail.out_c = off(up.out_c, sd, el);
+    rc = launch_step_unipc_scalar(tail, stream);
+  }
+  return finish(rc);
+}
+
 }  // namespace dpm
 
 using namespace dpm;
@@ -477,6 +536,10 @@ int dpm_duplicate(void* out, const void* x, uint64_t n, int dtype, dpm_stream_t 
 int dpm_step_multi(const dpm_step_desc* desc, const void* const* e_conds, const float* scales, int n_cond,
                    void* const* replicas, dpm_stream_t stream) {
   return step_multi_impl(desc, e_conds, scales, n_cond, replicas, static_cast<cudaStream_t>(stream));
+}
+
+int dpm_step_unipc(const dpm_step_desc* desc, const dpm_unipc_desc* u, dpm_stream_t stream) {
+  return step_unipc_impl(desc, u, static_cast<cudaStream_t>(stream));
 }
 
 int dpm_replicate(void* out, const void* x, uint64_t n, int copies, int dtype, dpm_stream_t stream) {

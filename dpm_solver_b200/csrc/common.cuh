@@ -79,6 +79,26 @@ struct MultiParams {
   int32_t n_cond;
 };
 
+// UniPC (dpm_step_unipc): the corrector of step i and the predictor of step i+1 around the conversion of KParams, whose
+// own update fields (form, a, c*, w*) are not read. k.x is x~_i (also the evaluation state), k.m0 m_i when n_model == 0,
+// k.m1 / k.m2 / m3 the buffers m_{i-1} / m_{i-2} / m_{i-3}; out_c (optional) receives the corrected x_i.
+struct UniParams {
+  KParams k;
+  const void* m3;
+  void* out_c;
+  int32_t pc, pp;      // corrector order 0..3 (0 = off), predictor order 0..3 (0 = none)
+  float cd[2], ct;     // corrector words
+  float a, c0, cp[2];  // predictor words
+};
+// the buffers a UniPC launch reads: m_{i-1} for the corrector or a predictor of order >= 2, m_{i-2} for a corrector of
+// order >= 2 or a predictor of order 3, m_{i-3} for a corrector of order 3
+struct UniReads {
+  bool m1, m2, m3;
+};
+__host__ __device__ __forceinline__ UniReads uni_reads(int pc, int pp) {
+  return {pc >= 1 || pp >= 2, pc >= 2 || pp >= 3, pc >= 3};
+}
+
 // ---- storage types ------------------------------------------------------------------------
 template <typename T> struct Raw;  // one packet as loaded (still packed)
 template <> struct Raw<float> { uint32_t r[8]; };

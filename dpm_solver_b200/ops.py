@@ -69,6 +69,11 @@ class StepArgs:
     e_conds: Optional[Tuple[torch.Tensor, ...]] = None
     scales: Optional[Tuple[float, ...]] = None
     replicas: Optional[Tuple[torch.Tensor, ...]] = None
+    # UniPC (dpm_step_unipc): the launch's words (plan.UniCoeffs), m_{i-3}, and an optional preallocated tensor that
+    # receives the corrected state x_i (required when the launch has no predictor). `x` is x~_i, `m1`/`m2` m_{i-1}/m_{i-2}.
+    unipc: Optional[object] = None
+    m3: Optional[torch.Tensor] = None
+    out_c: Optional[torch.Tensor] = None
 
     def state_tensors(self):
         return [t for t in (self.x, self.xe, self.m0, self.m1, self.m2) if t is not None]
@@ -202,7 +207,7 @@ class CudaBackend:
             if self._layout(m_out) != layout:
                 raise ValueError("dpm_solver_b200: preallocated m_out must be dense and laid out like the inputs")
             d.m_out = m_out.data_ptr()
-        if a.form != FORM_NONE:
+        if a.form != FORM_NONE and (a.unipc is None or a.unipc.pp > 0):
             out = a.out if a.out is not None else self._new_like(ref, sdt, layout)
             self._check(out, "out", ref.device, ref.numel(), sdt)
             if self._layout(out) != layout:
@@ -220,7 +225,9 @@ class CudaBackend:
                 raise TypeError(f"dpm_solver_b200: `{what}` must be a contiguous fp32 tensor on the tensors' device")
             if a.per_sample <= 0 or ref.numel() % a.per_sample or v.numel() != ref.numel() // a.per_sample:
                 raise ValueError(f"dpm_solver_b200: `{what}` needs one value per sample")
-        if a.e_conds is not None:
+        if a.unipc is not None:
+            self._step_unipc(a, d, ref, sdt, layout, keep)
+        elif a.e_conds is not None:
             self._step_multi(a, d, ref, sdt, layout, keep)
         elif a.guidance_b is not None:
             # (phi and 1 - phi as below; ignored without a ratio)
@@ -256,6 +263,27 @@ class CudaBackend:
         d.out2 = None
         self._launch(ref.device, self._lib.dpm_step_multi, C.byref(d),
                      (C.c_void_p * K)(*[e.data_ptr() for e in ecs]), (C.c_float * K)(*a.scales), C.c_int(K), reps)
+
+    def _step_unipc(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
+        """dpm_step_unipc: the UniPC words, m_{i-3} and the corrected-state output of a launch (d already filled)."""
+        if a.e_conds is not None or a.guidance_b is not None or a.ratio is not None:
+            raise ValueError("dpm_solver_b200: a UniPC step takes one guidance scale, without rescale")
+        w, u = a.unipc, _lib.UniDesc()
+        n = ref.numel()
+        if a.m3 is not None:
+            m3 = self._check(a.m3, "m3", ref.device, n, sdt, layout)
+            keep.append(m3)
+            u.m3 = m3.data_ptr()
+        if a.out_c is not None:
+            self._check(a.out_c, "out_c", ref.device, n, sdt)
+            if self._layout(a.out_c) != layout:
+                raise ValueError("dpm_solver_b200: out_c must be dense and laid out like the inputs")
+            u.out_c = a.out_c.data_ptr()
+        u.pc, u.pp = int(w.pc), int(w.pp)
+        u.cd[0], u.cd[1] = w.cd
+        u.ct, u.a, u.c0 = w.ct, w.a, w.c0
+        u.cp[0], u.cp[1] = w.cp
+        self._launch(ref.device, self._lib.dpm_step_unipc, C.byref(d), C.byref(u))
 
     def replicate(self, x: torch.Tensor, copies: int) -> torch.Tensor:
         """torch.cat([x] * copies) -- one read, `copies` writes (dpm_replicate); layout of x kept."""
@@ -528,7 +556,8 @@ class PreparedStep:
     @staticmethod
     def build(be: "CudaBackend", a: StepArgs) -> Optional["PreparedStep"]:
         if a.thr is not None or a.raw_round or a.ratio is not None or a.guidance_b is not None \
-                or a.e_conds is not None or a.coef_dev is not None or a.out is not None and a.out2 is None:
+                or a.e_conds is not None or a.coef_dev is not None or a.unipc is not None \
+                or a.out is not None and a.out2 is None:
             # (a rescaled step reads a fresh ratio tensor every evaluation, a guided one a scales tensor the
             # descriptor does not carry, a multi-condition one K outputs and scales it does not carry, one with device
             # coefficients a block the descriptor would point into without owning it: never frozen)

@@ -13,9 +13,11 @@ bit-identical to the reference evaluated on CPU. All `t` arguments are 1-D fp32 
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass, field
 from typing import List, Optional, Union
 
+import numpy as np
 import torch
 
 from ._lib import FORM_DIFF2, FORM_LIN1, FORM_MS3, FORM_SS3T
@@ -348,3 +350,94 @@ def singlestep_orders(steps: int, order: int) -> List[int]:
     if order == 1:
         return [1, ] * steps
     raise ValueError("'order' must be '1' or '2' or '3'.")
+
+
+# ---- UniPC multistep (unipc.py) ----------------------------------------------------------------
+
+@dataclass
+class UniCoeffs:
+    """Words of one dpm_step_unipc launch (python floats holding exact fp32 values, signs folded in): the corrector of
+    step i (order pc, 0 = off) and the predictor of step i+1 (order pp, 0 = none)."""
+    pc: int
+    pp: int
+    cd: tuple = (0.0, 0.0)
+    ct: float = 0.0
+    a: float = 0.0
+    c0: float = 0.0
+    cp: tuple = (0.0, 0.0)
+    form: int = FORM_LIN1       # (the descriptor's form: not read by dpm_step_unipc)
+    order: int = 0
+
+    def corrector_only(self) -> "UniCoeffs":
+        return UniCoeffs(self.pc, 0, self.cd, self.ct, order=self.order)
+
+    def predictor_only(self) -> "UniCoeffs":
+        return UniCoeffs(0, self.pp, a=self.a, c0=self.c0, cp=self.cp, order=self.order)
+
+
+def unipc_orders(steps: int, order: int, lower_order_final: bool) -> List[int]:
+    """Order p_i of UniPC step i = 1..steps: min(order, i), capped at steps + 1 - i with lower_order_final (for every
+    `steps`, unlike DPM_Solver's multistep rule, which lowers the final orders only when steps < 10)."""
+    return [min(order, i, steps + 1 - i) if lower_order_final else min(order, i) for i in range(1, steps + 1)]
+
+
+def _g(x: float, j: int) -> float:
+    """(e^x - sum_{m<=j} x^m/m!) / x^j in fp64: the series for |x| < 0.5, where the direct form cancels."""
+    if abs(x) < 0.5:
+        s, term = 0.0, 1.0
+        for m in range(j + 1, j + 30):
+            term = x ** (m - j) / math.factorial(m)
+            s += term
+        return s
+    return (math.expm1(x) - sum(x ** m / math.factorial(m) for m in range(1, j + 1))) / x ** j
+
+
+def unipc_step_weights(lam: List[float], i: int, p: int, pp_alg: bool, bh2: bool):
+    """fp64 scalars of UniPC step i (lam: the grid's lambda values): (hh, B, r[1..p], rho_p, rho_c)."""
+    h = lam[i] - lam[i - 1]
+    hh = -h if pp_alg else h
+    B = math.expm1(hh) if bh2 else hh
+    r = [(lam[i - 1 - k] - lam[i - 1]) / h for k in range(1, p)] + [1.0]
+    # b_j = h_phi_k * j! / B with h_phi_k = g_j(hh) after j - 1 steps of the recursion h_phi_k/hh - 1/f
+    b = [_g(hh, j) * math.factorial(j) / B for j in range(1, p + 1)]
+    R = [[rk ** (j - 1) for rk in r] for j in range(1, p + 1)]
+    if p == 1:
+        rho_p = []
+    elif p == 2:
+        rho_p = [0.5]
+    else:
+        rho_p = list(np.linalg.solve(np.array(R)[:p - 1, :p - 1], np.array(b[:p - 1])))
+    rho_c = [0.5] if p == 1 else list(np.linalg.solve(np.array(R), np.array(b)))
+    return hh, B, r, rho_p, rho_c
+
+
+def unipc_plan(algorithm_type: str, variant: str, marg: Marginals, orders: List[int], use_corrector: bool):
+    """(LIN1 Coeffs of step 1's predictor, [UniCoeffs of launches 1..N-1]). Every word is evaluated in fp64 from the
+    fp32 marginals and rounded to fp32 once."""
+    pp_alg, bh2 = algorithm_type == "dpmsolver++", variant == "bh2"
+    lam = marg.lam.double().tolist()
+    al = marg.alpha.double().tolist()
+    sg = marg.sigma.double().tolist()
+    N = len(orders)
+    f = lambda v: float(np.float32(v))
+    a1, c01 = _first(algorithm_type, marg[torch.tensor([0])], marg[torch.tensor([1])])
+    first = Coeffs(FORM_LIN1, _f(a1), _f(c01), order=1)
+    scale = sg if not pp_alg else al             # alpha_i for data prediction, sigma_i for noise prediction
+    W = [None] + [unipc_step_weights(lam, i, orders[i - 1], pp_alg, bh2) for i in range(1, N + 1)]
+    launches = []
+    for i in range(1, N):
+        p, q = orders[i - 1], orders[i]
+        _, B, r, rho_p, rho_c = W[i]
+        cd, ct, pc = [0.0, 0.0], 0.0, 0
+        if use_corrector:
+            pc = p
+            for k in range(1, p):
+                cd[k - 1] = f(-scale[i] * B * (rho_c[k - 1] - rho_p[k - 1]) / r[k - 1])
+            ct = f(-scale[i] * B * rho_c[p - 1])
+        hh2, B2, r2, rho_p2, _ = W[i + 1]
+        a = sg[i + 1] / sg[i] if pp_alg else al[i + 1] / al[i]
+        cp = [0.0, 0.0]
+        for k in range(1, q):
+            cp[k - 1] = f(-scale[i + 1] * B2 * rho_p2[k - 1] / r2[k - 1])
+        launches.append(UniCoeffs(pc, q, tuple(cd), ct, f(a), f(-scale[i + 1] * math.expm1(hh2)), tuple(cp), order=q))
+    return first, launches

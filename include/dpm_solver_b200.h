@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 103 /* 0.1.3: DPM_PARAM_FLOW, dpm_adaptive_ctl.schedule_kind 2 (flow) */
+#define DPM_B200_VERSION 104 /* 0.1.4: dpm_step_unipc */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -323,6 +323,33 @@ DPM_API int dpm_cfg_rescale_ratio_guided(float* ratio_out, const void* e_cond, c
 DPM_API int dpm_step_multi(const dpm_step_desc* desc, const void* const* e_conds, const float* scales, int n_cond,
                            void* const* replicas, dpm_stream_t stream);
 DPM_API int dpm_replicate(void* out, const void* x, uint64_t n, int copies, int dtype, dpm_stream_t stream);
+
+/* ---- UniPC multistep (Zhao et al. 2023, "UniPC: A Unified Predictor-Corrector Framework", arXiv:2302.04867) ------
+ * One launch per network evaluation i: the corrector of step i and the predictor of step i+1 (dpm_solver_b200/unipc.py
+ * states the method and how the host folds the words below). With x~ = desc->x, the predictor output x~_i that the
+ * network was evaluated at, and m_i its model value (desc->n_model >= 1: converted from the raw outputs exactly as
+ * dpm_step converts them -- parameterisation, CFG, eps -> x0, clamp -- rounded to the state dtype and written to
+ * desc->m_out when set; n_model == 0: read from desc->m0), m_{i-1} = desc->m1, m_{i-2} = desc->m2, m_{i-3} = u->m3:
+ *   pc > 0 : x_i = x~ [+ cd[0]*(m_{i-2} - m_{i-1}) [+ cd[1]*(m_{i-3} - m_{i-1})]] + ct*(m_i - m_{i-1})
+ *            (cd[0] from pc >= 2, cd[1] from pc == 3), rounded to the state dtype in registers
+ *   pc = 0 : x_i = x~
+ *   pp > 0 : x~_{i+1} = a*x_i + c0*m_i [+ cp[0]*(m_{i-1} - m_i) [+ cp[1]*(m_{i-2} - m_i)]]  (cp[0] from pp >= 2,
+ *            cp[1] from pp == 3) -> desc->out, and desc->out2 when set (the doubled CFG batch)
+ *   out_c  : optional, receives x_i (intermediates, hooks); required when pp == 0
+ * Differences first, then the sums left to right, each product and sum rounded to fp32. desc->xe, form, c0_on_old
+ * and a, c0..c2, w0..w4 are not read. Returns DPM_ERR_ARG before any launch for pc or pp outside 0..3, pc == pp == 0,
+ * raw_round != 0, dev_coef != NULL, or a NULL operand the orders need. Served by packet kernels for the five dtype
+ * pairs (tails, unaligned views and other pairs by the generic kernel); never by the TMA variant. */
+typedef struct dpm_unipc_desc {
+  const void* m3;   /* m_{i-3}, state dtype; read when pc == 3 */
+  void* out_c;      /* optional: the corrected state x_i      */
+  int32_t pc;       /* corrector order 0..3 (0 = off)         */
+  int32_t pp;       /* predictor order 0..3 (0 = none)        */
+  float cd[2], ct;  /* corrector words                        */
+  float a, c0;      /* predictor words                        */
+  float cp[2];
+} dpm_unipc_desc;
+DPM_API int dpm_step_unipc(const dpm_step_desc* desc, const dpm_unipc_desc* u, dpm_stream_t stream);
 
 /* ---- dpm_solver_adaptive with the controller on the device (:956-1010) -------------------------------------
  * Device buffers (caller-allocated, fp32): state[16] (s, lambda_s, lambda_0, h, t, nfe, done, accept, iterations as
