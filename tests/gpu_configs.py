@@ -106,9 +106,7 @@ class Rig:
 
     def __init__(self, mod, c, device="cpu"):
         self.mod, self.c, self.device, self.calls = mod, c, torch.device(device), None
-        kind, betas = make_betas(c["schedule"])
-        self.ns = mod.NoiseScheduleVP("linear") if kind == "linear" else \
-            mod.NoiseScheduleVP("discrete", betas=torch.from_numpy(betas))
+        self.ns = self.make_schedule()
         B, md, cl = c["B"], DT[c["model_dtype"]], c["channels_last"]
 
         def net(xx, tt, cc=None):
@@ -122,6 +120,7 @@ class Rig:
                 o = o.to(md)
             return o.contiguous(memory_format=torch.channels_last) if cl else o
 
+        self.net = net
         g = c["guidance"]
         if g == "none":
             self.fn = mod.model_wrapper(lambda xx, tt: net(xx, tt), self.ns, model_type=c["model_type"])
@@ -142,6 +141,11 @@ class Rig:
                 scale = torch.tensor(c["scales"], dtype=torch.float32, device=self.device)
         self.scale = scale
         self.fn = mod.model_wrapper(net, self.ns, condition=cond, guidance_scale=scale, **kw)
+
+    def make_schedule(self):
+        kind, betas = make_betas(self.c["schedule"])
+        return self.mod.NoiseScheduleVP("linear") if kind == "linear" else \
+            self.mod.NoiseScheduleVP("discrete", betas=torch.from_numpy(betas))
 
     def solver(self, **kw):
         c = self.c
