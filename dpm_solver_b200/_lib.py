@@ -15,10 +15,10 @@ LIB_PATH = _PKG / "lib" / "libdpmsolver_b200.so"
 # enums (mirror include/dpm_solver_b200.h)
 DPM_F32, DPM_BF16, DPM_F16 = 0, 1, 2
 FORM_NONE, FORM_LIN1, FORM_LIN2, FORM_LIN3, FORM_DIFF2, FORM_MS3, FORM_SS3T = range(7)
-PARAM_NOISE, PARAM_X_START, PARAM_V, PARAM_SCORE, PARAM_FLOW = range(5)
+PARAM_NOISE, PARAM_X_START, PARAM_V, PARAM_SCORE, PARAM_FLOW, PARAM_EDM = range(6)
 
 PARAM_BY_NAME = {"noise": PARAM_NOISE, "x_start": PARAM_X_START, "v": PARAM_V, "score": PARAM_SCORE,
-                 "flow": PARAM_FLOW}
+                 "flow": PARAM_FLOW, "edm": PARAM_EDM}
 
 
 class StepDesc(C.Structure):

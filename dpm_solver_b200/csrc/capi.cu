@@ -95,7 +95,7 @@ static int build_params(const dpm_step_desc* d, KParams* kp, Needs* nd, bool for
   const int form = for_quantile ? DPM_FORM_NONE : d->form;
   if (form < DPM_FORM_NONE || form > DPM_FORM_SS3T) { set_error("bad form %d", form); return DPM_ERR_ARG; }
   if (d->n_model < 0 || d->n_model > 2) { set_error("n_model must be 0, 1 or 2"); return DPM_ERR_ARG; }
-  if (d->param < DPM_PARAM_NOISE || d->param > DPM_PARAM_FLOW) { set_error("bad param %d", d->param); return DPM_ERR_ARG; }
+  if (d->param < DPM_PARAM_NOISE || d->param > DPM_PARAM_EDM) { set_error("bad param %d", d->param); return DPM_ERR_ARG; }
   if (d->raw_round != 0 && ((d->raw_round & ~7) != 0 || ((d->raw_round & 3) != DPM_BF16 && (d->raw_round & 3) != DPM_F16))) {
     set_error("raw_round must be 0 or (DPM_BF16 | DPM_F16) [+ 4]");
     return DPM_ERR_ARG;
@@ -104,7 +104,10 @@ static int build_params(const dpm_step_desc* d, KParams* kp, Needs* nd, bool for
     set_error("raw_round needs an fp32 state and is not available in dpm_dynamic_threshold");
     return DPM_ERR_ARG;
   }
-  if (d->param == DPM_PARAM_FLOW && d->raw_round != 0) { set_error("raw_round is not available with DPM_PARAM_FLOW"); return DPM_ERR_ARG; }
+  if (direct_param(d->param) && d->raw_round != 0) {
+    set_error("raw_round is not available with DPM_PARAM_%s", d->param == DPM_PARAM_FLOW ? "FLOW" : "EDM");
+    return DPM_ERR_ARG;
+  }
   if ((d->n >> 3) > 0xffffffffull) { set_error("n too large (max 2^35-1 elements per call)"); return DPM_ERR_ARG; }
 
   const FormReads reads = form_reads(form);
@@ -114,7 +117,7 @@ static int build_params(const dpm_step_desc* d, KParams* kp, Needs* nd, bool for
   nd->m2 = reads.m2;
   nd->ec = d->n_model >= 1;
   nd->eu = d->n_model == 2;
-  nd->xe = d->n_model >= 1 && (d->param == DPM_PARAM_X_START || d->param == DPM_PARAM_V || d->param == DPM_PARAM_FLOW ||
+  nd->xe = d->n_model >= 1 && (d->param == DPM_PARAM_X_START || d->param == DPM_PARAM_V || direct_param(d->param) ||
                                d->predict_x0);
 
   if (for_quantile) {
@@ -159,7 +162,7 @@ static int build_params(const dpm_step_desc* d, KParams* kp, Needs* nd, bool for
   kp->w0 = d->w0; kp->w1 = d->w1; kp->w2 = d->w2; kp->w3 = d->w3; kp->w4 = d->w4;
   // reciprocal-refinement division (common.cuh: div_const) is used when every divisor the launch
   // can touch qualifies; host IEEE division gives the correctly rounded fp32 reciprocals
-  const bool need_alpha = d->n_model >= 1 && d->predict_x0 && d->param != DPM_PARAM_FLOW;   // FLOW: x0 without :439
+  const bool need_alpha = d->n_model >= 1 && d->predict_x0 && !direct_param(d->param);   // FLOW, EDM: x0 without :439
   const bool need_w4 = form == DPM_FORM_SS3T;
   bool ok = true;
   if (need_alpha) ok = ok && recip_div_ok(d->alpha_e);
@@ -169,6 +172,11 @@ static int build_params(const dpm_step_desc* d, KParams* kp, Needs* nd, bool for
   kp->r_w4 = need_w4 && ok ? 1.0f / d->w4 : 0.f;
   kp->fast_div = ok ? 1 : 0;
   kp->dev_coef = for_quantile ? nullptr : d->dev_coef;
+  if (d->param == DPM_PARAM_EDM) {
+    kp->conv_a = d->alpha_e; kp->conv_b = d->sigma_e;
+  } else if (d->param == DPM_PARAM_FLOW) {
+    kp->conv_a = 1.f; kp->conv_b = d->predict_x0 ? -d->sigma_e : d->alpha_e;
+  }
   return DPM_OK;
 }
 

@@ -64,6 +64,9 @@ struct KParams {
   // per-sample classifier-free guidance (dpm_step_guided): fp32 scale per sample [n/per_sample], in place of
   // `guidance`. Only the <PG = true> instantiations read it; with it, `ratio` may be NULL (no rescale).
   const float* gscale;
+  // FLOW and EDM (direct_param): the conversion v = conv_a*xe + conv_b*out of the packet kernels (flow8), formed on the
+  // host from param, predict_x0 and the by-value alpha_e, sigma_e (build_params). Only flow8 reads them.
+  float conv_a, conv_b;
 };
 
 // multi-condition classifier-free guidance (dpm_step_multi): eps = eps_u; eps = eps + s[k]*(eps_k - eps_u) for k < n_cond,
@@ -305,7 +308,12 @@ __device__ __forceinline__ float min_nan(float a, float b) {
 __device__ __forceinline__ float flow_value(bool x0, float out, float xe, float alpha, float sigma) {
   return x0 ? xe - sigma * out : xe + alpha * out;
 }
-// model_wrapper.noise_pred_fn :288-298. FLOW returns x0 when p.predict_x0 and eps otherwise (finish_x0 then skips :439).
+// FLOW and EDM convert straight into the solver's space: x0 when p.predict_x0, else eps, with no eps -> x0 division
+__host__ __device__ __forceinline__ bool direct_param(int param) {
+  return param == DPM_PARAM_FLOW || param == DPM_PARAM_EDM;
+}
+// model_wrapper.noise_pred_fn :288-298. FLOW and EDM return x0 when p.predict_x0 and eps otherwise (finish_x0 then skips
+// :439); EDM's alpha_e / sigma_e are the host words of that space.
 __device__ __forceinline__ float convert_param(const KParams& p, float out, float xe) {
   const float alpha = p.alpha_e, sigma = p.sigma_e;
   switch (p.param) {
@@ -313,13 +321,14 @@ __device__ __forceinline__ float convert_param(const KParams& p, float out, floa
     case DPM_PARAM_V: return alpha * out + sigma * xe;           // :295
     case DPM_PARAM_SCORE: return (-sigma) * out;                 // :298
     case DPM_PARAM_FLOW: return flow_value(p.predict_x0 != 0, out, xe, alpha, sigma);
+    case DPM_PARAM_EDM: return alpha * xe + sigma * out;
     default: return out;                                         // :289
   }
 }
 // converted and combined prediction -> buffered model value: eps, or x0 (:439, the thresholding clamp :424)
 __device__ __forceinline__ float finish_x0(const KParams& p, float eps, float xe, float thr, bool clamp) {
   if (!p.predict_x0) return eps;
-  float x0 = p.param == DPM_PARAM_FLOW ? eps : (xe - p.sigma_e * eps) / p.alpha_e;  // data_prediction_fn :439
+  float x0 = direct_param(p.param) ? eps : (xe - p.sigma_e * eps) / p.alpha_e;  // data_prediction_fn :439
   if (clamp) x0 = clamp_sym(x0, thr) / thr;  // dynamic_thresholding_fn :424
   return x0;
 }
@@ -442,25 +451,23 @@ __device__ __forceinline__ float update_value(const KParams& p, float x, float T
   return 0.f;
 }
 
-// ---- the fast path: noise- and flow-parameterised networks, exact constant division ------
+// ---- the fast path: noise-, flow- and EDM-parameterised networks, exact constant division ------
 // Launch-uniform switches are taken once per PACKET (uniform branches), every loop below is
-// straight-line code over 8 elements. Callers guarantee: p.param == NOISE or FLOW; p.fast_div when a division
-// is needed (a FLOW conversion has none); a clamp threshold `s` that is uniform over the packet.
-// FLOW converts each output first (flow8: one multiply and one add per element, in the solver's space) and combines the
-// converted values; a rescaled combine runs on the raw outputs and is converted afterwards. ec and eu are overwritten.
+// straight-line code over 8 elements. Callers guarantee: p.param == NOISE, FLOW or EDM; p.fast_div when a division
+// is needed (a FLOW or EDM conversion has none); a clamp threshold `s` that is uniform over the packet.
+// FLOW and EDM convert each output first (flow8, in the solver's space) and combine the converted values; a rescaled
+// combine runs on the raw outputs and is converted afterwards. ec and eu are overwritten.
+// Both are one affine map v = conv_a*xe + conv_b*v with launch-uniform words (KParams::conv_a, conv_b): EDM's
+// (alpha_e, sigma_e), and for FLOW conv_a = 1 with conv_b = -sigma_e (x0) or alpha_e (eps). 1*xe is xe and
+// xe + (-s)*v is xe - s*v exactly, zeros and NaNs included, so a FLOW value is bit for bit flow_value's.
 __device__ __forceinline__ void flow8(const KParams& p, const float (&xe)[8], float (&v)[8]) {
-  if (p.predict_x0) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = xe[i] - p.sigma_e * v[i];
-  } else {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) v[i] = xe[i] + p.alpha_e * v[i];
-  }
+  for (int i = 0; i < 8; ++i) v[i] = p.conv_a * xe[i] + p.conv_b * v[i];
 }
-// combined prediction T -> buffered model value: eps -> x0 (:439; a FLOW value is x0 already) and the clamp (:424)
+// combined prediction T -> buffered model value: eps -> x0 (:439; a FLOW or EDM value is x0 already) and the clamp (:424)
 __device__ __forceinline__ void fast_finish8(const KParams& p, const float (&xe)[8], bool clamp, float s, float (&T)[8]) {
   if (!p.predict_x0) return;
-  if (p.param != DPM_PARAM_FLOW) {
+  if (!direct_param(p.param)) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) T[i] = xe[i] - p.sigma_e * T[i];
     div_const8(T, p.alpha_e, p.r_alpha);  // :439
@@ -483,7 +490,7 @@ template <int NE, bool RS = false, bool PG = false>
 __device__ __forceinline__ void fast_model8(const KParams& p, const float (&xe)[8], float (&ec)[8],
                                             float (&eu)[8], bool clamp, float s, float (&T)[8],
                                             float r = 1.f, float gs = 1.f) {
-  const bool flow = p.param == DPM_PARAM_FLOW;
+  const bool flow = direct_param(p.param);
   const bool raw_combine = RS || (PG && p.ratio != nullptr);   // rescaled: combine the raw outputs, convert after
   if (flow && !raw_combine) {
     flow8(p, xe, ec);
@@ -492,7 +499,7 @@ __device__ __forceinline__ void fast_model8(const KParams& p, const float (&xe)[
   if constexpr (PG) {
     if (gs == 1.f) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) T[i] = ec[i];   // :323 (NOISE: the conversion is the identity; FLOW: done above or below)
+      for (int i = 0; i < 8; ++i) T[i] = ec[i];   // :323 (NOISE: the conversion is the identity; FLOW, EDM: done above or below)
     } else {
 #pragma unroll
       for (int i = 0; i < 8; ++i) T[i] = eu[i] + gs * (ec[i] - eu[i]);  // :330
@@ -548,8 +555,8 @@ __device__ __forceinline__ void fast_update8(const KParams& p, const float (&x)[
 __host__ __forceinline__ bool fast_path_ok(const KParams& p) {
   if (p.form == DPM_FORM_SS3T && !p.fast_div) return false;
   if (p.n_model == 0) return true;
-  if (p.param != DPM_PARAM_NOISE && p.param != DPM_PARAM_FLOW) return false;
-  if (p.param == DPM_PARAM_NOISE && p.predict_x0 && !p.fast_div) return false;   // FLOW: no division by alpha_e
+  if (p.param != DPM_PARAM_NOISE && !direct_param(p.param)) return false;
+  if (p.param == DPM_PARAM_NOISE && p.predict_x0 && !p.fast_div) return false;   // FLOW, EDM: no division by alpha_e
   if ((p.thr != nullptr || p.ratio != nullptr || p.gscale != nullptr) && p.pk_per_sample == 0) return false;
   return true;
 }

@@ -115,7 +115,7 @@ __device__ __forceinline__ void keys_of_packet(const KParams& p, const Raw<TS>& 
 #pragma unroll
   for (int i = 0; i < 8; ++i) fu[i] = 0.f;
   if (NE == 2) unpack(ru, fu);
-  if (p.param == DPM_PARAM_FLOW || (p.fast_div && p.param == DPM_PARAM_NOISE)) {   // (FLOW: x0 without a division)
+  if (direct_param(p.param) || (p.fast_div && p.param == DPM_PARAM_NOISE)) {   // (FLOW, EDM: x0 without a division)
     fast_model8<NE>(p, fx, fc, fu, false, 1.f, fT);
   } else {
 #pragma unroll
@@ -698,7 +698,7 @@ int launch_quantile(float* s_out, const KParams& p, uint64_t n_samples, float q,
     qp.slice = (uint32_t)((ps + per_cta - 1) / per_cta);
     qp.work = static_cast<uint32_t*>(workspace);
     // division-free classification and |numerator| candidates need the plain eps -> x0 map with a positive alpha
-    // (a FLOW x0 has no divisor: its keys are compared with the pivots as they are, keys_of_packet)
+    // (a FLOW or EDM x0 has no divisor: its keys are compared with the pivots as they are, keys_of_packet)
     qp.num_space = (vec && p.param == DPM_PARAM_NOISE && p.predict_x0 && p.alpha_e > 0.f) ? 1u : 0u;
     if (n_samples * qp.slice > 0x7fffffffull) { set_error("too many chunks"); return DPM_ERR_UNSUPPORTED; }
     QKernel kp = p.n_model == 2 ? k_q_pivots<2> : k_q_pivots<1>;

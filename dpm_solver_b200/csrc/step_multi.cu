@@ -17,7 +17,7 @@ namespace dpm {
 constexpr int kMultiUnroll = 2;
 constexpr int kMultiThreads = 256;
 
-// FAST: param == NOISE (the conversion is the identity) or FLOW (each block converted by flow8, one uniform branch per
+// FAST: param == NOISE (the conversion is the identity) or FLOW / EDM (each block converted by flow8, one uniform branch per
 // packet, no division), exact constant division, a clamp threshold uniform per packet (fast_path_ok). FAST = false:
 // every parameterisation, per-element thresholds, IEEE division.
 template <typename TE, typename TS, int FORM, bool FAST>
@@ -80,7 +80,7 @@ __global__ void __launch_bounds__(kMultiThreads) k_step_multi(const __grid_const
         }
         unpack(reu[u], fu);
         if (FAST) {
-          const bool flow = p.param == DPM_PARAM_FLOW;
+          const bool flow = direct_param(p.param);
           if (flow) flow8(p, fxe, fu);
 #pragma unroll
           for (int i = 0; i < 8; ++i) g[i] = fu[i];
@@ -98,7 +98,7 @@ __global__ void __launch_bounds__(kMultiThreads) k_step_multi(const __grid_const
           const float s_thr = clamp ? __ldg(p.thr + (uint32_t)pk / p.pk_per_sample) : 1.f;
 #pragma unroll
           for (int i = 0; i < 8; ++i) fT[i] = g[i];
-          fast_finish8(p, fxe, clamp, s_thr, fT);   // eps->x0 (a FLOW value is x0 already) and the clamp
+          fast_finish8(p, fxe, clamp, s_thr, fT);   // eps->x0 (a FLOW or EDM value is x0 already) and the clamp
         } else {
 #pragma unroll
           for (int i = 0; i < 8; ++i) {

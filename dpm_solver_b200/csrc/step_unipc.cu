@@ -35,7 +35,7 @@ __device__ __forceinline__ float unipc_value(const UniParams& u, float fx, float
   return o;
 }
 
-// FAST: param == NOISE or FLOW, exact constant division, a clamp threshold uniform per packet (fast_path_ok);
+// FAST: param == NOISE, FLOW or EDM, exact constant division, a clamp threshold uniform per packet (fast_path_ok);
 // FAST = false: every parameterisation, per-element thresholds, IEEE division. NE == 0 reads m_i from k.m0.
 template <typename TE, typename TS, int NE, bool FAST>
 __global__ void __launch_bounds__(kUniThreads) k_step_unipc(const __grid_constant__ UniParams up) {

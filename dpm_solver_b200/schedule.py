@@ -1,5 +1,6 @@
 """Noise schedule scalars: log(alpha_t), alpha_t, sigma_t, lambda_t and lambda^-1, for the reference's VP schedules
-(`NoiseScheduleVP`) and for flow-matching models on the linear path (`NoiseScheduleFlow`).
+(`NoiseScheduleVP`), for flow-matching models on the linear path (`NoiseScheduleFlow`) and for EDM-preconditioned
+models (`NoiseScheduleEDM`).
 
 API-compatible with `NoiseScheduleVP` of the reference (dpm_solver_pytorch.py:6-167) -- same
 constructor, attributes and methods -- but every method is a handful of vectorised ops: the
@@ -12,7 +13,7 @@ from __future__ import annotations
 
 import torch
 
-__all__ = ["NoiseScheduleVP", "NoiseScheduleFlow", "interpolate_fn", "expand_dims"]
+__all__ = ["NoiseScheduleVP", "NoiseScheduleFlow", "NoiseScheduleEDM", "interpolate_fn", "expand_dims"]
 
 
 def _piecewise_linear(x: torch.Tensor, xp: torch.Tensor, yp: torch.Tensor) -> torch.Tensor:
@@ -207,3 +208,100 @@ class NoiseScheduleFlow:
     def model_input_time(self, t):
         """What the network receives for the continuous label t: time_scale * sigma_t."""
         return self.time_scale * self.marginal_std(t)
+
+
+class NoiseScheduleEDM:
+    """Schedule of an EDM-preconditioned network (Karras et al. 2022, "Elucidating the Design Space of Diffusion-Based
+    Generative Models"; not in the reference; `schedule == "edm"` is the tag other code switches on). The network is
+    the raw F of
+
+        D(x; s) = c_skip(s)*x + c_out(s)*F(c_in(s)*x, c_noise(s)),   x = x0 + s*n,
+        c_skip = sd^2/(s^2 + sd^2),  c_out = s*sd/sqrt(s^2 + sd^2),  c_in = 1/sqrt(s^2 + sd^2),  c_noise = ln(s)/4
+
+    with sd = sigma_data. The solver integrates in the network's input space y = c_in(s)*x, where
+
+        y_t = alpha_t*x0 + sigma_t*n,   alpha_t = 1/sqrt(s^2 + sd^2),   sigma_t = s/sqrt(s^2 + sd^2),   lambda_t = -ln s,
+
+    so `model_wrapper(..., model_type="edm")` converts F with two words and no division: x0 = (sd^2*alpha_t)*y +
+    (sd*sigma_t)*F and eps = sigma_t*y - (sd*alpha_t)*F. The network receives y and c_noise. Start from
+    x_T = marginal_std(T) * randn (that is, c_in*sigma_max*n); denoise_to_zero=True returns D(.; sigma_min) in data
+    space, which is how Karras's sampler ends.
+
+    The label t in [1/total_N, 1] maps to s by Karras's ramp over u = (t - 1/N)/(1 - 1/N): t = 1 is sigma_max, t = 1/N
+    is sigma_min, and skip_type="time_uniform" between the default ends is Karras's grid.
+
+    Every method is fp32 torch arithmetic on `t` with python-float operands formed in double (c = fl32(1/N), 1 - c,
+    sigma_min^(1/rho), sigma_max^(1/rho) - sigma_min^(1/rho), 1/rho, rho, sd^2), in exactly this order:
+
+        u      = (t - c) / (1. - c)
+        s      = (smin_r + u * span_r) ** rho                      # smin_r = sigma_min^(1/rho), span_r: the difference
+        r      = sqrt(s * s + sd^2)
+        alpha  = 1. / r;   sigma = s / r;   log_alpha = -log(r);   lambda = -log(s)
+        inverse_lambda: s = exp(-lambda);   u = (s ** (1/rho) - smin_r) / span_r;   t = u * (1. - c) + c
+        model input time = 0.25 * log(s)
+    """
+
+    schedule = "edm"
+
+    def __init__(self, sigma_min=0.002, sigma_max=80., sigma_data=0.5, rho=7., total_N=1000):
+        sigma_min, sigma_max, sigma_data, rho = float(sigma_min), float(sigma_max), float(sigma_data), float(rho)
+        if not (0. < sigma_min < sigma_max < float("inf")):
+            raise ValueError("NoiseScheduleEDM: need 0 < sigma_min < sigma_max < inf, got sigma_min={}, sigma_max={}"
+                             .format(sigma_min, sigma_max))
+        if not (0. < sigma_data < float("inf")):
+            raise ValueError("NoiseScheduleEDM: sigma_data must be a positive finite number, got {}".format(sigma_data))
+        if not (0. < rho < float("inf")):
+            raise ValueError("NoiseScheduleEDM: rho must be a positive finite number, got {}".format(rho))
+        if int(total_N) != total_N or total_N < 2:
+            raise ValueError("NoiseScheduleEDM: total_N must be an integer >= 2, got {}".format(total_N))
+        self.sigma_min, self.sigma_max, self.sigma_data, self.rho = sigma_min, sigma_max, sigma_data, rho
+        self.total_N = int(total_N)
+        self.T = 1.
+        self._c = float(torch.tensor(1. / self.total_N, dtype=torch.float32))     # fl32(1/N), the default end label
+        self._smin_r = sigma_min ** (1. / rho)
+        self._span_r = sigma_max ** (1. / rho) - self._smin_r
+        self._sd2 = sigma_data * sigma_data
+
+    def sigma(self, t):
+        """Karras's noise level s(t) (the VE sigma of x = x0 + s*n)."""
+        u = (t - self._c) / (1. - self._c)
+        return (self._smin_r + u * self._span_r) ** self.rho
+
+    def _r(self, s):
+        return torch.sqrt(s * s + self._sd2)
+
+    def marginal_alpha(self, t):
+        return 1. / self._r(self.sigma(t))
+
+    def marginal_std(self, t):
+        s = self.sigma(t)
+        return s / self._r(s)
+
+    def marginal_log_mean_coeff(self, t):
+        return -torch.log(self._r(self.sigma(t)))
+
+    def marginal_lambda(self, t):
+        return -torch.log(self.sigma(t))
+
+    def marginals(self, t):
+        """(log_alpha, sigma, lambda, alpha) of a vector of times in one pass (plan.Marginals)."""
+        s = self.sigma(t)
+        r = self._r(s)
+        return -torch.log(r), s / r, -torch.log(s), 1. / r
+
+    def inverse_lambda(self, lamb):
+        s = torch.exp(-lamb)
+        u = (s ** (1. / self.rho) - self._smin_r) / self._span_r
+        return u * (1. - self._c) + self._c
+
+    def model_input_time(self, t):
+        """What the network receives for the continuous label t: c_noise = ln(s(t))/4."""
+        return 0.25 * torch.log(self.sigma(t))
+
+    def conversion_words(self, alpha, sigma, x0):
+        """The two words of DPM_PARAM_EDM at the fp32 marginals (alpha_t, sigma_t): (sd^2*alpha_t, sd*sigma_t) for x0,
+        (sigma_t, -sd*alpha_t) for eps. Each is formed in double and rounded to fp32 once."""
+        f = lambda v: float(torch.tensor(v, dtype=torch.float64).float())
+        if x0:
+            return f(self._sd2 * alpha), f(self.sigma_data * sigma)
+        return f(sigma), f(-self.sigma_data * alpha)

@@ -27,7 +27,7 @@ import torch
 import torch.distributed as dist
 
 from . import ops, plan as P
-from ._lib import FORM_LIN1, FORM_NONE, FORM_SS3T, PARAM_BY_NAME, PARAM_FLOW, PARAM_NOISE
+from ._lib import FORM_LIN1, FORM_NONE, FORM_SS3T, PARAM_BY_NAME, PARAM_EDM, PARAM_FLOW, PARAM_NOISE
 from .ops import StepArgs
 
 __all__ = ["model_wrapper", "DPM_Solver", "WrappedModel"]
@@ -52,7 +52,7 @@ class RawOutput:
     # and their fp32-rounded scales; `guidance` is then not read
     e_conds: Optional[tuple] = None
     scales: Optional[tuple] = None
-    is_x0: bool = False     # `e_cond` is a materialised x0 (a guided flow prediction): it is only clamped, not converted
+    is_x0: bool = False     # `e_cond` is a materialised x0 (a guided flow or EDM prediction): it is only clamped, not converted
 
 
 def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale):
@@ -156,8 +156,8 @@ class WrappedModel:
         """[1/N, 1] -> [0, 1000*(N-1)/N] for discrete-time models (:271-280)."""
         if self.noise_schedule.schedule == 'discrete':
             return (t_continuous - 1. / self.noise_schedule.total_N) * 1000.
-        if self.noise_schedule.schedule == 'flow':
-            return self.noise_schedule.model_input_time(t_continuous)     # time_scale * sigma_t
+        if self.noise_schedule.schedule in ('flow', 'edm'):
+            return self.noise_schedule.model_input_time(t_continuous)     # time_scale * sigma_t, or ln(s)/4
         return t_continuous
 
     def _call_model(self, x, t_continuous, cond=None, t_input=None):
@@ -315,7 +315,9 @@ class WrappedModel:
         if r.e_uncond is None and r.param == PARAM_NOISE:
             return r.e_cond
         pairs = self._alpha_sigma(t_continuous) if r.param != PARAM_NOISE else [(1.0, 0.0)]
-        needs_x = r.param in (PARAM_BY_NAME["x_start"], PARAM_BY_NAME["v"], PARAM_FLOW)
+        if r.param == PARAM_EDM:
+            pairs = [self.noise_schedule.conversion_words(al, sg, False) for al, sg in pairs]   # eps words
+        needs_x = r.param in (PARAM_BY_NAME["x_start"], PARAM_BY_NAME["v"], PARAM_FLOW, PARAM_EDM)
         xo = x.to(r.e_cond.dtype) if needs_x else None
         ratio = _cfg_ratio(be, r)      # over the whole batch: each sample's ratio reads its own values only
 
@@ -344,6 +346,13 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     combined; guidance_rescale combines and rescales the raw velocities, then converts. A NoiseScheduleFlow also takes
     "noise" and "x_start" networks; "v" and "score" (VP formulas) and guidance_type="classifier" are rejected.
 
+    model_type="edm" (not in the reference; needs a `NoiseScheduleEDM`, which takes no other model type): the network
+    is the raw F of an EDM-preconditioned model and receives the solver's state y = c_in*x and c_noise = ln(s)/4. The
+    solver converts F straight into its own space with two words computed on the host from the fp32 marginals and
+    rounded once: x0 = (sd^2*alpha_t)*y + (sd*sigma_t)*F for dpmsolver++ and denoise_to_zero, eps = sigma_t*y -
+    (sd*alpha_t)*F for dpmsolver (this callable returns the latter), three rounded ops and no division. Guidance works
+    as for "flow"; guidance_type="classifier" and DPM_Solver(reference_rounding=True) are rejected.
+
     guidance_rescale=phi (classifier-free guidance only; not in the reference): guidance rescale of Lin et al.
     2023 as diffusers' `rescale_noise_cfg` does it, in the network's output space (eps for a noise network, v for
     a v network): g = out_u + s*(out_c - out_u), r_b = std(out_c_b)/std(g_b) per sample (unbiased),
@@ -366,7 +375,7 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     torch's eager ops compute it. Every output is combined, whatever the scales (no bypass). One condition in a list is
     exactly the tensor form. With K >= 2: unconditional_condition is required, and guidance_rescale, per-sample scales
     and DPM_Solver(reference_rounding=True) are not available (ValueError)."""
-    assert model_type in ["noise", "x_start", "v", "score", "flow"]
+    assert model_type in ["noise", "x_start", "v", "score", "flow", "edm"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
     flow_schedule = getattr(noise_schedule, "schedule", None) == "flow"
     if model_type == "flow" and not flow_schedule:
@@ -376,6 +385,13 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
                          "'flow', 'noise' or 'x_start'".format(model_type))
     if flow_schedule and guidance_type == "classifier":
         raise ValueError("classifier guidance is not available with a NoiseScheduleFlow")
+    edm_schedule = getattr(noise_schedule, "schedule", None) == "edm"
+    if model_type == "edm" and not edm_schedule:
+        raise ValueError("model_type='edm' needs a NoiseScheduleEDM")
+    if edm_schedule and model_type != "edm":
+        raise ValueError("a NoiseScheduleEDM takes model_type='edm' only, got '{}'".format(model_type))
+    if edm_schedule and guidance_type == "classifier":
+        raise ValueError("classifier guidance is not available with a NoiseScheduleEDM")
     guidance_rescale = float(guidance_rescale)
     if not math.isfinite(guidance_rescale):
         raise ValueError("guidance_rescale must be finite, got {}".format(guidance_rescale))
@@ -447,8 +463,9 @@ class DPM_Solver:
         self.state_dtype = state_dtype
         self.plan_broadcast = bool(plan_broadcast)
         self.reference_rounding = bool(reference_rounding)
-        if self.reference_rounding and getattr(noise_schedule, "schedule", None) == "flow":
-            raise ValueError("reference_rounding=True reproduces the reference, which has no flow schedule")
+        if self.reference_rounding and getattr(noise_schedule, "schedule", None) in ("flow", "edm"):
+            raise ValueError("reference_rounding=True reproduces the reference, which has no {} schedule".format(
+                noise_schedule.schedule))
         if self.reference_rounding and getattr(model_fn, "guidance_rescale", 0) != 0:
             raise ValueError("guidance_rescale is not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "per_sample_guidance", False):
@@ -574,7 +591,8 @@ class DPM_Solver:
                     self.__dict__.pop(name, None)
             return ("discrete", id(la), la._version, id(ta), ta._version, ns.total_N)
         return (getattr(ns, "schedule", None), getattr(ns, "beta_0", None), getattr(ns, "beta_1", None),
-                getattr(ns, "T", None), getattr(ns, "shift", None), getattr(ns, "time_scale", None))
+                getattr(ns, "T", None), getattr(ns, "shift", None), getattr(ns, "time_scale", None)) + \
+            tuple(getattr(ns, k, None) for k in ("sigma_min", "sigma_max", "sigma_data", "rho", "total_N"))
 
     def _plan_id(self, key):
         """Hashable identity of a cached plan (schedule + algorithm + sampling arguments): prepared launches are
@@ -639,7 +657,7 @@ class DPM_Solver:
         """[n_evals, rows] device matrix of model-input times for a whole run (one tiny kernel per
         sample() instead of two per model call); None when the model takes t_continuous itself."""
         w = self._wrapped
-        if not (isinstance(w, WrappedModel) and w.fusable and w.noise_schedule.schedule in ('discrete', 'flow')):
+        if not (isinstance(w, WrappedModel) and w.fusable and w.noise_schedule.schedule in ('discrete', 'flow', 'edm')):
             return None
         t_in = self._upload(w.get_model_input_time(t_host.reshape(-1)), device)   # (t - 1/N) * 1000, fp32, :278
         return t_in[:, None].expand(t_in.shape[0], w.input_rows(batch)).contiguous()
@@ -659,6 +677,8 @@ class DPM_Solver:
                 pass        # (alpha_t, sigma_t) arrive with the launch's device coefficient block (StepArgs.coef_dev)
             else:
                 a.alpha_e, a.sigma_e = alsig if isinstance(alsig, tuple) else self._alpha_sigma(alsig)
+                if raw.param == PARAM_EDM:
+                    a.alpha_e, a.sigma_e = self._wrapped.noise_schedule.conversion_words(a.alpha_e, a.sigma_e, x0)
             a.xe = xe
         return a
 
@@ -743,8 +763,9 @@ class DPM_Solver:
             # sample's scale, as the reference orders it (+1 launch) -- or, with several conditions, their combined
             # noise, each block parameterised first (+1 launch)
             if ratio is None and (raw.guidance_b is not None or raw.e_conds is not None):
-                # (a flow network's outputs are converted to x0 directly and combined as x0: no eps -> x0 follows)
-                flow = raw.param == PARAM_FLOW
+                # (a flow or EDM network's outputs are converted to x0 directly and combined as x0: no eps -> x0
+                # follows)
+                flow = raw.param in (PARAM_FLOW, PARAM_EDM)
                 a = self._conv_args(raw, xe, alsig, torch.float32, flow)
                 if a.xe is not None and a.xe.dtype != torch.float32:
                     a.xe = a.xe.float()
@@ -887,7 +908,19 @@ class DPM_Solver:
 
     # -- reference API: time grids ---------------------------------------------------------------
     def get_time_steps(self, skip_type, t_T, t_0, N, device):
-        """Time grid of N+1 points (:453-480). Computed on the host, moved to `device`."""
+        """Time grid of N+1 points (:453-480). Computed on the host, moved to `device`.
+
+        skip_type='karras' (not in the reference; every schedule): Karras et al.'s rho = 7 spacing of the noise level
+        s = exp(-lambda) (the VE sigma, sigma_t/alpha_t): with lambda_T, lambda_0 taken as 'logSNR' takes them,
+        r = linspace(exp(-lambda_T/7), exp(-lambda_0/7), N+1)^7 in fp32 (ends formed in double) and the grid is
+        inverse_lambda(-log(r)), with no endpoint pinning, like 'logSNR'. This is the "Karras" spacing of DPM-Solver++
+        front ends; on a discrete VP schedule the labels are not rounded to integer timesteps (diffusers rounds them),
+        so the grid differs from diffusers' there."""
+        if skip_type == 'karras':
+            lambda_T = self.noise_schedule.marginal_lambda(torch.tensor(t_T)).item()
+            lambda_0 = self.noise_schedule.marginal_lambda(torch.tensor(t_0)).item()
+            r = torch.linspace(math.exp(-lambda_T / 7.), math.exp(-lambda_0 / 7.), N + 1).pow(7.)
+            return self.noise_schedule.inverse_lambda(-torch.log(r)).to(device)
         if skip_type == 'logSNR':
             lambda_T = self.noise_schedule.marginal_lambda(torch.tensor(t_T))
             lambda_0 = self.noise_schedule.marginal_lambda(torch.tensor(t_0))
@@ -900,7 +933,7 @@ class DPM_Solver:
             return torch.linspace(t_T ** (1. / t_order), t_0 ** (1. / t_order), N + 1).pow(t_order).to(device)
         else:
             raise ValueError("Unsupported skip_type {}, need to be 'logSNR' or 'time_uniform' or "
-                             "'time_quadratic'".format(skip_type))
+                             "'time_quadratic' or 'karras'".format(skip_type))
 
     def get_orders_and_timesteps_for_singlestep_solver(self, steps, order, skip_type, t_T, t_0, device):
         """Orders and outer grid of 'DPM-Solver-fast' (:482-539)."""

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 104 /* 0.1.4: dpm_step_unipc */
+#define DPM_B200_VERSION 105 /* 0.1.5: DPM_PARAM_EDM */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -81,6 +81,13 @@ typedef enum dpm_form {
  * separately rounded ops and no division:
  *   predict_x0 == 1 : x0  = xe - sigma_e*out      (the eps -> x0 division :439 is skipped; the clamp follows)
  *   predict_x0 == 0 : eps = xe + alpha_e*out
+ * DPM_PARAM_EDM (not in the reference): the raw network F of an EDM-preconditioned model (Karras et al. 2022),
+ * D(x; s) = c_skip*x + c_out*F(c_in*x, c_noise), integrated in the network's input space y = c_in*x. alpha_e and
+ * sigma_e then carry two host-computed words instead of the marginals, and the conversion is one affine map in either
+ * space, three separately rounded ops and no division:
+ *   value = alpha_e*xe + sigma_e*out
+ *   predict_x0 == 1 : words (sd^2*alpha_t, sd*sigma_t)  -> x0   (the eps -> x0 division :439 is skipped)
+ *   predict_x0 == 0 : words (sigma_t, -sd*alpha_t)       -> eps
  * Classifier-free guidance in every form converts each output so and combines the converted values
  * (T = T_u + s*(T_c - T_u)); a rescaled step combines and rescales the raw outputs, then converts. */
 typedef enum dpm_param {
@@ -88,7 +95,8 @@ typedef enum dpm_param {
   DPM_PARAM_X_START = 1, /* eps = (xe - alpha*out)/sigma      :292 */
   DPM_PARAM_V = 2,       /* eps = alpha*out + sigma*xe        :295 */
   DPM_PARAM_SCORE = 3,   /* eps = (-sigma)*out                :298 */
-  DPM_PARAM_FLOW = 4     /* x0 = xe - sigma*out  or  eps = xe + alpha*out (see above) */
+  DPM_PARAM_FLOW = 4,    /* x0 = xe - sigma*out  or  eps = xe + alpha*out (see above) */
+  DPM_PARAM_EDM = 5      /* alpha*xe + sigma*out, alpha / sigma the words above      */
 } dpm_param;
 
 /* One fused solver step. With n_model == 0 this is a pure update on buffered model values.
@@ -120,7 +128,7 @@ typedef struct dpm_step_desc {
   int32_t form;        /* dpm_form                                                         */
   int32_t n_model;     /* 0, 1 or 2 raw network outputs                                    */
   int32_t param;       /* dpm_param                                                        */
-  int32_t predict_x0;  /* 1: buffered value is x0 = (xe - sigma_e*eps)/alpha_e :439 (DPM_PARAM_FLOW: see there) */
+  int32_t predict_x0;  /* 1: buffered value is x0 = (xe - sigma_e*eps)/alpha_e :439 (FLOW, EDM: see there) */
   int32_t c0_on_old;   /* DIFF2 only                                                       */
   int32_t raw_round;   /* 0 (default). Reference-rounding mode for networks that return 16-bit NOISE into an
                           fp32 state: bits 0-1 = DPM_BF16 / DPM_F16, the type the raw outputs arrived in --
@@ -130,7 +138,7 @@ typedef struct dpm_step_desc {
                           to that type before the fp32 coefficients widen them. Served by the vector
                           kernels for bf16 / f16 network outputs, else by the generic kernel.          */
   float guidance;      /* CFG scale s: eps = eps_u + s*(eps_c - eps_u) :330                */
-  float alpha_e;       /* alpha, sigma at the model evaluation time                         */
+  float alpha_e;       /* alpha, sigma at the model evaluation time (DPM_PARAM_EDM: its two words) */
   float sigma_e;
   float a, c0, c1, c2; /* update coefficients (signs folded in)                            */
   float w0, w1, w2, w3, w4;
