@@ -99,6 +99,9 @@ PROTOTYPES = {
     "dpm_step_multi": (C.c_int, [C.POINTER(StepDesc), C.POINTER(_vp), C.POINTER(_f), _i, C.POINTER(_vp), _vp]),
     "dpm_replicate": (C.c_int, [_vp, _vp, _u64, _i, _i, _vp]),
     "dpm_step_unipc": (C.c_int, [C.POINTER(StepDesc), C.POINTER(UniDesc), _vp]),
+    "dpm_apg_workspace": (C.c_size_t, [_u64, _u64]),
+    "dpm_apg_words": (C.c_int, [_vp, C.POINTER(StepDesc), _vp, _f, _f, _f, _vp, _vp, _vp, C.c_size_t, _vp]),
+    "dpm_step_apg": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _vp, _f, _f, _vp]),
 }
 
 MAX_CONDITIONS = 4      # DPM_MAX_CONDITIONS

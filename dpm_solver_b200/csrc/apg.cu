@@ -1,0 +1,186 @@
+// apg.cu -- the per-sample words of adaptive projected guidance (dpm_apg_words; Sadat, Hilliges and Weber,
+// "Eliminating Oversaturation and Artifacts of High Guidance Scales in Diffusion Models", ICLR 2025):
+//   c = x0(out_c), u = x0(out_u), D = c - u                       (the step's conversion, each op rounded)
+//   R = D, or R = D + beta*R_prev                                  (momentum; written to r_out when set)
+//   k = min(1, r/||R||) (r > 0), p = <R, c>/max(||c||, 1e-12)^2
+//   A = 1 - (w - 1)*(1 - eta)*k*p,  B = (w - 1)*k                  (fp64, each rounded to fp32 once)
+// so that the step's guided prediction c + (w - 1)*(k*R - (1 - eta)*k*p*c) is A*c + B*R.
+// Same chunking as the rescale ratio (adaptive.cu): CTA (b, c) reduces chunk c of sample b to three fp64 partials, the
+// final kernel merges a sample's chunks in chunk order. Every thread owns the same elements on the vector and the
+// element-wise path and every sum runs in a fixed order, so the words of sample b depend on its values only.
+// Algorithmic bytes per element: x, out_c, out_u read, plus 4 + 4 of R_prev / R with momentum.
+#include "common.cuh"
+#include "launch.cuh"
+
+namespace dpm {
+
+constexpr int kAThreads = 256;
+constexpr int kAChunk = 8192;   // elements per CTA
+
+struct AParams {
+  KParams k;             // xe, ec, eu, param, alpha_e, sigma_e (x0 words), guidance, dtypes, dev_coef
+  const float* gscale;   // per-sample scales [n_samples], or NULL: k.guidance
+  const float* r_prev;   // NULL: R = D
+  float* r_out;          // NULL: R is not written
+  double* partial;       // [n_samples * chunks][3]: ||R||^2, <R, c>, ||c||^2
+  float* words;          // [2][n_samples]
+  uint64_t per_sample;
+  uint64_t n_samples;
+  uint32_t chunks;       // per sample
+  float eta, norm_threshold, momentum;
+};
+
+// deterministic CTA sum of one double per thread (butterfly within the warps, then the warps in order)
+__device__ __forceinline__ double apg_cta_sum(double v, double* warp_part) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();   // warp_part may still be read from the previous call
+  if ((threadIdx.x & 31) == 0) warp_part[threadIdx.x >> 5] = v;
+  __syncthreads();
+  double s = 0.0;
+#pragma unroll
+  for (int w = 0; w < kAThreads / 32; ++w) s += warp_part[w];
+  return s;
+}
+
+// VEC: per_sample % 8 == 0 and every operand aligned; TE, TS the packet pair. Otherwise element-wise (load_any).
+template <typename TE, typename TS, bool VEC>
+__global__ void __launch_bounds__(kAThreads) k_apg_partial(const __grid_constant__ AParams p) {
+  __shared__ double warp_part[kAThreads / 32];
+  KParams k = p.k;
+  if (k.dev_coef != nullptr) { k.alpha_e = k.dev_coef[9]; k.sigma_e = k.dev_coef[10]; }
+  const uint64_t sample = blockIdx.x / p.chunks;
+  const uint32_t chunk = blockIdx.x % p.chunks;
+  const uint64_t c_begin = (uint64_t)chunk * kAChunk;
+  const uint64_t c_end = c_begin + kAChunk < p.per_sample ? c_begin + kAChunk : p.per_sample;
+  const uint32_t cnt = (uint32_t)(c_end - c_begin);
+  const size_t e0 = sample * p.per_sample + c_begin;
+  const int tid = threadIdx.x;
+  constexpr int U = kAChunk / kPacket / kAThreads;   // 4
+  double srr = 0.0, src = 0.0, scc = 0.0;
+  auto term = [&](float xe, float oc, float ou, float rp, float& R) {
+    const float c = apg_x0(k, oc, xe);
+    const float D = c - apg_x0(k, ou, xe);
+    R = p.r_prev != nullptr ? D + p.momentum * rp : D;
+    srr += (double)R * (double)R;
+    src += (double)R * (double)c;
+    scc += (double)c * (double)c;
+  };
+  // element (u, i) of this thread is chunk element (u*kAThreads + tid)*8 + i on both paths
+#pragma unroll
+  for (int u = 0; u < U; ++u) {
+    const uint32_t pk = u * kAThreads + tid;
+    if (VEC) {
+      if (pk * kPacket < cnt) {
+        const size_t e = e0 + (size_t)pk * kPacket;
+        Raw<TS> rx;
+        Raw<TE> rc, ru;
+        Raw<float> rp;
+        ldg_pk(rx, static_cast<const TS*>(k.xe) + e);
+        ldg_pk(rc, static_cast<const TE*>(k.ec) + e);
+        ldg_pk(ru, static_cast<const TE*>(k.eu) + e);
+        if (p.r_prev != nullptr) ldg_pk(rp, p.r_prev + e);
+        float fx[8], fc[8], fu[8], fp[8], fr[8];
+        unpack(rx, fx);
+        unpack(rc, fc);
+        unpack(ru, fu);
+        if (p.r_prev != nullptr) unpack(rp, fp);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) term(fx[i], fc[i], fu[i], p.r_prev != nullptr ? fp[i] : 0.f, fr[i]);
+        if (p.r_out != nullptr) {
+          Raw<float> ro;
+          pack(ro, fr);
+          stg_pk(p.r_out + e, ro);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const uint32_t j = pk * kPacket + i;
+        if (j < cnt) {
+          const size_t e = e0 + j;
+          float R;
+          term(load_any(k.xe, k.state_dtype, e), load_any(k.ec, k.model_dtype, e), load_any(k.eu, k.model_dtype, e),
+               p.r_prev != nullptr ? p.r_prev[e] : 0.f, R);
+          if (p.r_out != nullptr) p.r_out[e] = R;
+        }
+      }
+    }
+  }
+  srr = apg_cta_sum(srr, warp_part);
+  src = apg_cta_sum(src, warp_part);
+  scc = apg_cta_sum(scc, warp_part);
+  if (tid == 0) {
+    double* o = p.partial + (size_t)blockIdx.x * 3;
+    o[0] = srr; o[1] = src; o[2] = scc;
+  }
+}
+
+__global__ void __launch_bounds__(kAThreads) k_apg_final(const __grid_constant__ AParams p) {
+  const uint64_t b = (uint64_t)blockIdx.x * kAThreads + threadIdx.x;
+  if (b >= p.n_samples) return;
+  const double* part = p.partial + b * p.chunks * 3;
+  double srr = 0.0, src = 0.0, scc = 0.0;
+  for (uint32_t c = 0; c < p.chunks; ++c) {
+    srr += part[c * 3];
+    src += part[c * 3 + 1];
+    scc += part[c * 3 + 2];
+  }
+  double kk = 1.0;
+  if (p.norm_threshold > 0.f) {
+    const double q = (double)p.norm_threshold / sqrt(srr);
+    kk = q < 1.0 ? q : 1.0;
+  }
+  const double sc = sqrt(scc);
+  const double nc = sc < 1e-12 ? 1e-12 : sc;                 // F.normalize's epsilon (a NaN norm stays NaN)
+  const double proj = src / (nc * nc);
+  const double w = (double)(p.gscale != nullptr ? p.gscale[b] : p.k.guidance);
+  const double A = 1.0 - (w - 1.0) * (1.0 - (double)p.eta) * kk * proj;
+  const double B = (w - 1.0) * kk;
+  p.words[b] = (float)A;
+  p.words[p.n_samples + b] = (float)B;
+}
+
+size_t apg_workspace_bytes(uint64_t n_samples, uint64_t per_sample) {
+  if (per_sample == 0 || n_samples == 0) return 0;
+  const uint64_t chunks = (per_sample + kAChunk - 1) / kAChunk;
+  return (size_t)(n_samples * chunks) * 3 * sizeof(double);
+}
+
+int launch_apg_words(float* words, const KParams& kp, const float* gscale, float eta, float norm_threshold,
+                     float momentum, const float* r_prev, float* r_out, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  AParams p;
+  memset(&p, 0, sizeof(p));
+  p.k = kp;
+  p.gscale = gscale; p.r_prev = r_prev; p.r_out = r_out; p.words = words;
+  p.per_sample = kp.per_sample; p.n_samples = kp.n / kp.per_sample;
+  p.chunks = (uint32_t)((p.per_sample + kAChunk - 1) / kAChunk);
+  p.eta = eta; p.norm_threshold = norm_threshold; p.momentum = momentum;
+  p.partial = static_cast<double*>(ws);
+  if (ws == nullptr || ws_bytes < apg_workspace_bytes(p.n_samples, p.per_sample) ||
+      (reinterpret_cast<uintptr_t>(ws) & 7)) {
+    set_error("apg words: workspace too small or not 8-byte aligned");
+    return DPM_ERR_ARG;
+  }
+  if (p.n_samples * p.chunks > 0x7fffffffull) { set_error("apg words: too many chunks"); return DPM_ERR_UNSUPPORTED; }
+  auto al = [](const void* q, int dt) { return (reinterpret_cast<uintptr_t>(q) & (dt == DPM_F32 ? 31 : 15)) == 0; };
+  const bool vec = p.per_sample % kPacket == 0 && al(kp.xe, kp.state_dtype) && al(kp.ec, kp.model_dtype) &&
+                   al(kp.eu, kp.model_dtype) && (r_prev == nullptr || al(r_prev, DPM_F32)) &&
+                   (r_out == nullptr || al(r_out, DPM_F32));
+  typedef void (*AKernel)(const AParams);
+  AKernel k = nullptr;
+  if (vec) {
+    k = with_packet_pair(kp.model_dtype, kp.state_dtype, [&](auto pair) -> AKernel {
+      using Pair = decltype(pair);
+      return k_apg_partial<typename Pair::TE, typename Pair::TS, true>;
+    });
+  }
+  if (k == nullptr) k = k_apg_partial<float, float, false>;   // any dtype pair, alignment or sample size
+  k<<<(unsigned)(p.n_samples * p.chunks), kAThreads, 0, stream>>>(p);
+  k_apg_final<<<(unsigned)((p.n_samples + kAThreads - 1) / kAThreads), kAThreads, 0, stream>>>(p);
+  count_launch();
+  count_launch();
+  return DPM_OK;
+}
+
+}  // namespace dpm

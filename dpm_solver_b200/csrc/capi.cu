@@ -222,15 +222,36 @@ struct Rescale {
   float phi, psi;
 };
 
+// apg (optional): adaptive projected guidance of an n_model == 2 step -- words [2][n/per_sample], the direction r (or
+// NULL) and the marginals of the x0 -> eps conversion
+struct Apg {
+  const float* words;
+  const float* r;
+  float alpha_t, sigma_t;
+};
+
 // gscale (optional): per-sample guidance of an n_model == 2 step, fp32 [n/per_sample]; rs then may be NULL
 static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale* rs = nullptr,
-                     const float* gscale = nullptr) {
+                     const float* gscale = nullptr, const Apg* apg = nullptr) {
   KParams p;
   Needs nd;
   if (d != nullptr && d->n == 0) return DPM_OK;  // empty tensors: nothing to do (pointers may be NULL)
-  int rc = build_params(d, &p, &nd, false);
+  dpm_step_desc dx;
+  if (apg != nullptr) {   // both halves are converted to x0 whatever the step buffers: validated as a predict_x0 step
+    dx = *d;
+    dx.predict_x0 = 1;
+  }
+  int rc = build_params(apg != nullptr ? &dx : d, &p, &nd, false);
   if (rc != DPM_OK) return rc;
   if (p.n == 0) return DPM_OK;
+  if (apg != nullptr) {
+    p.predict_x0 = d->predict_x0 ? 1 : 0;
+    p.apg_a = apg->words;
+    p.apg_b = apg->words + d->n / d->per_sample;
+    p.apg_r = apg->r;
+    p.apg_alpha = apg->alpha_t;
+    p.apg_sigma = apg->sigma_t;
+  }
   if (rs != nullptr) {
     if (rs->ratio == nullptr || d->n_model != 2 || d->raw_round != 0 || d->per_sample == 0 || d->n % d->per_sample) {
       set_error("rescaled step: needs ratio, n_model == 2, raw_round == 0 and per_sample dividing n");
@@ -242,13 +263,15 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale*
   Tuning t{g_variant.load(), g_threads.load(), g_ctas.load()};
 
   bool body_done = false;
-  if (p.npk > 0 && all_aligned(p, nd) && p.dev_coef == nullptr) {   // device-side scalars: generic kernel only
+  const bool aligned_all = all_aligned(p, nd) && (p.apg_r == nullptr || aligned(p.apg_r, DPM_F32));
+  if (p.npk > 0 && aligned_all && p.dev_coef == nullptr) {   // device-side scalars: generic kernel only
     int r = 1;
     // auto: the direct variant for every launch. On H100 its one-tile-per-CTA grid streams the 16-bit steps
     // faster than the ring (DESIGN.md §4); the ring runs when it is asked for
     const bool tma = p.raw_round == 0 &&   // reference-rounding mode: the direct variant's <RND> kernels
                      p.ratio == nullptr &&  // guidance rescale: the direct variant's <RS> kernels
                      p.gscale == nullptr &&  // per-sample guidance: the direct variant's <PG> kernels
+                     p.apg_a == nullptr &&   // adaptive projected guidance: the direct variant's <APG> kernels
                      t.variant == 1;
     if (tma) r = launch_step_tma(p, t, stream);
     if (r == 1) r = launch_step_direct(p, t, stream);
@@ -448,6 +471,51 @@ int dpm_cfg_rescale_ratio_guided(float* ratio_out, const void* e_cond, const voi
   if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) { set_error("cfg rescale: bad dtype or sizes"); return DPM_ERR_ARG; }
   return finish(launch_cfg_rescale_ratio(ratio_out, e_cond, e_uncond, 0.f, per_sample, n, model_dtype, workspace,
                                          workspace_bytes, static_cast<cudaStream_t>(stream), guidance));
+}
+
+size_t dpm_apg_workspace(uint64_t n_samples, uint64_t per_sample) {
+  return apg_workspace_bytes(n_samples, per_sample);
+}
+
+// the checks both APG entries share: a CFG pair of whole samples, no reference rounding, no EDM words from dev_coef
+static int apg_check(const dpm_step_desc* desc, const float* words, const char* what) {
+  if (desc == nullptr || words == nullptr || desc->n_model != 2 || desc->raw_round != 0 || desc->per_sample == 0 ||
+      desc->n % desc->per_sample) {
+    set_error("%s: needs words, n_model == 2, raw_round == 0 and per_sample dividing n", what);
+    return DPM_ERR_ARG;
+  }
+  if (desc->param == DPM_PARAM_EDM && desc->dev_coef != nullptr) {
+    set_error("%s: DPM_PARAM_EDM takes its words by value, not from dev_coef", what);
+    return DPM_ERR_ARG;
+  }
+  return DPM_OK;
+}
+
+int dpm_apg_words(float* words, const dpm_step_desc* desc, const float* guidance, float eta, float norm_threshold,
+                  float momentum, const float* r_prev, float* r_out, void* workspace, size_t workspace_bytes,
+                  dpm_stream_t stream) {
+  if (desc != nullptr && desc->n == 0) return DPM_OK;
+  int rc = apg_check(desc, words, "apg words");
+  if (rc != DPM_OK) return rc;
+  dpm_step_desc d = *desc;
+  d.predict_x0 = 1;           // the halves are converted to x0 (xe is read)
+  KParams kp;
+  Needs nd;
+  rc = build_params(&d, &kp, &nd, true);   // the quantile's validation: form, thr and outputs are not read
+  if (rc != DPM_OK) return rc;
+  kp.dev_coef = desc->dev_coef;
+  return finish(launch_apg_words(words, kp, guidance, eta, norm_threshold, momentum, r_prev, r_out, workspace,
+                                 workspace_bytes, static_cast<cudaStream_t>(stream)));
+}
+
+int dpm_step_apg(const dpm_step_desc* desc, const float* words, const float* guidance, const float* r, float alpha_t,
+                 float sigma_t, dpm_stream_t stream) {
+  if (desc != nullptr && desc->n == 0) return DPM_OK;
+  int rc = apg_check(desc, words, "apg step");
+  if (rc != DPM_OK) return rc;
+  if (desc->thr != nullptr && !desc->predict_x0) { set_error("apg step: thr requires predict_x0"); return DPM_ERR_ARG; }
+  const Apg apg{words, r, alpha_t, sigma_t};
+  return step_impl(desc, static_cast<cudaStream_t>(stream), nullptr, guidance, &apg);
 }
 
 static dpm_step_desc base_desc(void* out, const void* x, uint64_t n, int dtype, int form) {

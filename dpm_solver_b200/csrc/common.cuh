@@ -67,6 +67,14 @@ struct KParams {
   // FLOW and EDM (direct_param): the conversion v = conv_a*xe + conv_b*out of the packet kernels (flow8), formed on the
   // host from param, predict_x0 and the by-value alpha_e, sigma_e (build_params). Only flow8 reads them.
   float conv_a, conv_b;
+  // adaptive projected guidance (dpm_step_apg): the per-sample words A_b = apg_a[b], B_b = apg_b[b] of dpm_apg_words,
+  // the fp32 guidance direction R (NULL: R = x0_c - x0_u from e_uncond), and the marginals of the x0 -> eps conversion
+  // (predict_x0 == 0). `gscale`, when set, marks the samples whose scale is 1 (bypass). Only the <APG = true>
+  // instantiations read them.
+  const float* apg_a;
+  const float* apg_b;
+  const float* apg_r;
+  float apg_alpha, apg_sigma;
 };
 
 // multi-condition classifier-free guidance (dpm_step_multi): eps = eps_u; eps = eps + s[k]*(eps_k - eps_u) for k < n_cond,
@@ -394,6 +402,30 @@ __device__ __forceinline__ float model_value(const KParams& p, float xe, float e
     }
   }
   return finish_x0(p, eps, xe, thr, clamp);
+}
+
+// ---- adaptive projected guidance (Sadat et al. 2025) ------------------------------------------------------------
+// one network output -> the denoised prediction by the step's parameterisation, each op rounded: FLOW x0 = xe -
+// sigma_e*out, EDM alpha_e*xe + sigma_e*out with the x0 words, every other one converted to eps (:288-298) and then to
+// x0 (:439). alpha_e, sigma_e are those of a predict_x0 step, whatever the launch buffers.
+__device__ __forceinline__ float apg_x0(const KParams& p, float out, float xe) {
+  if (p.param == DPM_PARAM_FLOW) return xe - p.sigma_e * out;
+  const float v = convert_param(p, out, xe);
+  return p.param == DPM_PARAM_EDM ? v : (xe - p.sigma_e * v) / p.alpha_e;
+}
+// the guided denoised prediction A*c + B*R (c for a bypassed sample), then the buffered value: x0 with the clamp
+// (:424), or eps by the x_start conversion with the marginals apg_alpha, apg_sigma (:292). `ru` is R when has_r, else
+// the unconditional output.
+__device__ __forceinline__ float apg_value(const KParams& p, float xe, float ec, float ru, bool has_r, float A, float B,
+                                           bool bypass, float thr, bool clamp) {
+  const float c = apg_x0(p, ec, xe);
+  float g = c;
+  if (!bypass) {
+    const float R = has_r ? ru : c - apg_x0(p, ru, xe);
+    g = A * c + B * R;
+  }
+  if (p.predict_x0) return clamp ? clamp_sym(g, thr) / thr : g;
+  return (xe - p.apg_alpha * g) / p.apg_sigma;
 }
 
 // round a packet to its storage type once: returns the packed words and rewrites f[] with the

@@ -131,5 +131,8 @@ size_t cfg_rescale_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
 int launch_cfg_rescale_ratio(float* ratio, const void* ec, const void* eu, float guidance, uint64_t per_sample,
                              uint64_t n, int dtype, void* ws, size_t ws_bytes, cudaStream_t stream,
                              const float* gscale = nullptr);
+size_t apg_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
+int launch_apg_words(float* words, const KParams& kp, const float* gscale, float eta, float norm_threshold,
+                     float momentum, const float* r_prev, float* r_out, void* ws, size_t ws_bytes, cudaStream_t stream);
 
 }  // namespace dpm

@@ -21,9 +21,11 @@ constexpr int kMaxThreads = 512;
 // like the per-sample thresholds.
 // PG (only with NE == 2, RND = false and RS = false): per-sample guidance (dpm_step_guided) with the scale p.gscale
 // and, when p.ratio is set, the rescale -- one kernel family for rescale on and off.
-template <typename TE, typename TS, int NE, int FORM, bool FAST, bool RND = false, bool RS = false, bool PG = false>
-__global__ void __launch_bounds__(kMaxThreads)
-    k_step_direct(const __grid_constant__ KParams p) {
+// APG (only with NE == 2, FAST = false and no other option; the kernel k_step_direct_apg): adaptive projected guidance
+// (dpm_step_apg) with the per-sample words p.apg_a / p.apg_b; reads the fp32 direction p.apg_r in place of e_uncond
+// when it is set.
+template <typename TE, typename TS, int NE, int FORM, bool FAST, bool RND, bool RS, bool PG, bool APG>
+__device__ __forceinline__ void step_direct_body(const KParams& p) {
   constexpr bool kX = form_reads(FORM).x, kM1 = form_reads(FORM).m1, kM2 = form_reads(FORM).m2;
   const TS* __restrict__ gx = static_cast<const TS*>(p.x);
   const TS* __restrict__ gxe = static_cast<const TS*>(p.xe);
@@ -40,6 +42,7 @@ __global__ void __launch_bounds__(kMaxThreads)
   const uint32_t tile_pk = blockDim.x * kUnroll;
   const bool sep_xe = (NE > 0) && p.use_xe && !(kX && p.xe_is_x);
   const bool clamp = (NE > 0) && (p.thr != nullptr);
+  const bool apg_r = APG && p.apg_r != nullptr;
   pdl_trigger();
   pdl_wait();
 
@@ -47,6 +50,7 @@ __global__ void __launch_bounds__(kMaxThreads)
        tile0 += (uint64_t)gridDim.x * tile_pk) {
     Raw<TS> rx[kUnroll], rxe[kUnroll], rm0[kUnroll], rm1[kUnroll], rm2[kUnroll];
     Raw<TE> rec[kUnroll], reu[kUnroll];
+    Raw<float> rr[APG ? kUnroll : 1];
     // ---- issue every load of the tile ----
 #pragma unroll
     for (int u = 0; u < kUnroll; ++u) {
@@ -56,7 +60,12 @@ __global__ void __launch_bounds__(kMaxThreads)
         if (kX) ldg_pk(rx[u], gx + e);
         if (NE > 0) {
           ldg_pk(rec[u], gec + e);
-          if (NE == 2) ldg_pk(reu[u], geu + e);
+          if constexpr (APG) {
+            if (apg_r) ldg_pk(rr[u], p.apg_r + e);
+            else ldg_pk(reu[u], geu + e);
+          } else if (NE == 2) {
+            ldg_pk(reu[u], geu + e);
+          }
           if (sep_xe) ldg_pk(rxe[u], gxe + e);
         } else {
           ldg_pk(rm0[u], gm0 + e);
@@ -104,7 +113,12 @@ __global__ void __launch_bounds__(kMaxThreads)
         } else if (NE > 0) {
           float fec[8], feu[8];
           unpack(rec[u], fec);
-          if (NE == 2) unpack(reu[u], feu);
+          if constexpr (APG) {
+            if (apg_r) unpack(rr[u], feu);
+            else unpack(reu[u], feu);
+          } else if (NE == 2) {
+            unpack(reu[u], feu);
+          }
           if (sep_xe) {
             unpack(rxe[u], fxe);
           } else if (kX) {
@@ -114,7 +128,15 @@ __global__ void __launch_bounds__(kMaxThreads)
 #pragma unroll
             for (int i = 0; i < 8; ++i) fxe[i] = 0.f;
           }
-          if constexpr (PG) {
+          if constexpr (APG) {
+            // samples hold whole packets here (pick_direct): the sample's words, bypass and threshold are one scalar each
+            const uint32_t b = (uint32_t)(pk / p.pk_per_sample);
+            const float A = __ldg(p.apg_a + b), B = __ldg(p.apg_b + b);
+            const bool bypass = p.gscale != nullptr && __ldg(p.gscale + b) == 1.f;
+            const float tpk = clamp ? __ldg(p.thr + b) : 1.f;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) fT[i] = apg_value(p, fxe[i], fec[i], feu[i], apg_r, A, B, bypass, tpk, clamp);
+          } else if constexpr (PG) {
             // samples hold whole packets here (pick_direct): the sample's scale, ratio (when the launch is rescaled) and
             // threshold are one scalar each per packet
             const uint32_t b = (uint32_t)(pk / p.pk_per_sample);
@@ -189,13 +211,23 @@ __global__ void __launch_bounds__(kMaxThreads)
   }
 }
 
+template <typename TE, typename TS, int NE, int FORM, bool FAST, bool RND = false, bool RS = false, bool PG = false>
+__global__ void __launch_bounds__(kMaxThreads) k_step_direct(const __grid_constant__ KParams p) {
+  step_direct_body<TE, TS, NE, FORM, FAST, RND, RS, PG, false>(p);
+}
+template <typename TE, typename TS, int FORM>
+__global__ void __launch_bounds__(kMaxThreads) k_step_direct_apg(const __grid_constant__ KParams p) {
+  step_direct_body<TE, TS, 2, FORM, false, false, false, false, true>(p);
+}
+
 // ---- fully generic element-wise kernel: any dtype mix, any alignment, tails ------------------
 // RND = true: reference-rounding mode (common.cuh) for the launches the <RND> vector kernels do not serve:
 // unaligned views, tails and fp32 network outputs.
 // RS = true: guidance rescale (n_model == 2) for unaligned views, tails and dev_coef launches.
 // PG = true: per-sample guidance (n_model == 2; rescale iff p.ratio is set), likewise.
-template <bool RND, bool RS = false, bool PG = false>
-__global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KParams pc) {
+// APG = true (the kernel k_step_scalar_apg): adaptive projected guidance (n_model == 2), likewise.
+template <bool RND, bool RS, bool PG, bool APG>
+__device__ __forceinline__ void step_scalar_body(const KParams& pc) {
   KParams p = pc;
   if (pc.dev_coef != nullptr) {
     // scalars produced on the device by the adaptive controller (adaptive_ctl.cu: CO_* layout)
@@ -204,6 +236,7 @@ __global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KPa
     p.w0 = c[4]; p.w1 = c[5]; p.w2 = c[6]; p.w3 = c[7]; p.w4 = c[8];
     p.alpha_e = c[9]; p.sigma_e = c[10];
     p.fast_div = 0;
+    if (APG) { p.apg_alpha = c[9]; p.apg_sigma = c[10]; }   // (no EDM launch takes dev_coef: the marginals)
   }
   const int sd = p.state_dtype, md = p.model_dtype;
   const FormReads reads = form_reads(p.form);
@@ -218,10 +251,16 @@ __global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KPa
     if (p.n_model > 0) {
       float xe = p.use_xe ? ((need_x && p.xe_is_x) ? x : load_any(p.xe, sd, i)) : 0.f;
       float ec = load_any(p.ec, md, i);
-      float eu = p.n_model == 2 ? load_any(p.eu, md, i) : 0.f;
+      const bool apg_r = APG && p.apg_r != nullptr;
+      float eu = p.n_model == 2 && !apg_r ? load_any(p.eu, md, i) : 0.f;
       float thr = clamp ? p.thr[(i + p.elem_offset) / p.per_sample] : 1.f;
       float mv;
-      if constexpr (PG) {
+      if constexpr (APG) {
+        const uint64_t b = (i + p.elem_offset) / p.per_sample;
+        const bool bypass = p.gscale != nullptr && p.gscale[b] == 1.f;
+        mv = apg_value(p, xe, ec, apg_r ? p.apg_r[i + p.elem_offset] : eu, apg_r, p.apg_a[b], p.apg_b[b], bypass, thr,
+                       clamp);
+      } else if constexpr (PG) {
         const uint64_t b = (i + p.elem_offset) / p.per_sample;
         mv = model_value<2, false, false, kPgAny>(p, xe, ec, eu, thr, clamp, p.ratio != nullptr ? p.ratio[b] : 1.f,
                                                   p.gscale[b]);
@@ -251,6 +290,14 @@ __global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KPa
   }
 }
 
+template <bool RND, bool RS = false, bool PG = false>
+__global__ void __launch_bounds__(256) k_step_scalar(const __grid_constant__ KParams pc) {
+  step_scalar_body<RND, RS, PG, false>(pc);
+}
+__global__ void __launch_bounds__(256) k_step_scalar_apg(const __grid_constant__ KParams pc) {
+  step_scalar_body<false, false, false, true>(pc);
+}
+
 // ---- dispatch ---------------------------------------------------------------------------------
 typedef void (*StepKernel)(const KParams);
 
@@ -259,13 +306,22 @@ typedef void (*StepKernel)(const KParams);
 // (NE == 0, differences rounded).
 // RS: guidance rescale, NE == 2 only (the C-ABI rejects it together with raw_round).
 // PG: per-sample guidance, NE == 2 only; serves rescaled and plain launches alike (so it is tested before RS).
+// APG: adaptive projected guidance, NE == 2 only, on the IEEE-division instantiations (tested first: it carries gscale
+// for its bypass).
 static StepKernel pick_direct(const KParams& p) {
   const bool fast = fast_path_ok(p), rnd = p.raw_round != 0, rs = p.ratio != nullptr, pg = p.gscale != nullptr;
-  if (pg && p.pk_per_sample == 0) return nullptr;
+  const bool apg = p.apg_a != nullptr;
+  if ((pg || apg) && p.pk_per_sample == 0) return nullptr;
   return pick_step<StepKernel>(p, [&](auto pair, auto ne, auto form) -> StepKernel {
     using TE = typename decltype(pair)::TE;
     using TS = typename decltype(pair)::TS;
     constexpr int NE = decltype(ne)::value, FORM = decltype(form)::value;
+    if (apg) {   // samples that do not hold whole packets: the generic kernel (k_step_scalar_apg)
+      if constexpr (NE == 2)
+        return k_step_direct_apg<TE, TS, FORM>;
+      else
+        return nullptr;
+    }
     if (pg) {   // samples that do not hold whole packets: the generic kernel (k_step_scalar<PG>)
       if constexpr (NE == 2)
         return fast ? k_step_direct<TE, TS, 2, FORM, true, false, false, true>
@@ -318,6 +374,7 @@ int launch_step_scalar(const KParams& p, cudaStream_t stream) {
   uint64_t cap = (uint64_t)sm_count() * 8;
   uint32_t grid = (uint32_t)(blocks < cap ? blocks : cap);
   if (p.raw_round) k_step_scalar<true><<<grid, threads, 0, stream>>>(p);
+  else if (p.apg_a) k_step_scalar_apg<<<grid, threads, 0, stream>>>(p);
   else if (p.gscale) k_step_scalar<false, false, true><<<grid, threads, 0, stream>>>(p);
   else if (p.ratio) k_step_scalar<false, true><<<grid, threads, 0, stream>>>(p);
   else k_step_scalar<false><<<grid, threads, 0, stream>>>(p);

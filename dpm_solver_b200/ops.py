@@ -8,6 +8,7 @@ install another executor with `set_backend()` to exercise the host-side logic wi
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 from dataclasses import dataclass
 from typing import Optional, Tuple
 
@@ -74,6 +75,14 @@ class StepArgs:
     unipc: Optional[object] = None
     m3: Optional[torch.Tensor] = None
     out_c: Optional[torch.Tensor] = None
+    # adaptive projected guidance (dpm_step_apg; n_model == 2, per_sample set): the words [2, B] of `apg_words()`, the
+    # fp32 direction R it wrote (read in place of `e_uncond`; None: R from e_uncond), and the marginals of the x0 -> eps
+    # conversion of an eps step. `alpha_e`, `sigma_e` are those of the x0 conversion (EDM: its x0 words); `guidance_b`,
+    # when set, gives the per-sample scales (a scale of 1 bypasses).
+    apg_words: Optional[torch.Tensor] = None
+    apg_r: Optional[torch.Tensor] = None
+    alpha_t: float = 1.0
+    sigma_t: float = 0.0
 
     def state_tensors(self):
         return [t for t in (self.x, self.xe, self.m0, self.m1, self.m2) if t is not None]
@@ -218,17 +227,19 @@ class CudaBackend:
                 if self._layout(a.out2) != layout:      # dense, laid out like `out` (a channels_last half of the
                     raise ValueError("dpm_solver_b200: out2 must be dense and laid out like out")   # doubled CFG batch is)
                 d.out2 = a.out2.data_ptr()
-        for v, what in ((a.ratio, "ratio"), (a.guidance_b, "guidance_b")):
-            if v is None:
-                continue
-            if not v.is_cuda or v.dtype != torch.float32 or not v.is_contiguous() or v.device != ref.device:
-                raise TypeError(f"dpm_solver_b200: `{what}` must be a contiguous fp32 tensor on the tensors' device")
-            if a.per_sample <= 0 or ref.numel() % a.per_sample or v.numel() != ref.numel() // a.per_sample:
-                raise ValueError(f"dpm_solver_b200: `{what}` needs one value per sample")
+        self._check_per_sample(a, ref)
         if a.unipc is not None:
             self._step_unipc(a, d, ref, sdt, layout, keep)
         elif a.e_conds is not None:
             self._step_multi(a, d, ref, sdt, layout, keep)
+        elif a.apg_words is not None:
+            r = None
+            if a.apg_r is not None:
+                r = self._check(a.apg_r, "apg_r", ref.device, ref.numel(), torch.float32, layout)
+                keep.append(r)
+            self._launch(ref.device, self._lib.dpm_step_apg, C.byref(d), C.c_void_p(a.apg_words.data_ptr()),
+                         C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()),
+                         C.c_void_p(None if r is None else r.data_ptr()), C.c_float(a.alpha_t), C.c_float(a.sigma_t))
         elif a.guidance_b is not None:
             # (phi and 1 - phi as below; ignored without a ratio)
             self._launch(ref.device, self._lib.dpm_step_guided, C.byref(d), C.c_void_p(a.guidance_b.data_ptr()),
@@ -241,6 +252,45 @@ class CudaBackend:
         else:
             self._launch(ref.device, self._lib.dpm_step, C.byref(d))
         return m_out, out
+
+    @staticmethod
+    def _check_per_sample(a: StepArgs, ref) -> None:
+        """The per-sample operands of a step: fp32 on the tensors' device, one value per sample (the APG words two)."""
+        for v, what, k in ((a.ratio, "ratio", 1), (a.guidance_b, "guidance_b", 1), (a.apg_words, "apg_words", 2)):
+            if v is None:
+                continue
+            if not v.is_cuda or v.dtype != torch.float32 or not v.is_contiguous() or v.device != ref.device:
+                raise TypeError(f"dpm_solver_b200: `{what}` must be a contiguous fp32 tensor on the tensors' device")
+            if a.per_sample <= 0 or ref.numel() % a.per_sample or v.numel() != k * (ref.numel() // a.per_sample):
+                raise ValueError(f"dpm_solver_b200: `{what}` needs {k} value(s) per sample")
+
+    def apg_words(self, a: StepArgs, eta: float, norm_threshold: float, momentum: float,
+                  r_prev: Optional[torch.Tensor] = None, r_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The per-sample words (A, B) of adaptive projected guidance as fp32 [2, B] on the device (dpm_apg_words), from
+        the CFG pair, conversion and scale(s) of `a` (a.guidance_b: per-sample scales). R = D, or D + momentum*r_prev
+        when r_prev is given; r_out (fp32, laid out like the outputs, may be r_prev) receives R."""
+        d, keep, ref, _, layout = self._fill(a)
+        if a.n_model != 2 or a.per_sample <= 0 or ref.numel() % a.per_sample:
+            raise ValueError("dpm_solver_b200: the APG words take a CFG pair (n_model == 2) and per_sample")
+        nb = ref.numel() // a.per_sample
+        self._check_per_sample(dataclasses.replace(a, apg_words=None), ref)
+        rp = ro = None
+        if r_prev is not None:
+            rp = self._check(r_prev, "r_prev", ref.device, ref.numel(), torch.float32, layout)
+            keep.append(rp)
+        if r_out is not None:
+            self._check(r_out, "r_out", ref.device, ref.numel(), torch.float32)
+            if self._layout(r_out) != layout:
+                raise ValueError("dpm_solver_b200: r_out must be dense and laid out like the inputs")
+            ro = r_out
+        words = torch.empty(2, nb, dtype=torch.float32, device=ref.device)
+        ws_bytes = int(self._lib.dpm_apg_workspace(nb, a.per_sample))
+        ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=ref.device)
+        self._launch(ref.device, self._lib.dpm_apg_words, C.c_void_p(words.data_ptr()), C.byref(d),
+                     C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()), C.c_float(eta),
+                     C.c_float(norm_threshold), C.c_float(momentum), C.c_void_p(None if rp is None else rp.data_ptr()),
+                     C.c_void_p(None if ro is None else ro.data_ptr()), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
+        return words
 
     def _step_multi(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
         """dpm_step_multi: the K conditional outputs and scales of a multi-condition CFG step (d already filled)."""
@@ -266,8 +316,8 @@ class CudaBackend:
 
     def _step_unipc(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
         """dpm_step_unipc: the UniPC words, m_{i-3} and the corrected-state output of a launch (d already filled)."""
-        if a.e_conds is not None or a.guidance_b is not None or a.ratio is not None:
-            raise ValueError("dpm_solver_b200: a UniPC step takes one guidance scale, without rescale")
+        if a.e_conds is not None or a.guidance_b is not None or a.ratio is not None or a.apg_words is not None:
+            raise ValueError("dpm_solver_b200: a UniPC step takes one guidance scale, without rescale or APG")
         w, u = a.unipc, _lib.UniDesc()
         n = ref.numel()
         if a.m3 is not None:
@@ -349,9 +399,9 @@ class CudaBackend:
         """Per-sample s_b = max(quantile(|x0_b|, q), max_val) -> fp32 [B].
         return_stats=True also returns the pipeline's per-sample header words (int32 [B, 8]:
         lo key, hi key, #below, #inside, path (1 bracket / 2 exact fallback), ...) for diagnostics."""
-        if a.guidance_b is not None or a.e_conds is not None:
-            raise ValueError("dpm_solver_b200: the quantile takes one guidance scale; materialise a per-sample "
-                             "or multi-condition combine first")
+        if a.guidance_b is not None or a.e_conds is not None or a.apg_words is not None:
+            raise ValueError("dpm_solver_b200: the quantile takes one guidance scale; materialise a per-sample, "
+                             "multi-condition or APG combine first")
         d, keep, ref, _, _ = self._fill(a)
         if a.per_sample <= 0 or ref.numel() % a.per_sample:
             raise ValueError("dpm_solver_b200: per_sample must divide numel")
@@ -557,8 +607,8 @@ class PreparedStep:
     def build(be: "CudaBackend", a: StepArgs) -> Optional["PreparedStep"]:
         if a.thr is not None or a.raw_round or a.ratio is not None or a.guidance_b is not None \
                 or a.e_conds is not None or a.coef_dev is not None or a.unipc is not None \
-                or a.out is not None and a.out2 is None:
-            # (a rescaled step reads a fresh ratio tensor every evaluation, a guided one a scales tensor the
+                or a.apg_words is not None or a.out is not None and a.out2 is None:
+            # (a rescaled step reads a fresh ratio tensor every evaluation, an APG one fresh words, a guided one a scales tensor the
             # descriptor does not carry, a multi-condition one K outputs and scales it does not carry, one with device
             # coefficients a block the descriptor would point into without owning it: never frozen)
             return None

@@ -17,6 +17,7 @@ The order of model evaluations, their (x, t) arguments, the hooks (`correcting_x
 """
 from __future__ import annotations
 
+import contextlib
 import dataclasses
 import inspect
 import math
@@ -53,6 +54,7 @@ class RawOutput:
     e_conds: Optional[tuple] = None
     scales: Optional[tuple] = None
     is_x0: bool = False     # `e_cond` is a materialised x0 (a guided flow or EDM prediction): it is only clamped, not converted
+    apg: Optional[tuple] = None     # adaptive projected guidance of the combine: (eta, norm_threshold, momentum)
 
 
 def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale):
@@ -107,6 +109,23 @@ def _guidance_args(a: StepArgs, ratio: Optional[torch.Tensor], raw: RawOutput, r
     return a
 
 
+def _apg_args(be, raw: RawOutput, xe, marg, sdtype, x0: bool, ns, coef_dev=None, r_prev=None, r_out=None) -> StepArgs:
+    """StepArgs of an adaptive-projected-guidance evaluation of `raw`, its words computed (dpm_apg_words, 2 launches):
+    both halves converted to x0 with the marginals `marg` = (alpha_t, sigma_t) (EDM: its x0 words), or with those of the
+    device block `coef_dev` when `marg` is None; the guided x0 buffered when `x0`, else converted to eps with the same
+    marginals. r_prev / r_out: the momentum buffer (read / written), or None."""
+    eta, norm_threshold, momentum = raw.apg
+    al, sg = marg if marg is not None else (1.0, 0.0)
+    a = StepArgs(n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=raw.param, guidance=raw.guidance,
+                 predict_x0=x0, xe=xe, alpha_e=al, sigma_e=sg, alpha_t=al, sigma_t=sg, state_dtype=sdtype,
+                 guidance_b=raw.guidance_b, per_sample=raw.e_cond.numel() // raw.e_cond.shape[0], coef_dev=coef_dev)
+    if raw.param == PARAM_EDM:
+        a.alpha_e, a.sigma_e = ns.conversion_words(al, sg, True)
+    a.apg_words = be.apg_words(a, eta, norm_threshold, momentum, r_prev, r_out)
+    a.apg_r = r_out
+    return a
+
+
 def _scale_vector(guidance_scale, guidance_type):
     """model_wrapper's guidance_scale as per-sample scales (a 1-D tensor, or None for one scale). A python number, a
     0-dim or a one-element tensor is one scale, as before; any other tensor must be 1-D."""
@@ -128,9 +147,12 @@ class WrappedModel:
     """
 
     def __init__(self, model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
-                 unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale=0.):
+                 unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale=0.,
+                 apg_eta=None, apg_norm_threshold=0., apg_momentum=0.):
         self.model = model
         self.guidance_rescale = guidance_rescale
+        self.apg_eta = apg_eta
+        self.apg = None if apg_eta is None else (float(apg_eta), float(apg_norm_threshold), float(apg_momentum))
         self.noise_schedule = noise_schedule
         self.model_type = model_type
         self.model_kwargs = model_kwargs
@@ -265,8 +287,8 @@ class WrappedModel:
             t_in = None if t_input is not None else torch.cat([t_continuous] * 2)
             out_u, out_c = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(2)  # uncond first
             if gb is not None:
-                return RawOutput(out_c, out_u, param, 1.0, self.guidance_rescale, gb)
-            return RawOutput(out_c, out_u, param, float(self._one_scale()), self.guidance_rescale)
+                return RawOutput(out_c, out_u, param, 1.0, self.guidance_rescale, gb, apg=self.apg)
+            return RawOutput(out_c, out_u, param, float(self._one_scale()), self.guidance_rescale, apg=self.apg)
         raise RuntimeError("raw() is not available with classifier guidance")
 
     def _alpha_sigma(self, t_continuous):
@@ -314,6 +336,18 @@ class WrappedModel:
         r = self.raw(x, t_continuous)
         if r.e_uncond is None and r.param == PARAM_NOISE:
             return r.e_cond
+        if r.apg is not None and r.e_uncond is not None:
+            # adaptive projected guidance: the words pass, then the guided x0 converted to noise (a direct call is the
+            # first evaluation of its own: no momentum)
+            xo = x.to(r.e_cond.dtype)
+
+            def apg(rows, alpha, sigma):
+                rr = dataclasses.replace(r, e_cond=r.e_cond[rows], e_uncond=r.e_uncond[rows],
+                                         guidance_b=None if r.guidance_b is None else r.guidance_b[rows])
+                a = _apg_args(be, rr, xo[rows], (alpha, sigma), r.e_cond.dtype, False, self.noise_schedule)
+                a.form = FORM_NONE
+                return be.step(a)[0]
+            return self._per_sample(self._alpha_sigma(t_continuous), x.shape[0], apg)
         pairs = self._alpha_sigma(t_continuous) if r.param != PARAM_NOISE else [(1.0, 0.0)]
         if r.param == PARAM_EDM:
             pairs = [self.noise_schedule.conversion_words(al, sg, False) for al, sg in pairs]   # eps words
@@ -334,7 +368,7 @@ class WrappedModel:
 
 def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, guidance_type="uncond",
                   condition=None, unconditional_condition=None, guidance_scale=1., classifier_fn=None,
-                  classifier_kwargs={}, guidance_rescale=0.):
+                  classifier_kwargs={}, guidance_rescale=0., apg_eta=None, apg_norm_threshold=0., apg_momentum=0.):
     """Wrap a network into `model_fn(x, t_continuous) -> noise`; same contract as the reference
     (:170-334): model_type in {noise, x_start, v, score}, guidance_type in {uncond, classifier,
     classifier-free}.
@@ -374,7 +408,20 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     parameterisation, then eps = eps_u + s1*(eps_1 - eps_u) + ... + sK*(eps_K - eps_u), left to right in fp32, as
     torch's eager ops compute it. Every output is combined, whatever the scales (no bypass). One condition in a list is
     exactly the tensor form. With K >= 2: unconditional_condition is required, and guidance_rescale, per-sample scales
-    and DPM_Solver(reference_rounding=True) are not available (ValueError)."""
+    and DPM_Solver(reference_rounding=True) are not available (ValueError).
+
+    apg_eta=eta (classifier-free guidance only; not in the reference; None, the default, is off): adaptive projected
+    guidance (Sadat, Hilliges and Weber, ICLR 2025) on the denoised prediction. Both outputs are converted to x0 by the
+    parameterisation, c = x0_cond and D = c - x0_uncond; with apg_momentum=beta != 0, R = D + beta*R_prev across the
+    evaluations of one sample() / inverse() run (R = D at its first evaluation and in a direct call of this callable);
+    with apg_norm_threshold=r > 0, k = min(1, r/||R||) per sample, else 1; p = <R, c>/max(||c||, 1e-12)^2 per sample;
+    guided x0 = c + (w - 1)*(k*R - (1 - eta)*k*p*c). The guided x0 is then what the solver buffers (dpmsolver++,
+    thresholded when enabled) or converts to noise with the x_start conversion (dpmsolver, and this callable). eta = 1,
+    r = 0, beta = 0 is plain CFG in exact arithmetic. It takes a scalar or a per-sample guidance_scale; a scalar scale of
+    1 keeps the bypass (one network half, no APG), a per-sample scale of 1 gives that row c. Not available (ValueError):
+    other guidance types, no unconditional_condition, several conditions, guidance_rescale != 0, a non-finite eta or
+    momentum, a negative or non-finite threshold, DPM_Solver(reference_rounding=True) and apg_momentum != 0 with
+    method="adaptive"."""
     assert model_type in ["noise", "x_start", "v", "score", "flow", "edm"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
     flow_schedule = getattr(noise_schedule, "schedule", None) == "flow"
@@ -397,8 +444,26 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
         raise ValueError("guidance_rescale must be finite, got {}".format(guidance_rescale))
     if guidance_rescale != 0 and guidance_type != "classifier-free":
         raise ValueError("guidance_rescale needs guidance_type='classifier-free', got '{}'".format(guidance_type))
+    apg_norm_threshold, apg_momentum = float(apg_norm_threshold), float(apg_momentum)
+    if apg_eta is None:
+        if apg_norm_threshold != 0 or apg_momentum != 0:
+            raise ValueError("apg_norm_threshold and apg_momentum need apg_eta")
+    else:
+        apg_eta = float(apg_eta)
+        if guidance_type != "classifier-free" or unconditional_condition is None:
+            raise ValueError("adaptive projected guidance needs guidance_type='classifier-free' and an "
+                             "unconditional_condition")
+        if isinstance(condition, (list, tuple)) and len(condition) >= 2:
+            raise ValueError("adaptive projected guidance is not available with several conditions")
+        if guidance_rescale != 0:
+            raise ValueError("adaptive projected guidance is not available with guidance_rescale")
+        if not (math.isfinite(apg_eta) and math.isfinite(apg_momentum)):
+            raise ValueError("apg_eta and apg_momentum must be finite, got {} and {}".format(apg_eta, apg_momentum))
+        if not (math.isfinite(apg_norm_threshold) and apg_norm_threshold >= 0):
+            raise ValueError("apg_norm_threshold must be finite and >= 0, got {}".format(apg_norm_threshold))
     return WrappedModel(model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
-                        unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale)
+                        unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale,
+                        apg_eta, apg_norm_threshold, apg_momentum)
 
 
 # =================================================================================================
@@ -472,6 +537,8 @@ class DPM_Solver:
             raise ValueError("a per-sample guidance_scale is not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "n_cond", 0) >= 2:
             raise ValueError("several conditions are not available with reference_rounding=True")
+        if self.reference_rounding and getattr(model_fn, "apg", None) is not None:
+            raise ValueError("adaptive projected guidance is not available with reference_rounding=True")
         self._rr_run = 0     # raw_round of the buffered values of the run in flight (reference_rounding)
         self._prep_cache = {}   # frozen launch descriptors of cached plan steps (ops.PreparedStep)
         self._prep_on = False
@@ -729,7 +796,8 @@ class DPM_Solver:
             # meet a launch frozen for one condition)
             # (and so is dynamic thresholding: a launch frozen without the clamp never serves a solver switched to it)
             pkey = (slot, raw.param, raw.guidance, raw.phi, raw.guidance_b is None, raw.e_uncond is None,
-                    raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, raw.scales, self._dynamic_thresholding)
+                    raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, raw.scales, self._dynamic_thresholding,
+                    raw.apg)
             prep = self._prep_cache.get(pkey)
             if prep is not None:
                 r = prep.launch((x, xe, raw.e_cond, m1, m2, raw.e_cond, raw.e_uncond))
@@ -746,6 +814,46 @@ class DPM_Solver:
         code = self._rr_code(raw)
         rr = 0
         q_raw = None        # what the quantile reads, when not `raw` itself
+        apg_a = None        # the step arguments of an adaptive-projected-guidance evaluation
+        split = False       # the buffered value and the update in two launches
+        if raw.apg is not None and raw.e_uncond is not None:
+            # the words pass (+2 launches), then the fused step. With dynamic thresholding (the quantile takes one
+            # plain combine) the guided x0 is materialised once in fp32 (+1 launch) and handed on as one network output.
+            # Under UniPC, whose launch converts at its own state and takes one network output, a FORM_NONE launch
+            # writes the buffered value and the UniPC launch reads it as a pure update.
+            if alsig is _DEV:
+                if co is None or co.dev is None:
+                    raise RuntimeError("device-side scalars need the coefficient block of the consuming launch")
+                marg, cdev = None, co.dev
+            else:
+                marg, cdev = (alsig if isinstance(alsig, tuple) else self._alpha_sigma(alsig)), None
+            thresholded = x0 and self._dynamic_thresholding
+            r_prev, r_out = self._apg_buffers(raw, xe)
+            xa = xe.float() if thresholded and xe.dtype != torch.float32 else xe
+            a = _apg_args(be, raw, xa, marg, torch.float32 if thresholded else sd, x0, self._wrapped.noise_schedule,
+                          cdev, r_prev, r_out)
+            if thresholded:
+                a.form = FORM_NONE
+                raw = RawOutput(be.step(a)[0], None, PARAM_NOISE, 1.0, is_x0=x0)
+                split = self._apg_materialise
+            elif self._apg_materialise:
+                a.form = FORM_NONE
+                m_new = be.step(a)[0]
+                if custom_fix:
+                    m_new = self._state_like(self.correcting_x0_fn(m_new, t_dev), sd)
+                if co is None:
+                    return m_new, None
+                b = StepArgs(n_model=0, m0=m_new, state_dtype=sd)
+                self._fill_update(b, co, x, m1, m2)
+                dup = self._dup_target(x) if dup_out else None
+                if dup is not None:
+                    b.out, b.out2 = dup[1], dup[2]
+                x_next = be.step(b)[1]
+                if dup is not None:
+                    self._xin_pair = (x_next, dup[0])
+                return m_new, x_next
+            else:
+                apg_a = a
         ratio = _cfg_ratio(be, raw)     # guidance rescale: one streaming pass over both halves (+2 launches)
         if code:
             # reference-rounding mode (raw 16-bit NOISE outputs, fp32 state): bits 0-1 make the fused kernel take the
@@ -794,7 +902,7 @@ class DPM_Solver:
             x_next = self._pure_update(co, x, m_new, m1, m2, rr=rr & 4 and rr, pkey=pkey if m_new is raw.e_cond else None) \
                 if co is not None else None
             return m_new, x_next
-        a = _guidance_args(self._conv_args(raw, xe, alsig, sd, x0), ratio, raw)
+        a = apg_a if apg_a is not None else _guidance_args(self._conv_args(raw, xe, alsig, sd, x0), ratio, raw)
         if alsig is _DEV:
             if co is None or co.dev is None:
                 raise RuntimeError("device-side scalars need the coefficient block of the consuming launch")
@@ -807,7 +915,7 @@ class DPM_Solver:
                 qa.per_sample, qa.coef_dev = a.per_sample, a.coef_dev
             a.thr = be.dynamic_threshold(qa, float(self.dynamic_thresholding_ratio),
                                          float(self.thresholding_max_val))
-        if custom_fix or co is None:
+        if custom_fix or co is None or split:
             a.form = FORM_NONE
             a.raw_round = rr & 3
             m_new = be.step(a)[0]
@@ -830,6 +938,33 @@ class DPM_Solver:
         if pkey is not None and not a.per_sample and a.e_conds is None:
             self._remember(pkey, a, dup)
         return m_new, x_next
+
+    _apg_materialise = False     # UniPC: its launch takes one network output, so an APG value is materialised first
+
+    def _apg_buffers(self, raw: RawOutput, xe):
+        """(r_prev, r_out) of an APG evaluation. Without momentum, or outside a sample() / inverse() run: (None, None).
+        The first evaluation of a run allocates the run's fp32 buffer and writes it without reading it (so a captured
+        graph needs no reset launch); later ones update it in place."""
+        if raw.apg[2] == 0 or not self.__dict__.get("_apg_run"):
+            return None, None
+        r = self.__dict__.get("_apg_r")
+        if r is None:
+            self._apg_r = torch.empty_like(xe, dtype=torch.float32)
+            return None, self._apg_r
+        return r, r
+
+    @contextlib.contextmanager
+    def _apg_scope(self):
+        """One sample() / inverse() run: the APG momentum buffer lives for its duration."""
+        self._apg_run, self._apg_r = True, None
+        try:
+            yield
+        finally:
+            self._apg_run, self._apg_r = False, None
+
+    def _apg_momentum(self) -> float:
+        apg = getattr(self._wrapped, "apg", None)
+        return 0. if apg is None else apg[2]
 
     def _remember(self, pkey, a: StepArgs, dup=None) -> None:
         """Freeze the launch that just ran as the prepared form of its plan step."""
@@ -1288,6 +1423,9 @@ class DPM_Solver:
             assert method in ['multistep', 'singlestep', 'singlestep_fixed'], "Cannot use adaptive solver when saving intermediate values"
         if self.correcting_xt_fn is not None:
             assert method in ['multistep', 'singlestep', 'singlestep_fixed'], "Cannot use adaptive solver when correcting_xt_fn is not None"
+        if method == 'adaptive' and self._apg_momentum() != 0:
+            raise ValueError("apg_momentum != 0 is not available with method='adaptive': its evaluations, the device "
+                             "controller's surplus iterations included, define no momentum sequence")
         device = x.device
         intermediates = []
         ns = self.noise_schedule
@@ -1296,7 +1434,7 @@ class DPM_Solver:
         # prepared launches: the CUDA executor, no python-side x0 hook, no 16-bit reference-rounding mode
         self._prep_on = (hasattr(ops.backend(), "prepare") and not self.reference_rounding
                          and (self.correcting_x0_fn is None or self._dynamic_thresholding))
-        with torch.no_grad():
+        with torch.no_grad(), self._apg_scope():
             x = self._state(x)
             sd = x.dtype
             if method == 'adaptive':

@@ -53,6 +53,10 @@ predictor launch reads the hooked state. A custom `correcting_x0_fn` sees the ma
 hook, then the UniPC launch on the hooked value). `return_intermediate` returns x_T, the corrected x_1 .. x_{N-1}
 and x_N.
 
+Adaptive projected guidance (model_wrapper's apg_eta) runs with a scalar scale: per evaluation the words pass, one
+launch that writes the buffered value m_i, then the UniPC launch reading it (n_model == 0). With dynamic thresholding
+the guided x0 is materialised in fp32 first, then thresholded, then buffered.
+
 Not available (ValueError before any launch): per-sample guidance scales, several conditions, guidance rescale,
 reference_rounding, plan_broadcast, orders outside 1..3, steps < order.
 """
@@ -79,6 +83,8 @@ class _Launch:
 
 
 class UniPC(DPM_Solver):
+    _apg_materialise = True     # adaptive projected guidance: the buffered value (+1 launch), then this launch on it
+
     def __init__(self, model_fn, noise_schedule, algorithm_type="dpmsolver++", variant="bh2", correcting_x0_fn=None,
                  correcting_xt_fn=None, thresholding_max_val=1., dynamic_thresholding_ratio=0.995, state_dtype=None):
         """UniPC multistep sampler. `algorithm_type` as in DPM_Solver ("dpmsolver++": data prediction,
@@ -138,7 +144,7 @@ class UniPC(DPM_Solver):
         self._xin_pair = None
         self._rr_run = 0
         self._prep_on = False           # UniPC launches are never frozen as prepared launches
-        with torch.no_grad():
+        with torch.no_grad(), self._apg_scope():
             x = self._state(x)
             sd = x.dtype
             key = ("unipc", self.variant, steps, order, skip_type, t_T, t_0, lower_order_final, bool(use_corrector))

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 105 /* 0.1.5: DPM_PARAM_EDM */
+#define DPM_B200_VERSION 106 /* 0.1.6: adaptive projected guidance (dpm_apg_words, dpm_step_apg) */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -312,6 +312,39 @@ DPM_API int dpm_step_guided(const dpm_step_desc* desc, const float* guidance, co
 DPM_API int dpm_cfg_rescale_ratio_guided(float* ratio_out, const void* e_cond, const void* e_uncond,
                                          const float* guidance, uint64_t per_sample, uint64_t n, int model_dtype,
                                          void* workspace, size_t workspace_bytes, dpm_stream_t stream);
+
+/* ---- adaptive projected guidance (Sadat, Hilliges and Weber, ICLR 2025, arXiv:2410.02416) ---------------------
+ * Classifier-free guidance on the denoised prediction, with the guidance difference split into a part parallel to the
+ * conditional prediction, down-weighted by eta, and a part orthogonal to it; optionally norm-clipped and with reverse
+ * momentum across evaluations. Per sample b of per_sample elements, with both outputs first converted to x0 by the
+ * parameterisation as a predict_x0 step converts them (alpha_e, sigma_e: the marginals; DPM_PARAM_EDM: its x0 words),
+ * every op rounded to fp32:
+ *   c = x0(e_cond), u = x0(e_uncond), D = c - u
+ *   R = D  (r_prev == NULL)   or   R = D + momentum*r_prev                          (two rounded ops)
+ *   k_b = min(1, norm_threshold/||R_b||) if norm_threshold > 0, else 1
+ *   p_b = <R_b, c_b> / max(||c_b||, 1e-12)^2
+ *   A_b = 1 - (w_b - 1)*(1 - eta)*k_b*p_b,  B_b = (w_b - 1)*k_b                      (fp64, each rounded to fp32 once)
+ *   guided = A_b*c + B_b*R      (two products and a sum, each rounded; a sample with guidance[b] == 1: c itself)
+ * The sums run over the sample's elements in fp64, per 8192-element chunk, merged in chunk order: the bits of A_b, B_b
+ * depend on sample b's values only. w_b = guidance[b] when the per-sample array is given, else desc->guidance.
+ * dpm_apg_words: A -> words[0 .. B), B -> words[B .. 2B), B = n/per_sample, fp32 device memory. Reads desc->xe (NULL =>
+ *   desc->x), e_cond, e_uncond, param, alpha_e, sigma_e, guidance, dtypes and dev_coef (alpha_e, sigma_e from the
+ *   block); form, thr, outputs and predict_x0 are not read. r_out (optional, fp32 [n]) receives R and may be r_prev
+ *   (element-wise in place). workspace: dpm_apg_workspace(n/per_sample, per_sample) bytes of 8-byte aligned device
+ *   memory (contents irrelevant). Two launches.
+ * dpm_step_apg: dpm_step with the guided value in place of the combine: for predict_x0 it is the buffered x0 (the clamp
+ *   by thr follows), else eps = (xe - alpha_t*guided)/sigma_t (:292; with dev_coef, alpha_t and sigma_t are read from
+ *   the block like alpha_e, sigma_e). r: the R that dpm_apg_words wrote, read in place of e_uncond, or NULL (R = D from
+ *   e_uncond). guidance: NULL, or the per-sample scales (only their value 1 is read here).
+ * Both need desc->n_model == 2, desc->raw_round == 0, desc->per_sample != 0 dividing n and words != NULL, and refuse
+ * DPM_PARAM_EDM with dev_coef and a thr without predict_x0 (DPM_ERR_ARG). dpm_step_apg is served by the direct vector
+ * kernels (tails, unaligned views and dev_coef launches by the generic kernel); never by the TMA variant. */
+DPM_API size_t dpm_apg_workspace(uint64_t n_samples, uint64_t per_sample);
+DPM_API int dpm_apg_words(float* words, const dpm_step_desc* desc, const float* guidance, float eta,
+                          float norm_threshold, float momentum, const float* r_prev, float* r_out, void* workspace,
+                          size_t workspace_bytes, dpm_stream_t stream);
+DPM_API int dpm_step_apg(const dpm_step_desc* desc, const float* words, const float* guidance, const float* r,
+                         float alpha_t, float sigma_t, dpm_stream_t stream);
 
 /* ---- multi-condition classifier-free guidance (composable prompts, Liu et al. 2022) ----------------------------
  * The network runs once on cat([x] * (n_cond + 1)) with the conditions cat([uc, c_1, ..., c_n]) and returns
