@@ -6,7 +6,10 @@
   and the part orthogonal to it, the parallel part scaled by eta.
 * `x0_fp64`: each parameterisation's denoised prediction in float64.
 * `APGOracle`: the numpy executor (edm_oracle.EDMOracle: every parameterisation, guidance form and dpm_step_unipc) plus
-  dpm_apg_words and dpm_step_apg as include/dpm_solver_b200.h states them, op for op in IEEE fp32, the sums in fp64.
+  dpm_apg_words and dpm_step_apg as include/dpm_solver_b200.h states them, op for op in IEEE fp32, the sums in fp64
+  (numpy's pairwise order; `exact=True`: apg.cu's order, `apg_words_exact`, so that the words are bit-exact).
+* `apg_words_exact`: the words of apg.cu operation for operation -- its chunks, thread ownership, warp butterflies,
+  warp order, chunk merge and k_apg_final's left-to-right fp64 formula.
 * `reference_solver`: the UNMODIFIED reference DPM_Solver driven by an fp64 APG data-prediction function, with the
   momentum kept in its closure.
 """
@@ -68,10 +71,75 @@ def x0_fp64(param, out, x, alpha, sigma, sigma_data=None):
     raise ValueError(param)
 
 
+# ---- apg.cu's reduction, operation for operation -----------------------------------------------------------------------
+
+CHUNK, THREADS, WARP = 8192, 256, 32
+
+
+def apg_sums_exact(R, c):
+    """(||R||^2, <R, c>, ||c||^2) per sample as k_apg_partial + k_apg_final sum them, from fp32 [B, per_sample] arrays.
+    CTA (b, chunk) covers chunk elements [chunk*8192, min(+8192, per_sample)); thread tid owns the elements
+    (u*256 + tid)*8 + i, u = 0..3, i = 0..7, and adds their fp64 products in that order to sums that start at 0.0 (the
+    product of two fp32 values is exact in fp64). Each warp folds its 32 lanes by v += shfl_xor(v, o), o = 16 .. 1; then
+    s = 0.0 + warp 0 + ... + warp 7, and the chunks are merged from 0.0 in chunk order. Elements past the end of the
+    sample contribute the product +0.0, which leaves every such sum (never -0.0: it starts at +0.0) unchanged."""
+    R, c = np.asarray(R, f32), np.asarray(c, f32)
+    Bn, ps = R.shape
+    chunks = -(-ps // CHUNK)
+    pad = chunks * CHUNK - ps
+    out = []
+    with np.errstate(all="ignore"):
+        for a, b in ((R, R), (R, c), (c, c)):
+            prod = a.astype(np.float64) * b.astype(np.float64)
+            prod = np.concatenate([prod, np.zeros((Bn, pad))], axis=1) if pad else prod
+            # [B, chunk, u, tid, i] -> [B, chunk, tid, (u, i)]: each thread's 32 products in the order it adds them
+            per_thread = prod.reshape(Bn, chunks, 4, THREADS, 8).transpose(0, 1, 3, 2, 4).reshape(Bn, chunks, THREADS, 32)
+            v = np.zeros((Bn, chunks, THREADS))
+            for k in range(32):
+                v = v + per_thread[..., k]
+            lanes = v.reshape(Bn, chunks, THREADS // WARP, WARP)
+            for o in (16, 8, 4, 2, 1):
+                lanes = lanes + lanes[..., np.arange(WARP) ^ o]
+            s = np.zeros((Bn, chunks))
+            for w in range(THREADS // WARP):
+                s = s + lanes[:, :, w, 0]
+            t = np.zeros(Bn)
+            for ch in range(chunks):
+                t = t + s[:, ch]
+            out.append(t)
+    return tuple(out)
+
+
+def apg_final(srr, src, scc, w, eta, norm_threshold):
+    """k_apg_final from the merged sums: fp64, left to right, each word rounded to fp32 once -> fp32 [2, B]. `w`: the
+    scale of each sample as fp64 (an fp32 value widened)."""
+    with np.errstate(all="ignore"):
+        k = np.ones(len(srr))
+        if f32(norm_threshold) > 0:
+            q = np.float64(f32(norm_threshold)) / np.sqrt(srr)
+            k = np.where(q < 1.0, q, 1.0)            # (a NaN quotient gives 1, as `q < 1.0 ? q : 1.0` does)
+        sc = np.sqrt(scc)
+        nc = np.where(sc < 1e-12, 1e-12, sc)
+        p = src / (nc * nc)
+        A = 1.0 - (((w - 1.0) * (1.0 - np.float64(f32(eta)))) * k) * p
+        Bw = (w - 1.0) * k
+        return np.stack([A, Bw]).astype(f32)
+
+
+def apg_words_exact(R, c, w, eta, norm_threshold):
+    """The words [2, B] of dpm_apg_words from R and c (fp32 [B, per_sample]) and the per-sample scales `w` (fp64 [B])."""
+    return apg_final(*apg_sums_exact(R, c), w, eta, norm_threshold)
+
+
 # ---- the executor ----------------------------------------------------------------------------------------------------
 
 class APGOracle(EDMOracle):
-    """The numpy executor with dpm_apg_words and dpm_step_apg."""
+    """The numpy executor with dpm_apg_words and dpm_step_apg. `exact`: the words summed in apg.cu's order
+    (apg_words_exact), bit-exact with the device; otherwise in numpy's pairwise order (within an ulp of it)."""
+
+    def __init__(self, exact=False):
+        super().__init__()
+        self.exact = exact
 
     @staticmethod
     def _x0(a, out, xe):
@@ -107,21 +175,21 @@ class APGOracle(EDMOracle):
             R = D if r_prev is None else (D + f32(momentum) * _np(r_prev)).astype(f32)
         if r_out is not None:
             r_out.copy_(torch.from_numpy(np.ascontiguousarray(R)).reshape(r_out.shape))
-        R64, c64 = R.reshape(B, -1).astype(np.float64), c.reshape(B, -1).astype(np.float64)
-        with np.errstate(all="ignore"):
-            srr, src, scc = (R64 * R64).sum(1), (R64 * c64).sum(1), (c64 * c64).sum(1)
-            k = np.ones(B)
-            if f32(norm_threshold) > 0:
-                q = np.float64(f32(norm_threshold)) / np.sqrt(srr)
-                k = np.where(q < 1.0, q, 1.0)
-            sc = np.sqrt(scc)
-            nc = np.where(sc < 1e-12, 1e-12, sc)
-            p = src / (nc * nc)
-            w = (_np(a.guidance_b).astype(np.float64) if a.guidance_b is not None
-                 else np.full(B, np.float64(f32(a.guidance))))
-            A = 1.0 - (w - 1.0) * (1.0 - np.float64(f32(eta))) * k * p
-            Bw = (w - 1.0) * k
-        return torch.from_numpy(np.stack([A, Bw]).astype(f32))
+        w = (_np(a.guidance_b).astype(np.float64) if a.guidance_b is not None
+             else np.full(B, np.float64(f32(a.guidance))))
+        if self.exact:
+            # the device sums in storage order: a channels_last launch (laid out like xe) holds each sample as (h, w, c)
+            ref = a.xe if a.xe is not None else a.x
+            if ref.dim() in (4, 5) and not ref.is_contiguous() and ref.is_contiguous(
+                    memory_format=torch.channels_last if ref.dim() == 4 else torch.channels_last_3d):
+                perm = (0,) + tuple(range(2, ref.dim())) + (1,)
+                R, c = R.transpose(perm), c.transpose(perm)
+            sums = apg_sums_exact(R.reshape(B, -1), c.reshape(B, -1))
+        else:
+            R64, c64 = R.reshape(B, -1).astype(np.float64), c.reshape(B, -1).astype(np.float64)
+            with np.errstate(all="ignore"):
+                sums = (R64 * R64).sum(1), (R64 * c64).sum(1), (c64 * c64).sum(1)
+        return torch.from_numpy(apg_final(*sums, w, eta, norm_threshold))
 
     def _model_value(self, a, thr=None):
         if getattr(a, "apg_words", None) is None:

@@ -1,0 +1,36 @@
+"""The CPU side of tests/test_gpu_apg_random_configs.py, pinned where there is no device: the exact executor's result
+for every configuration the device test draws, within REF_TOL of the unmodified reference driven by an fp64 APG data
+prediction wherever the reference can express the configuration; the refused configurations are exactly the
+documented ones; and the fixed seeds reach every path the device test must meet."""
+import pytest
+
+from apg_configs import CHUNKS, REQUIRED, configurations, cpu_oracle, reference_expressible, refused, tally_static
+from oracle import ref_loader
+
+pytestmark = pytest.mark.skipif(not ref_loader.available(), reason="oracle/_ref not built and no reference tree")
+TALLY = {}
+CHUNKS_RUN = set()
+
+
+@pytest.mark.parametrize("chunk", range(CHUNKS))
+def test_oracle_of_every_drawn_configuration(chunk):
+    for c in configurations(chunk):
+        out = cpu_oracle(c)
+        assert ("error" in out) == refused(c), (c, out.get("error"))
+        if "error" in out:
+            assert isinstance(out["error"], ValueError), (c, out["error"])
+            TALLY["rejected"] = TALLY.get("rejected", 0) + 1
+            continue
+        assert out["calls"] and all(t.dtype == out["y"].dtype for t in out["inter"]), c
+        assert ("pinned" in out) == reference_expressible(c), c
+        for k in tally_static(c) + (["pinned"] if "pinned" in out else []):
+            TALLY[k] = TALLY.get(k, 0) + 1
+    CHUNKS_RUN.add(chunk)
+
+
+def test_tally_of_the_drawn_configurations():
+    """After the chunks: every path the device test requires, a pinned and a refused draw were met."""
+    if len(CHUNKS_RUN) < CHUNKS:
+        pytest.skip("needs every chunk of test_oracle_of_every_drawn_configuration in the same session")
+    print("\ntally: %s" % dict(sorted(TALLY.items())))
+    assert not [k for k in REQUIRED + ["pinned", "rejected"] if not TALLY.get(k)]

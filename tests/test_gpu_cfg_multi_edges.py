@@ -390,20 +390,28 @@ def profile_mirror():
     kinds = {k for k in seen if isinstance(k[1], int)}
     assert {("multi-fast", 1), ("multi-fast", 2), ("multi-generic", 1), ("multi-generic", 2), ("scalar", 1),
             ("scalar(dev_coef)", 1)} <= kinds and len(chosen) >= 70, (kinds, len(chosen))
-    for spec in chosen:
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    # one profiler session for every launch (sessions opened one after another were seen to record no kernels): the
+    # step kernels run in launch order on one stream, so the recorded sequence must be the mirror's, launch by launch
+    want, owner = [], []
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for spec in chosen:
             ks = run_case(be, spec)
-            torch.cuda.synchronize()
-        ran = [e.name.replace(" ", "") for e in prof.events() if "k_step_multi" in e.name]
-        want = [kernel_name(k) + ("(" if k[0] == "scalar" else "") for k in ks]
-        assert len(ran) == len(want) and all(w in r for w, r in zip(want, ran)), (spec, want, ran)
+            want += [kernel_name(k) + ("(" if k[0] == "scalar" else "") for k in ks]
+            owner += [spec] * len(ks)
+        torch.cuda.synchronize()
+    ran = [e.name.replace(" ", "") for e in sorted((e for e in prof.events() if "k_step_multi" in e.name),
+                                                   key=lambda e: e.time_range.start)]
+    assert len(ran) == len(want), (len(ran), len(want))
+    for spec, w, r in zip(owner, want, ran):
+        assert w in r, (spec, w, r)
     print("%d profiled launches match the mirror" % len(chosen))
 
 
 def test_mirror_names_the_kernel_that_ran():
-    """profile_mirror() in a child process of its own: profiler sessions opened after many others in one process were
-    seen to record no kernels (tests/test_gpu_step_edges.py profiles in this process too), so neither test may leave
-    its profiler state to the other."""
+    """profile_mirror() in a child process of its own, in one profiler session: sessions opened after many others in
+    one process were seen to record no kernels (tests/test_gpu_step_edges.py profiles in this process too, and a child
+    that opened one session per launch once recorded nothing in one of them), so neither test may leave its profiler
+    state to the other."""
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     code = ("import sys; sys.path[:0] = %r; import test_gpu_cfg_multi_edges as t; t.profile_mirror()"
             % [root, os.path.join(root, "tests"), os.path.join(root, "tests", "golden")])
