@@ -102,6 +102,9 @@ PROTOTYPES = {
     "dpm_apg_workspace": (C.c_size_t, [_u64, _u64]),
     "dpm_apg_words": (C.c_int, [_vp, C.POINTER(StepDesc), _vp, _f, _f, _f, _vp, _vp, _vp, C.c_size_t, _vp]),
     "dpm_step_apg": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _vp, _f, _f, _vp]),
+    "dpm_cfgzero_workspace": (C.c_size_t, [_u64, _u64]),
+    "dpm_cfgzero_scale": (C.c_int, [_vp, _vp, _vp, _i, _u64, _u64, _vp, C.c_size_t, _vp]),
+    "dpm_step_cfgzero": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _vp]),
 }
 
 MAX_CONDITIONS = 4      # DPM_MAX_CONDITIONS

@@ -183,4 +183,117 @@ int launch_apg_words(float* words, const KParams& kp, const float* gscale, float
   return DPM_OK;
 }
 
+// ---- CFG-Zero* (dpm_cfgzero_scale; Fan, Zheng, Yeh and Liu, arXiv:2503.18886) -------------------------------------
+// s*_b = fl32(<c_b, u_b> / (||u_b||^2 + 1e-8)) over the two raw network halves of sample b, fp64 sums of the widened
+// outputs. The chunking, thread ownership and summation order of k_apg_partial / k_apg_final, with two sums of raw
+// values in place of three of converted ones: no x, no marginals, no dev_coef. Algorithmic bytes: 2*s_model per element.
+struct ZParams {
+  const void* ec;
+  const void* eu;
+  double* partial;       // [n_samples * chunks][2]: <c, u>, ||u||^2
+  float* s_out;          // [n_samples]
+  uint64_t per_sample;
+  uint64_t n_samples;
+  uint32_t chunks;
+  int32_t model_dtype;
+};
+
+// VEC: per_sample % 8 == 0 and both halves aligned, TE their type. Otherwise element-wise (load_any).
+template <typename TE, bool VEC>
+__global__ void __launch_bounds__(kAThreads) k_cfgzero_partial(const __grid_constant__ ZParams p) {
+  __shared__ double warp_part[kAThreads / 32];
+  const uint64_t sample = blockIdx.x / p.chunks;
+  const uint32_t chunk = blockIdx.x % p.chunks;
+  const uint64_t c_begin = (uint64_t)chunk * kAChunk;
+  const uint64_t c_end = c_begin + kAChunk < p.per_sample ? c_begin + kAChunk : p.per_sample;
+  const uint32_t cnt = (uint32_t)(c_end - c_begin);
+  const size_t e0 = sample * p.per_sample + c_begin;
+  const int tid = threadIdx.x;
+  constexpr int U = kAChunk / kPacket / kAThreads;   // 4
+  double scu = 0.0, suu = 0.0;
+  auto term = [&](float c, float u) {
+    scu += (double)c * (double)u;
+    suu += (double)u * (double)u;
+  };
+  // element (u, i) of this thread is chunk element (u*kAThreads + tid)*8 + i on both paths, as in k_apg_partial
+#pragma unroll
+  for (int u = 0; u < U; ++u) {
+    const uint32_t pk = u * kAThreads + tid;
+    if (VEC) {
+      if (pk * kPacket < cnt) {
+        const size_t e = e0 + (size_t)pk * kPacket;
+        Raw<TE> rc, ru;
+        ldg_pk(rc, static_cast<const TE*>(p.ec) + e);
+        ldg_pk(ru, static_cast<const TE*>(p.eu) + e);
+        float fc[8], fu[8];
+        unpack(rc, fc);
+        unpack(ru, fu);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) term(fc[i], fu[i]);
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const uint32_t j = pk * kPacket + i;
+        if (j < cnt) term(load_any(p.ec, p.model_dtype, e0 + j), load_any(p.eu, p.model_dtype, e0 + j));
+      }
+    }
+  }
+  scu = apg_cta_sum(scu, warp_part);
+  suu = apg_cta_sum(suu, warp_part);
+  if (tid == 0) {
+    double* o = p.partial + (size_t)blockIdx.x * 2;
+    o[0] = scu; o[1] = suu;
+  }
+}
+
+__global__ void __launch_bounds__(kAThreads) k_cfgzero_final(const __grid_constant__ ZParams p) {
+  const uint64_t b = (uint64_t)blockIdx.x * kAThreads + threadIdx.x;
+  if (b >= p.n_samples) return;
+  const double* part = p.partial + b * p.chunks * 2;
+  double scu = 0.0, suu = 0.0;
+  for (uint32_t c = 0; c < p.chunks; ++c) {
+    scu += part[c * 2];
+    suu += part[c * 2 + 1];
+  }
+  p.s_out[b] = (float)(scu / (suu + 1e-8));   // diffusers' cfg_zero_star_scale epsilon
+}
+
+size_t cfgzero_workspace_bytes(uint64_t n_samples, uint64_t per_sample) {
+  if (per_sample == 0 || n_samples == 0) return 0;
+  const uint64_t chunks = (per_sample + kAChunk - 1) / kAChunk;
+  return (size_t)(n_samples * chunks) * 2 * sizeof(double);
+}
+
+int launch_cfgzero_scale(float* s_out, const void* ec, const void* eu, int model_dtype, uint64_t per_sample,
+                         uint64_t n, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  ZParams p;
+  memset(&p, 0, sizeof(p));
+  p.ec = ec; p.eu = eu; p.s_out = s_out; p.model_dtype = model_dtype;
+  p.per_sample = per_sample; p.n_samples = n / per_sample;
+  p.chunks = (uint32_t)((per_sample + kAChunk - 1) / kAChunk);
+  p.partial = static_cast<double*>(ws);
+  if (ws == nullptr || ws_bytes < cfgzero_workspace_bytes(p.n_samples, per_sample) ||
+      (reinterpret_cast<uintptr_t>(ws) & 7)) {
+    set_error("cfg-zero* scale: workspace too small or not 8-byte aligned");
+    return DPM_ERR_ARG;
+  }
+  if (p.n_samples * p.chunks > 0x7fffffffull) { set_error("cfg-zero* scale: too many chunks"); return DPM_ERR_UNSUPPORTED; }
+  const uintptr_t am = model_dtype == DPM_F32 ? 31 : 15;
+  const bool vec = per_sample % kPacket == 0 && (reinterpret_cast<uintptr_t>(ec) & am) == 0 &&
+                   (reinterpret_cast<uintptr_t>(eu) & am) == 0;
+  typedef void (*ZKernel)(const ZParams);
+  ZKernel k = k_cfgzero_partial<float, false>;   // any dtype, alignment or sample size
+  if (vec) {
+    if (model_dtype == DPM_F32) k = k_cfgzero_partial<float, true>;
+    else if (model_dtype == DPM_BF16) k = k_cfgzero_partial<__nv_bfloat16, true>;
+    else if (model_dtype == DPM_F16) k = k_cfgzero_partial<__half, true>;
+  }
+  k<<<(unsigned)(p.n_samples * p.chunks), kAThreads, 0, stream>>>(p);
+  k_cfgzero_final<<<(unsigned)((p.n_samples + kAThreads - 1) / kAThreads), kAThreads, 0, stream>>>(p);
+  count_launch();
+  count_launch();
+  return DPM_OK;
+}
+
 }  // namespace dpm

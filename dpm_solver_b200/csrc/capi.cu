@@ -231,8 +231,9 @@ struct Apg {
 };
 
 // gscale (optional): per-sample guidance of an n_model == 2 step, fp32 [n/per_sample]; rs then may be NULL
+// zs (optional): the CFG-Zero* scales s* of an n_model == 2 step, fp32 [n/per_sample]; gscale then may be NULL
 static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale* rs = nullptr,
-                     const float* gscale = nullptr, const Apg* apg = nullptr) {
+                     const float* gscale = nullptr, const Apg* apg = nullptr, const float* zs = nullptr) {
   KParams p;
   Needs nd;
   if (d != nullptr && d->n == 0) return DPM_OK;  // empty tensors: nothing to do (pointers may be NULL)
@@ -260,6 +261,7 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale*
     p.ratio = rs->ratio; p.phi = rs->phi; p.psi = rs->psi;
   }
   p.gscale = gscale;
+  p.zs = zs;
   Tuning t{g_variant.load(), g_threads.load(), g_ctas.load()};
 
   bool body_done = false;
@@ -272,6 +274,7 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale*
                      p.ratio == nullptr &&  // guidance rescale: the direct variant's <RS> kernels
                      p.gscale == nullptr &&  // per-sample guidance: the direct variant's <PG> kernels
                      p.apg_a == nullptr &&   // adaptive projected guidance: the direct variant's <APG> kernels
+                     p.zs == nullptr &&      // CFG-Zero*: the direct variant's <PG> kernels
                      t.variant == 1;
     if (tma) r = launch_step_tma(p, t, stream);
     if (r == 1) r = launch_step_direct(p, t, stream);
@@ -516,6 +519,32 @@ int dpm_step_apg(const dpm_step_desc* desc, const float* words, const float* gui
   if (desc->thr != nullptr && !desc->predict_x0) { set_error("apg step: thr requires predict_x0"); return DPM_ERR_ARG; }
   const Apg apg{words, r, alpha_t, sigma_t};
   return step_impl(desc, static_cast<cudaStream_t>(stream), nullptr, guidance, &apg);
+}
+
+size_t dpm_cfgzero_workspace(uint64_t n_samples, uint64_t per_sample) {
+  return cfgzero_workspace_bytes(n_samples, per_sample);
+}
+
+int dpm_cfgzero_scale(float* s_out, const void* e_cond, const void* e_uncond, int model_dtype, uint64_t per_sample,
+                      uint64_t n, void* workspace, size_t workspace_bytes, dpm_stream_t stream) {
+  if (n == 0) return DPM_OK;
+  if (!s_out || !e_cond || !e_uncond) { set_error("cfg-zero* scale: NULL tensor"); return DPM_ERR_ARG; }
+  if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) {
+    set_error("cfg-zero* scale: bad dtype or sizes");
+    return DPM_ERR_ARG;
+  }
+  return finish(launch_cfgzero_scale(s_out, e_cond, e_uncond, model_dtype, per_sample, n, workspace, workspace_bytes,
+                                     static_cast<cudaStream_t>(stream)));
+}
+
+int dpm_step_cfgzero(const dpm_step_desc* desc, const float* s_star, const float* guidance, dpm_stream_t stream) {
+  if (desc != nullptr && desc->n == 0) return DPM_OK;
+  if (desc == nullptr || s_star == nullptr || desc->n_model != 2 || desc->raw_round != 0 || desc->per_sample == 0 ||
+      desc->n % desc->per_sample) {
+    set_error("cfg-zero* step: needs s_star, n_model == 2, raw_round == 0 and per_sample dividing n");
+    return DPM_ERR_ARG;
+  }
+  return step_impl(desc, static_cast<cudaStream_t>(stream), nullptr, guidance, nullptr, s_star);
 }
 
 static dpm_step_desc base_desc(void* out, const void* x, uint64_t n, int dtype, int form) {

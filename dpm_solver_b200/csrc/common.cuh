@@ -75,6 +75,10 @@ struct KParams {
   const float* apg_b;
   const float* apg_r;
   float apg_alpha, apg_sigma;
+  // CFG-Zero* (dpm_step_cfgzero): the per-sample optimised scale s*_b of dpm_cfgzero_scale, fp32 [n/per_sample]. Only
+  // the <PG = true> instantiations read it (kind kPgZeroStar); `gscale` may then be NULL (every sample's scale is
+  // `guidance`).
+  const float* zs;
 };
 
 // multi-condition classifier-free guidance (dpm_step_multi): eps = eps_u; eps = eps + s[k]*(eps_k - eps_u) for k < n_cond,
@@ -355,9 +359,11 @@ __device__ __forceinline__ float rescale_value(const KParams& p, float g, float 
 //   kPgBypass  gs == 1: the reference's bypass (:323), the converted conditional output alone (no combine, no rescale)
 //   kPgRescale p.ratio set: the rescaled combine of the RS path
 //   kPgCombine otherwise: the combine of the plain path
-enum { kPgAny = 1, kPgBypass = 2, kPgRescale = 3, kPgCombine = 4 };
+//   kPgZeroStar p.zs set: CFG-Zero* (Fan et al. 2025) in the network's output space with r = s*_b of the sample:
+//              us = eu*s*, g = us + gs*(ec - us), each op rounded, then the parameterisation converts g
+enum { kPgAny = 1, kPgBypass = 2, kPgRescale = 3, kPgCombine = 4, kPgZeroStar = 5 };
 __host__ __device__ __forceinline__ int pg_kind(const KParams& p, float gs) {
-  return gs == 1.f ? kPgBypass : (p.ratio != nullptr ? kPgRescale : kPgCombine);
+  return gs == 1.f ? kPgBypass : (p.zs != nullptr ? kPgZeroStar : (p.ratio != nullptr ? kPgRescale : kPgCombine));
 }
 template <int K>
 __device__ __forceinline__ float guided_value(const KParams& p, float xe, float ec, float eu, float r, float gs) {
@@ -365,11 +371,15 @@ __device__ __forceinline__ float guided_value(const KParams& p, float xe, float 
     const int k = pg_kind(p, gs);
     if (k == kPgBypass) return guided_value<kPgBypass>(p, xe, ec, eu, r, gs);
     if (k == kPgRescale) return guided_value<kPgRescale>(p, xe, ec, eu, r, gs);
+    if (k == kPgZeroStar) return guided_value<kPgZeroStar>(p, xe, ec, eu, r, gs);
     return guided_value<kPgCombine>(p, xe, ec, eu, r, gs);
   } else if constexpr (K == kPgBypass) {
     return convert_param(p, ec, xe);
   } else if constexpr (K == kPgRescale) {
     return convert_param(p, rescale_value(p, eu + gs * (ec - eu), r), xe);
+  } else if constexpr (K == kPgZeroStar) {
+    const float us = eu * r;
+    return convert_param(p, us + gs * (ec - us), xe);
   } else {
     const float epc = convert_param(p, ec, xe);
     const float epu = convert_param(p, eu, xe);

@@ -20,7 +20,8 @@ constexpr int kMaxThreads = 512;
 // RS (only with NE == 2 and RND = false): guidance rescale (dpm_step_rescaled) with the per-sample ratio p.ratio, read
 // like the per-sample thresholds.
 // PG (only with NE == 2, RND = false and RS = false): per-sample guidance (dpm_step_guided) with the scale p.gscale
-// and, when p.ratio is set, the rescale -- one kernel family for rescale on and off.
+// and, when p.ratio is set, the rescale -- one kernel family for rescale on and off. With FAST = false it also serves
+// CFG-Zero* (dpm_step_cfgzero: p.zs set, p.gscale NULL for one scale p.guidance).
 // APG (only with NE == 2, FAST = false and no other option; the kernel k_step_direct_apg): adaptive projected guidance
 // (dpm_step_apg) with the per-sample words p.apg_a / p.apg_b; reads the fp32 direction p.apg_r in place of e_uncond
 // when it is set.
@@ -140,7 +141,8 @@ __device__ __forceinline__ void step_direct_body(const KParams& p) {
             // samples hold whole packets here (pick_direct): the sample's scale, ratio (when the launch is rescaled) and
             // threshold are one scalar each per packet
             const uint32_t b = (uint32_t)(pk / p.pk_per_sample);
-            const float gpk = __ldg(p.gscale + b), rpk = p.ratio != nullptr ? __ldg(p.ratio + b) : 1.f;
+            const float gpk = p.gscale != nullptr ? __ldg(p.gscale + b) : p.guidance;
+            const float rpk = p.zs != nullptr ? __ldg(p.zs + b) : (p.ratio != nullptr ? __ldg(p.ratio + b) : 1.f);
             const float tpk = clamp ? __ldg(p.thr + b) : 1.f;
             // the kind of the combine is uniform per packet: one branch per packet, straight-line code per element
             auto guided8 = [&](auto kind) {
@@ -152,6 +154,7 @@ __device__ __forceinline__ void step_direct_body(const KParams& p) {
             const int kind = pg_kind(p, gpk);
             if (kind == kPgBypass) guided8(std::integral_constant<int, kPgBypass>{});
             else if (kind == kPgRescale) guided8(std::integral_constant<int, kPgRescale>{});
+            else if (kind == kPgZeroStar) guided8(std::integral_constant<int, kPgZeroStar>{});
             else guided8(std::integral_constant<int, kPgCombine>{});
           } else {
             float thr8[8];
@@ -224,7 +227,7 @@ __global__ void __launch_bounds__(kMaxThreads) k_step_direct_apg(const __grid_co
 // RND = true: reference-rounding mode (common.cuh) for the launches the <RND> vector kernels do not serve:
 // unaligned views, tails and fp32 network outputs.
 // RS = true: guidance rescale (n_model == 2) for unaligned views, tails and dev_coef launches.
-// PG = true: per-sample guidance (n_model == 2; rescale iff p.ratio is set), likewise.
+// PG = true: per-sample guidance (n_model == 2; rescale iff p.ratio is set) and CFG-Zero* (p.zs set), likewise.
 // APG = true (the kernel k_step_scalar_apg): adaptive projected guidance (n_model == 2), likewise.
 template <bool RND, bool RS, bool PG, bool APG>
 __device__ __forceinline__ void step_scalar_body(const KParams& pc) {
@@ -262,8 +265,9 @@ __device__ __forceinline__ void step_scalar_body(const KParams& pc) {
                        clamp);
       } else if constexpr (PG) {
         const uint64_t b = (i + p.elem_offset) / p.per_sample;
-        mv = model_value<2, false, false, kPgAny>(p, xe, ec, eu, thr, clamp, p.ratio != nullptr ? p.ratio[b] : 1.f,
-                                                  p.gscale[b]);
+        const float r = p.zs != nullptr ? p.zs[b] : (p.ratio != nullptr ? p.ratio[b] : 1.f);
+        mv = model_value<2, false, false, kPgAny>(p, xe, ec, eu, thr, clamp, r,
+                                                  p.gscale != nullptr ? p.gscale[b] : p.guidance);
       } else if (RS) {
         mv = model_value<2, false, true>(p, xe, ec, eu, thr, clamp, p.ratio[(i + p.elem_offset) / p.per_sample]);
       } else {
@@ -308,8 +312,11 @@ typedef void (*StepKernel)(const KParams);
 // PG: per-sample guidance, NE == 2 only; serves rescaled and plain launches alike (so it is tested before RS).
 // APG: adaptive projected guidance, NE == 2 only, on the IEEE-division instantiations (tested first: it carries gscale
 // for its bypass).
+// CFG-Zero* (p.zs): the <PG> instantiations with FAST = false, with or without per-sample scales.
 static StepKernel pick_direct(const KParams& p) {
-  const bool fast = fast_path_ok(p), rnd = p.raw_round != 0, rs = p.ratio != nullptr, pg = p.gscale != nullptr;
+  const bool zs = p.zs != nullptr;
+  const bool fast = fast_path_ok(p) && !zs, rnd = p.raw_round != 0, rs = p.ratio != nullptr;
+  const bool pg = p.gscale != nullptr || zs;
   const bool apg = p.apg_a != nullptr;
   if ((pg || apg) && p.pk_per_sample == 0) return nullptr;
   return pick_step<StepKernel>(p, [&](auto pair, auto ne, auto form) -> StepKernel {
@@ -375,7 +382,7 @@ int launch_step_scalar(const KParams& p, cudaStream_t stream) {
   uint32_t grid = (uint32_t)(blocks < cap ? blocks : cap);
   if (p.raw_round) k_step_scalar<true><<<grid, threads, 0, stream>>>(p);
   else if (p.apg_a) k_step_scalar_apg<<<grid, threads, 0, stream>>>(p);
-  else if (p.gscale) k_step_scalar<false, false, true><<<grid, threads, 0, stream>>>(p);
+  else if (p.gscale || p.zs) k_step_scalar<false, false, true><<<grid, threads, 0, stream>>>(p);
   else if (p.ratio) k_step_scalar<false, true><<<grid, threads, 0, stream>>>(p);
   else k_step_scalar<false><<<grid, threads, 0, stream>>>(p);
   count_launch();

@@ -83,6 +83,9 @@ class StepArgs:
     apg_r: Optional[torch.Tensor] = None
     alpha_t: float = 1.0
     sigma_t: float = 0.0
+    # CFG-Zero* (dpm_step_cfgzero; n_model == 2, per_sample set): the per-sample scales s* of `cfgzero_scale()`, fp32
+    # [B]; `guidance_b`, when set, gives the per-sample guidance scales (else `guidance`)
+    cfgzero_s: Optional[torch.Tensor] = None
 
     def state_tensors(self):
         return [t for t in (self.x, self.xe, self.m0, self.m1, self.m2) if t is not None]
@@ -240,6 +243,9 @@ class CudaBackend:
             self._launch(ref.device, self._lib.dpm_step_apg, C.byref(d), C.c_void_p(a.apg_words.data_ptr()),
                          C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()),
                          C.c_void_p(None if r is None else r.data_ptr()), C.c_float(a.alpha_t), C.c_float(a.sigma_t))
+        elif a.cfgzero_s is not None:
+            self._launch(ref.device, self._lib.dpm_step_cfgzero, C.byref(d), C.c_void_p(a.cfgzero_s.data_ptr()),
+                         C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()))
         elif a.guidance_b is not None:
             # (phi and 1 - phi as below; ignored without a ratio)
             self._launch(ref.device, self._lib.dpm_step_guided, C.byref(d), C.c_void_p(a.guidance_b.data_ptr()),
@@ -256,7 +262,8 @@ class CudaBackend:
     @staticmethod
     def _check_per_sample(a: StepArgs, ref) -> None:
         """The per-sample operands of a step: fp32 on the tensors' device, one value per sample (the APG words two)."""
-        for v, what, k in ((a.ratio, "ratio", 1), (a.guidance_b, "guidance_b", 1), (a.apg_words, "apg_words", 2)):
+        for v, what, k in ((a.ratio, "ratio", 1), (a.guidance_b, "guidance_b", 1), (a.apg_words, "apg_words", 2),
+                           (a.cfgzero_s, "cfgzero_s", 1)):
             if v is None:
                 continue
             if not v.is_cuda or v.dtype != torch.float32 or not v.is_contiguous() or v.device != ref.device:
@@ -292,6 +299,26 @@ class CudaBackend:
                      C.c_void_p(None if ro is None else ro.data_ptr()), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
         return words
 
+    def cfgzero_scale(self, e_cond: torch.Tensor, e_uncond: torch.Tensor) -> torch.Tensor:
+        """CFG-Zero*'s per-sample s*_b = <c_b, u_b> / (||u_b||^2 + 1e-8) of the two raw halves, as fp32 [B] on the
+        device (dpm_cfgzero_scale): fp64 sums in storage order, merged per chunk in order. Both halves keep a shared
+        dense layout (a sample is one contiguous block in row-major and channels_last storage alike)."""
+        n, dev = e_cond.numel(), e_cond.device
+        layout = self._layout(e_cond)
+        if layout is None or self._layout(e_uncond) != layout:
+            layout = "c"
+        ec = self._check(e_cond, "e_cond", dev, n, layout=layout)
+        eu = self._check(e_uncond, "e_uncond", dev, n, e_cond.dtype, layout)
+        nb = e_cond.shape[0]
+        per_sample = n // nb
+        s = torch.empty(nb, dtype=torch.float32, device=dev)
+        ws_bytes = int(self._lib.dpm_cfgzero_workspace(nb, per_sample))
+        ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev)
+        self._launch(dev, self._lib.dpm_cfgzero_scale, C.c_void_p(s.data_ptr()), C.c_void_p(ec.data_ptr()),
+                     C.c_void_p(eu.data_ptr()), C.c_int(_DTYPE_CODE[e_cond.dtype]), C.c_uint64(per_sample),
+                     C.c_uint64(n), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
+        return s
+
     def _step_multi(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
         """dpm_step_multi: the K conditional outputs and scales of a multi-condition CFG step (d already filled)."""
         K = len(a.e_conds)
@@ -316,8 +343,9 @@ class CudaBackend:
 
     def _step_unipc(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
         """dpm_step_unipc: the UniPC words, m_{i-3} and the corrected-state output of a launch (d already filled)."""
-        if a.e_conds is not None or a.guidance_b is not None or a.ratio is not None or a.apg_words is not None:
-            raise ValueError("dpm_solver_b200: a UniPC step takes one guidance scale, without rescale or APG")
+        if a.e_conds is not None or a.guidance_b is not None or a.ratio is not None or a.apg_words is not None \
+                or a.cfgzero_s is not None:
+            raise ValueError("dpm_solver_b200: a UniPC step takes one guidance scale, without rescale, APG or CFG-Zero*")
         w, u = a.unipc, _lib.UniDesc()
         n = ref.numel()
         if a.m3 is not None:
@@ -399,9 +427,9 @@ class CudaBackend:
         """Per-sample s_b = max(quantile(|x0_b|, q), max_val) -> fp32 [B].
         return_stats=True also returns the pipeline's per-sample header words (int32 [B, 8]:
         lo key, hi key, #below, #inside, path (1 bracket / 2 exact fallback), ...) for diagnostics."""
-        if a.guidance_b is not None or a.e_conds is not None or a.apg_words is not None:
+        if a.guidance_b is not None or a.e_conds is not None or a.apg_words is not None or a.cfgzero_s is not None:
             raise ValueError("dpm_solver_b200: the quantile takes one guidance scale; materialise a per-sample, "
-                             "multi-condition or APG combine first")
+                             "multi-condition, APG or CFG-Zero* combine first")
         d, keep, ref, _, _ = self._fill(a)
         if a.per_sample <= 0 or ref.numel() % a.per_sample:
             raise ValueError("dpm_solver_b200: per_sample must divide numel")
@@ -607,8 +635,9 @@ class PreparedStep:
     def build(be: "CudaBackend", a: StepArgs) -> Optional["PreparedStep"]:
         if a.thr is not None or a.raw_round or a.ratio is not None or a.guidance_b is not None \
                 or a.e_conds is not None or a.coef_dev is not None or a.unipc is not None \
-                or a.apg_words is not None or a.out is not None and a.out2 is None:
-            # (a rescaled step reads a fresh ratio tensor every evaluation, an APG one fresh words, a guided one a scales tensor the
+                or a.apg_words is not None or a.cfgzero_s is not None or a.out is not None and a.out2 is None:
+            # (a rescaled step reads a fresh ratio tensor every evaluation, an APG one fresh words, a CFG-Zero* one fresh
+            # scales s*, a guided one a scales tensor the
             # descriptor does not carry, a multi-condition one K outputs and scales it does not carry, one with device
             # coefficients a block the descriptor would point into without owning it: never frozen)
             return None

@@ -55,6 +55,7 @@ class RawOutput:
     scales: Optional[tuple] = None
     is_x0: bool = False     # `e_cond` is a materialised x0 (a guided flow or EDM prediction): it is only clamped, not converted
     apg: Optional[tuple] = None     # adaptive projected guidance of the combine: (eta, norm_threshold, momentum)
+    cfgzero: bool = False           # CFG-Zero*: the combine against s*-scaled `e_uncond` (model_wrapper's cfg_zero_star)
 
 
 def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale):
@@ -148,9 +149,11 @@ class WrappedModel:
 
     def __init__(self, model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                  unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale=0.,
-                 apg_eta=None, apg_norm_threshold=0., apg_momentum=0.):
+                 apg_eta=None, apg_norm_threshold=0., apg_momentum=0., cfg_zero_star=False, cfg_zero_init_steps=0):
         self.model = model
         self.guidance_rescale = guidance_rescale
+        self.cfg_zero_star = bool(cfg_zero_star)
+        self.cfg_zero_init_steps = cfg_zero_init_steps
         self.apg_eta = apg_eta
         self.apg = None if apg_eta is None else (float(apg_eta), float(apg_norm_threshold), float(apg_momentum))
         self.noise_schedule = noise_schedule
@@ -287,8 +290,10 @@ class WrappedModel:
             t_in = None if t_input is not None else torch.cat([t_continuous] * 2)
             out_u, out_c = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(2)  # uncond first
             if gb is not None:
-                return RawOutput(out_c, out_u, param, 1.0, self.guidance_rescale, gb, apg=self.apg)
-            return RawOutput(out_c, out_u, param, float(self._one_scale()), self.guidance_rescale, apg=self.apg)
+                return RawOutput(out_c, out_u, param, 1.0, self.guidance_rescale, gb, apg=self.apg,
+                                 cfgzero=self.cfg_zero_star)
+            return RawOutput(out_c, out_u, param, float(self._one_scale()), self.guidance_rescale, apg=self.apg,
+                             cfgzero=self.cfg_zero_star)
         raise RuntimeError("raw() is not available with classifier guidance")
 
     def _alpha_sigma(self, t_continuous):
@@ -354,12 +359,15 @@ class WrappedModel:
         needs_x = r.param in (PARAM_BY_NAME["x_start"], PARAM_BY_NAME["v"], PARAM_FLOW, PARAM_EDM)
         xo = x.to(r.e_cond.dtype) if needs_x else None
         ratio = _cfg_ratio(be, r)      # over the whole batch: each sample's ratio reads its own values only
+        zs = be.cfgzero_scale(r.e_cond, r.e_uncond) if r.cfgzero and r.e_uncond is not None else None   # likewise
 
         def convert(rows, alpha, sigma):
             a = StepArgs(form=FORM_NONE, n_model=2 if r.e_uncond is not None else 1, e_cond=r.e_cond[rows],
                          e_uncond=None if r.e_uncond is None else r.e_uncond[rows], param=r.param,
                          guidance=r.guidance, alpha_e=alpha, sigma_e=sigma, state_dtype=r.e_cond.dtype)
             _guidance_args(a, None if ratio is None else ratio[rows], r, rows)
+            if zs is not None:
+                a.cfgzero_s, a.per_sample = zs[rows], a.e_cond.numel() // a.e_cond.shape[0]
             if needs_x:
                 a.xe = xo[rows]
             return be.step(a)[0]
@@ -368,7 +376,8 @@ class WrappedModel:
 
 def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, guidance_type="uncond",
                   condition=None, unconditional_condition=None, guidance_scale=1., classifier_fn=None,
-                  classifier_kwargs={}, guidance_rescale=0., apg_eta=None, apg_norm_threshold=0., apg_momentum=0.):
+                  classifier_kwargs={}, guidance_rescale=0., apg_eta=None, apg_norm_threshold=0., apg_momentum=0.,
+                  cfg_zero_star=False, cfg_zero_init_steps=0):
     """Wrap a network into `model_fn(x, t_continuous) -> noise`; same contract as the reference
     (:170-334): model_type in {noise, x_start, v, score}, guidance_type in {uncond, classifier,
     classifier-free}.
@@ -421,7 +430,27 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     1 keeps the bypass (one network half, no APG), a per-sample scale of 1 gives that row c. Not available (ValueError):
     other guidance types, no unconditional_condition, several conditions, guidance_rescale != 0, a non-finite eta or
     momentum, a negative or non-finite threshold, DPM_Solver(reference_rounding=True) and apg_momentum != 0 with
-    method="adaptive"."""
+    method="adaptive".
+
+    cfg_zero_star=True (classifier-free guidance only; not in the reference; default False): CFG-Zero* (Fan, Zheng,
+    Yeh and Liu 2025, arXiv:2503.18886), in the network's raw output space -- the velocity of a "flow" network, the
+    noise of a "noise" one, whatever the network returns for "x_start", "v", "score" and "edm". Per sample b, with c
+    and u the conditional and unconditional outputs flattened over all non-batch dimensions in storage order:
+        s*_b = fl32(<c_b, u_b> / (||u_b||^2 + 1e-8))   (the sums in fp64 over the fp32-widened outputs, the division in
+                                                       fp64, rounded to fp32 once; 1e-8 is diffusers' epsilon)
+        us = u*s*_b;  g = us + w_b*(c - us)             (three fp32 ops, each rounded, no contraction, in this order)
+    and the parameterisation then converts g as it converts a single output (combine raw, convert the result, as
+    guidance_rescale does). diffusers casts s* to the model's dtype and combines in it (bf16 for a bf16 network); this
+    library combines in fp32, as its plain CFG combine does. A scalar guidance_scale of 1 keeps the bypass (one network
+    half, the conditional output alone); a per-sample scale of 1 gives that row c.
+    cfg_zero_init_steps=K (an int >= 0; needs cfg_zero_star=True): zero-init. The first K network evaluations of each
+    sample() / inverse() run (DPM_Solver and UniPC) have a raw output of exactly 0 and do not call the network; the
+    solver then takes a one-output step on that 0 (for "flow" x0 = x exactly). Evaluations are counted in run order:
+    one per step for multistep and UniPC, every intermediate evaluation for singlestep, and the denoise_to_zero
+    evaluation. A direct call of this callable is never zeroed. Not available (ValueError): other guidance types, no
+    unconditional_condition, several conditions, guidance_rescale != 0, apg_eta, DPM_Solver(reference_rounding=True),
+    a cfg_zero_init_steps that is not an int >= 0 or that is set without cfg_zero_star=True, and cfg_zero_init_steps
+    > 0 with method="adaptive" (rejected steps leave "the first K evaluations" undefined)."""
     assert model_type in ["noise", "x_start", "v", "score", "flow", "edm"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
     flow_schedule = getattr(noise_schedule, "schedule", None) == "flow"
@@ -461,9 +490,22 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
             raise ValueError("apg_eta and apg_momentum must be finite, got {} and {}".format(apg_eta, apg_momentum))
         if not (math.isfinite(apg_norm_threshold) and apg_norm_threshold >= 0):
             raise ValueError("apg_norm_threshold must be finite and >= 0, got {}".format(apg_norm_threshold))
+    if not isinstance(cfg_zero_init_steps, int) or isinstance(cfg_zero_init_steps, bool) or cfg_zero_init_steps < 0:
+        raise ValueError("cfg_zero_init_steps must be an int >= 0, got {!r}".format(cfg_zero_init_steps))
+    if cfg_zero_init_steps and not cfg_zero_star:
+        raise ValueError("cfg_zero_init_steps needs cfg_zero_star=True")
+    if cfg_zero_star:
+        if guidance_type != "classifier-free" or unconditional_condition is None:
+            raise ValueError("cfg_zero_star needs guidance_type='classifier-free' and an unconditional_condition")
+        if isinstance(condition, (list, tuple)) and len(condition) >= 2:
+            raise ValueError("cfg_zero_star is not available with several conditions")
+        if guidance_rescale != 0:
+            raise ValueError("cfg_zero_star is not available with guidance_rescale")
+        if apg_eta is not None:
+            raise ValueError("cfg_zero_star is not available with adaptive projected guidance (apg_eta)")
     return WrappedModel(model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                         unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale,
-                        apg_eta, apg_norm_threshold, apg_momentum)
+                        apg_eta, apg_norm_threshold, apg_momentum, cfg_zero_star, cfg_zero_init_steps)
 
 
 # =================================================================================================
@@ -539,6 +581,8 @@ class DPM_Solver:
             raise ValueError("several conditions are not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "apg", None) is not None:
             raise ValueError("adaptive projected guidance is not available with reference_rounding=True")
+        if self.reference_rounding and getattr(model_fn, "cfg_zero_star", False):
+            raise ValueError("cfg_zero_star is not available with reference_rounding=True")
         self._rr_run = 0     # raw_round of the buffered values of the run in flight (reference_rounding)
         self._prep_cache = {}   # frozen launch descriptors of cached plan steps (ops.PreparedStep)
         self._prep_on = False
@@ -611,8 +655,12 @@ class DPM_Solver:
 
     # -- model evaluation ---------------------------------------------------------------------
     def _evaluate(self, x, t_dev, t_input=None) -> RawOutput:
-        """Call the user's network at (x, t); same call the reference makes through self.model."""
+        """Call the user's network at (x, t); same call the reference makes through self.model. CFG-Zero*'s zero-init
+        evaluations of a run return a raw output of 0 instead, without calling it."""
         w = self._wrapped
+        if self.__dict__.get("_cfz_left"):
+            self._cfz_left -= 1
+            return RawOutput(self._cfz_zeros(x), None, PARAM_BY_NAME[w.model_type], 1.0)
         orig = self.__dict__.get("_net_input")
         if orig is not None and orig[0] is x:
             x = orig[1]                           # the caller's own (16-bit) tensor, as the reference passes it
@@ -797,7 +845,7 @@ class DPM_Solver:
             # (and so is dynamic thresholding: a launch frozen without the clamp never serves a solver switched to it)
             pkey = (slot, raw.param, raw.guidance, raw.phi, raw.guidance_b is None, raw.e_uncond is None,
                     raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, raw.scales, self._dynamic_thresholding,
-                    raw.apg)
+                    raw.apg, raw.cfgzero)
             prep = self._prep_cache.get(pkey)
             if prep is not None:
                 r = prep.launch((x, xe, raw.e_cond, m1, m2, raw.e_cond, raw.e_uncond))
@@ -854,6 +902,19 @@ class DPM_Solver:
                 return m_new, x_next
             else:
                 apg_a = a
+        cfz = None          # CFG-Zero*'s per-sample s* of a fused evaluation
+        if raw.cfgzero and raw.e_uncond is not None:
+            # the s* pass over both raw halves (+2 launches), then the fused step. With dynamic thresholding (the
+            # quantile takes one plain combine), and under UniPC (its launch takes one network output and converts at its
+            # own state), g is materialised once in fp32 (+1 launch) and handed on as one network output of the same
+            # parameterisation: the combine runs in raw space, so no x0 detour is needed.
+            cfz = be.cfgzero_scale(raw.e_cond, raw.e_uncond)
+            if (x0 and self._dynamic_thresholding) or self._apg_materialise:
+                a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
+                             guidance=raw.guidance, state_dtype=torch.float32, guidance_b=raw.guidance_b,
+                             per_sample=raw.e_cond.numel() // raw.e_cond.shape[0], cfgzero_s=cfz)
+                raw = RawOutput(be.step(a)[0], None, raw.param, 1.0)
+                cfz = None
         ratio = _cfg_ratio(be, raw)     # guidance rescale: one streaming pass over both halves (+2 launches)
         if code:
             # reference-rounding mode (raw 16-bit NOISE outputs, fp32 state): bits 0-1 make the fused kernel take the
@@ -903,6 +964,8 @@ class DPM_Solver:
                 if co is not None else None
             return m_new, x_next
         a = apg_a if apg_a is not None else _guidance_args(self._conv_args(raw, xe, alsig, sd, x0), ratio, raw)
+        if cfz is not None:
+            a.cfgzero_s, a.per_sample = cfz, raw.e_cond.numel() // raw.e_cond.shape[0]
         if alsig is _DEV:
             if co is None or co.dev is None:
                 raise RuntimeError("device-side scalars need the coefficient block of the consuming launch")
@@ -939,7 +1002,8 @@ class DPM_Solver:
             self._remember(pkey, a, dup)
         return m_new, x_next
 
-    _apg_materialise = False     # UniPC: its launch takes one network output, so an APG value is materialised first
+    _apg_materialise = False     # UniPC: its launch takes one network output, so an APG or CFG-Zero* value is
+                                 # materialised first
 
     def _apg_buffers(self, raw: RawOutput, xe):
         """(r_prev, r_out) of an APG evaluation. Without momentum, or outside a sample() / inverse() run: (None, None).
@@ -955,12 +1019,24 @@ class DPM_Solver:
 
     @contextlib.contextmanager
     def _apg_scope(self):
-        """One sample() / inverse() run: the APG momentum buffer lives for its duration."""
+        """One sample() / inverse() run: the APG momentum buffer lives for its duration, and so do CFG-Zero*'s count of
+        zero-init evaluations left and its zero outputs."""
         self._apg_run, self._apg_r = True, None
+        self._cfz_left, self._cfz_zero = getattr(self._wrapped, "cfg_zero_init_steps", 0), {}
         try:
             yield
         finally:
             self._apg_run, self._apg_r = False, None
+            self._cfz_left, self._cfz_zero = 0, {}
+
+    def _cfz_zeros(self, x):
+        """The raw output 0 of a zero-init evaluation at state x: laid out like x, allocated once per run and
+        (shape, dtype, layout), and only ever read."""
+        key = (tuple(x.shape), x.dtype, x.stride(), x.device)
+        z = self._cfz_zero.get(key)
+        if z is None:
+            z = self._cfz_zero[key] = torch.zeros_like(x)
+        return z
 
     def _apg_momentum(self) -> float:
         apg = getattr(self._wrapped, "apg", None)
@@ -1423,6 +1499,9 @@ class DPM_Solver:
             assert method in ['multistep', 'singlestep', 'singlestep_fixed'], "Cannot use adaptive solver when saving intermediate values"
         if self.correcting_xt_fn is not None:
             assert method in ['multistep', 'singlestep', 'singlestep_fixed'], "Cannot use adaptive solver when correcting_xt_fn is not None"
+        if method == 'adaptive' and getattr(self._wrapped, "cfg_zero_init_steps", 0) > 0:
+            raise ValueError("cfg_zero_init_steps > 0 is not available with method='adaptive': its rejected steps leave "
+                             "'the first K evaluations' undefined")
         if method == 'adaptive' and self._apg_momentum() != 0:
             raise ValueError("apg_momentum != 0 is not available with method='adaptive': its evaluations, the device "
                              "controller's surplus iterations included, define no momentum sequence")

@@ -57,6 +57,11 @@ Adaptive projected guidance (model_wrapper's apg_eta) runs with a scalar scale: 
 launch that writes the buffered value m_i, then the UniPC launch reading it (n_model == 0). With dynamic thresholding
 the guided x0 is materialised in fp32 first, then thresholded, then buffered.
 
+CFG-Zero* (model_wrapper's cfg_zero_star) runs with a scalar scale: per evaluation the s* pass, one launch that
+materialises the guided raw output g in fp32, then the UniPC launch converting g as a single network output at its own
+state. Zero-init evaluations (cfg_zero_init_steps) are one-output launches on a raw output of 0, counted as in
+DPM_Solver.
+
 Not available (ValueError before any launch): per-sample guidance scales, several conditions, guidance rescale,
 reference_rounding, plan_broadcast, orders outside 1..3, steps < order.
 """
@@ -83,7 +88,7 @@ class _Launch:
 
 
 class UniPC(DPM_Solver):
-    _apg_materialise = True     # adaptive projected guidance: the buffered value (+1 launch), then this launch on it
+    _apg_materialise = True     # APG: the buffered value (+1 launch), then this launch on it; CFG-Zero*: g (+1 launch)
 
     def __init__(self, model_fn, noise_schedule, algorithm_type="dpmsolver++", variant="bh2", correcting_x0_fn=None,
                  correcting_xt_fn=None, thresholding_max_val=1., dynamic_thresholding_ratio=0.995, state_dtype=None):

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 106 /* 0.1.6: adaptive projected guidance (dpm_apg_words, dpm_step_apg) */
+#define DPM_B200_VERSION 107 /* 0.1.7: CFG-Zero* (dpm_cfgzero_scale, dpm_step_cfgzero) */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -345,6 +345,31 @@ DPM_API int dpm_apg_words(float* words, const dpm_step_desc* desc, const float* 
                           size_t workspace_bytes, dpm_stream_t stream);
 DPM_API int dpm_step_apg(const dpm_step_desc* desc, const float* words, const float* guidance, const float* r,
                          float alpha_t, float sigma_t, dpm_stream_t stream);
+
+/* ---- CFG-Zero* (Fan, Zheng, Yeh and Liu, "CFG-Zero*: Improved Classifier-Free Guidance for Flow Matching Models",
+ * 2025, arXiv:2503.18886) -------------------------------------------------------------------------------------------
+ * Classifier-free guidance against the unconditional output scaled per sample by its least-squares fit to the
+ * conditional one, in the network's raw output space. Per sample b of per_sample elements (c = e_cond, u = e_uncond,
+ * both flattened in storage order):
+ *   s*_b = fl32( <c_b, u_b> / (||u_b||^2 + 1e-8) )      (fp64 sums of the fp32-widened outputs, fp64 division)
+ *   us = u*s*_b,  g = us + w_b*(c - us)                 (three ops, each rounded to fp32, in this order)
+ * and the parameterisation then converts g as it converts a single output (dpm_step with n_model == 1 on g). A sample
+ * with w_b == 1 gets the converted c alone. The sums run per 8192-element chunk, merged in chunk order, so the bits of
+ * s*_b depend on sample b's values only.
+ * dpm_cfgzero_scale: s*_b -> s_out[0 .. n/per_sample), fp32 device memory. Reads the two halves only (2*s_model bytes
+ *   per element). workspace: dpm_cfgzero_workspace(n/per_sample, per_sample) bytes of 8-byte aligned device memory
+ *   (contents irrelevant). Two launches.
+ * dpm_step_cfgzero: dpm_step with g in place of the combine. guidance: NULL (w_b = desc->guidance) or the per-sample
+ *   scales, fp32 [n/per_sample] in device memory. Needs desc->n_model == 2, desc->raw_round == 0, desc->per_sample != 0
+ *   dividing n and s_star != NULL (DPM_ERR_ARG). Served by the IEEE-division instantiations of the direct vector
+ *   kernels for per-sample guidance (tails, unaligned views and dev_coef launches by the generic kernel); never by the
+ *   TMA variant. Call the scale pass and then the step on one stream; neither synchronises or allocates. */
+DPM_API size_t dpm_cfgzero_workspace(uint64_t n_samples, uint64_t per_sample);
+DPM_API int dpm_cfgzero_scale(float* s_out, const void* e_cond, const void* e_uncond, int model_dtype,
+                              uint64_t per_sample, uint64_t n, void* workspace, size_t workspace_bytes,
+                              dpm_stream_t stream);
+DPM_API int dpm_step_cfgzero(const dpm_step_desc* desc, const float* s_star, const float* guidance,
+                             dpm_stream_t stream);
 
 /* ---- multi-condition classifier-free guidance (composable prompts, Liu et al. 2022) ----------------------------
  * The network runs once on cat([x] * (n_cond + 1)) with the conditions cat([uc, c_1, ..., c_n]) and returns
