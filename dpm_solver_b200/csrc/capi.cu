@@ -405,6 +405,44 @@ static int step_unipc_impl(const dpm_step_desc* desc, const dpm_unipc_desc* u, c
   return finish(rc);
 }
 
+static int step_cfgpp_impl(const dpm_step_desc* desc, float g, const float* guidance, cudaStream_t stream) {
+  if (desc != nullptr && desc->n == 0) return DPM_OK;
+  if (desc == nullptr || (desc->form != DPM_FORM_LIN1 && desc->form != DPM_FORM_DIFF2) || desc->c0_on_old ||
+      desc->n_model != 2 || !desc->predict_x0 || desc->thr != nullptr || desc->raw_round != 0 ||
+      desc->dev_coef != nullptr) {
+    set_error("cfg++ step: needs form LIN1 or DIFF2 with c0_on_old == 0, n_model == 2, predict_x0 == 1, thr == NULL, "
+              "raw_round == 0 and dev_coef == NULL");
+    return DPM_ERR_ARG;
+  }
+  if (guidance != nullptr && (desc->per_sample == 0 || desc->n % desc->per_sample)) {
+    set_error("cfg++ step: per-sample guidance needs per_sample dividing n");
+    return DPM_ERR_ARG;
+  }
+  CfgppParams q;
+  memset(&q, 0, sizeof(q));
+  Needs nd;
+  int rc = build_params(desc, &q.k, &nd, false);
+  if (rc != DPM_OK) return rc;
+  q.k.gscale = guidance;
+  q.g = g;
+  const KParams& p = q.k;
+  Tuning t{g_variant.load(), g_threads.load(), g_ctas.load()};
+  bool body_done = false;
+  if (p.npk > 0 && all_aligned(p, nd)) {
+    const int r = launch_step_cfgpp(q, t, stream);
+    if (r < 0 || r > 1) return r;
+    body_done = (r == 0);
+  }
+  if (!body_done) {
+    rc = launch_step_cfgpp_scalar(q, stream);
+  } else if (p.n % kPacket) {
+    CfgppParams tail = q;
+    tail.k = shifted(p, (uint64_t)p.npk * kPacket);
+    rc = launch_step_cfgpp_scalar(tail, stream);
+  }
+  return finish(rc);
+}
+
 }  // namespace dpm
 
 using namespace dpm;
@@ -545,6 +583,10 @@ int dpm_step_cfgzero(const dpm_step_desc* desc, const float* s_star, const float
     return DPM_ERR_ARG;
   }
   return step_impl(desc, static_cast<cudaStream_t>(stream), nullptr, guidance, nullptr, s_star);
+}
+
+int dpm_step_cfgpp(const dpm_step_desc* desc, float g, const float* guidance, dpm_stream_t stream) {
+  return step_cfgpp_impl(desc, g, guidance, static_cast<cudaStream_t>(stream));
 }
 
 static dpm_step_desc base_desc(void* out, const void* x, uint64_t n, int dtype, int form) {

@@ -105,6 +105,13 @@ struct UniParams {
   float cd[2], ct;     // corrector words
   float a, c0, cp[2];  // predictor words
 };
+// CFG++ (dpm_step_cfgpp): a LIN1 or multistep DIFF2 update of a CFG pair (KParams as dpm_step builds it; gscale NULL
+// or the per-sample scales) that buffers the unguided x0 and adds g*(G - U); g = alpha_t of the step's end time.
+struct CfgppParams {
+  KParams k;
+  float g;
+};
+
 // the buffers a UniPC launch reads: m_{i-1} for the corrector or a predictor of order >= 2, m_{i-2} for a corrector of
 // order >= 2 or a predictor of order 3, m_{i-3} for a corrector of order 3
 struct UniReads {

@@ -120,6 +120,8 @@ int launch_step_multi(const MultiParams& mp, const Tuning& t, cudaStream_t strea
 int launch_step_multi_scalar(const MultiParams& mp, cudaStream_t stream);
 int launch_step_unipc(const UniParams& up, const Tuning& t, cudaStream_t stream);
 int launch_step_unipc_scalar(const UniParams& up, cudaStream_t stream);
+int launch_step_cfgpp(const CfgppParams& q, const Tuning& t, cudaStream_t stream);
+int launch_step_cfgpp_scalar(const CfgppParams& q, cudaStream_t stream);
 int launch_replicate(void* dst, const void* src, uint64_t bytes, int copies, cudaStream_t stream);
 int launch_quantile(float* s_out, const KParams& p, uint64_t n_samples, float q, float max_val,
                     void* workspace, size_t workspace_bytes, cudaStream_t stream);

@@ -86,6 +86,10 @@ class StepArgs:
     # CFG-Zero* (dpm_step_cfgzero; n_model == 2, per_sample set): the per-sample scales s* of `cfgzero_scale()`, fp32
     # [B]; `guidance_b`, when set, gives the per-sample guidance scales (else `guidance`)
     cfgzero_s: Optional[torch.Tensor] = None
+    # CFG++ (dpm_step_cfgpp; form LIN1 or DIFF2, n_model == 2, predict_x0): alpha_t of the update's end time, the weight
+    # of G - U; None is off. m_out then receives U, the x0 of e_uncond alone; `guidance_b`, when set, gives the
+    # per-sample scales (else `guidance`, always combined)
+    cfgpp_g: Optional[float] = None
 
     def state_tensors(self):
         return [t for t in (self.x, self.xe, self.m0, self.m1, self.m2) if t is not None]
@@ -243,6 +247,12 @@ class CudaBackend:
             self._launch(ref.device, self._lib.dpm_step_apg, C.byref(d), C.c_void_p(a.apg_words.data_ptr()),
                          C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()),
                          C.c_void_p(None if r is None else r.data_ptr()), C.c_float(a.alpha_t), C.c_float(a.sigma_t))
+        elif a.cfgpp_g is not None:
+            if a.thr is not None or a.ratio is not None or a.cfgzero_s is not None:
+                raise ValueError("dpm_solver_b200: a CFG++ step takes one or per-sample scales, without thresholds, "
+                                 "rescale or CFG-Zero*")
+            self._launch(ref.device, self._lib.dpm_step_cfgpp, C.byref(d), C.c_float(a.cfgpp_g),
+                         C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()))
         elif a.cfgzero_s is not None:
             self._launch(ref.device, self._lib.dpm_step_cfgzero, C.byref(d), C.c_void_p(a.cfgzero_s.data_ptr()),
                          C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()))
@@ -344,8 +354,9 @@ class CudaBackend:
     def _step_unipc(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
         """dpm_step_unipc: the UniPC words, m_{i-3} and the corrected-state output of a launch (d already filled)."""
         if a.e_conds is not None or a.guidance_b is not None or a.ratio is not None or a.apg_words is not None \
-                or a.cfgzero_s is not None:
-            raise ValueError("dpm_solver_b200: a UniPC step takes one guidance scale, without rescale, APG or CFG-Zero*")
+                or a.cfgzero_s is not None or a.cfgpp_g is not None:
+            raise ValueError("dpm_solver_b200: a UniPC step takes one guidance scale, without rescale, APG, CFG-Zero* "
+                             "or CFG++")
         w, u = a.unipc, _lib.UniDesc()
         n = ref.numel()
         if a.m3 is not None:
@@ -635,9 +646,10 @@ class PreparedStep:
     def build(be: "CudaBackend", a: StepArgs) -> Optional["PreparedStep"]:
         if a.thr is not None or a.raw_round or a.ratio is not None or a.guidance_b is not None \
                 or a.e_conds is not None or a.coef_dev is not None or a.unipc is not None \
-                or a.apg_words is not None or a.cfgzero_s is not None or a.out is not None and a.out2 is None:
+                or a.apg_words is not None or a.cfgzero_s is not None or a.cfgpp_g is not None \
+                or a.out is not None and a.out2 is None:
             # (a rescaled step reads a fresh ratio tensor every evaluation, an APG one fresh words, a CFG-Zero* one fresh
-            # scales s*, a guided one a scales tensor the
+            # scales s*, a CFG++ one goes through its own entry point, a guided one a scales tensor the
             # descriptor does not carry, a multi-condition one K outputs and scales it does not carry, one with device
             # coefficients a block the descriptor would point into without owning it: never frozen)
             return None

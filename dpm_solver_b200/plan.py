@@ -42,6 +42,7 @@ class Coeffs:
     order: int = 1
     r_tensor: int = 0   # SS3T: bit 0 / 1 = r1 / r2 came as tensors (matters to reference_rounding only)
     dev: Optional[torch.Tensor] = None   # scalars live in this device block instead (on-device adaptive controller)
+    g: float = 0.0      # CFG++ (dpm_step_cfgpp): alpha_t of the update's end time, the weight of G - U; 0 when not asked
 
 
 def _cpu(t: torch.Tensor) -> torch.Tensor:
@@ -196,9 +197,11 @@ def multistep_orders(steps: int, order: int, lower_order_final: bool) -> List[in
 
 
 def multistep_plan(ns, algorithm_type, solver_type, timesteps: torch.Tensor, order: int,
-                   lower_order_final: bool, marginals: Optional[Marginals] = None) -> List[Coeffs]:
+                   lower_order_final: bool, marginals: Optional[Marginals] = None, cfg_pp: bool = False) -> List[Coeffs]:
     """Coefficients of every update of a multistep run; plan[i] moves timesteps[i] -> [i+1].
-    One vectorised evaluation of the schedule over the grid, then one vector op set per order."""
+    One vectorised evaluation of the schedule over the grid, then one vector op set per order.
+    cfg_pp=True (dpmsolver++, orders 1 and 2): each update also carries g = alpha_t of its end time, the fp32 alpha its
+    c0 = -(alpha_t*phi_1) is formed from."""
     ts = _cpu(timesteps)
     steps = ts.numel() - 1
     M = marginals if marginals is not None else Marginals(ns, ts)
@@ -215,6 +218,10 @@ def multistep_plan(ns, algorithm_type, solver_type, timesteps: torch.Tensor, ord
         a, c0, c1, w0 = (v.reshape(-1).tolist() for v in _ms2(algorithm_type, solver_type, M[i - 1], M[i], M[i + 1]))
         for k, j in enumerate(idx[2]):
             plan[j] = Coeffs(FORM_DIFF2, a[k], c0[k], c1[k], w0=w0[k], order=2)
+    if cfg_pp:
+        g = M.alpha.reshape(-1).tolist()
+        for j in idx[1] + idx[2]:
+            plan[j].g = g[j + 1]
     if idx[3]:
         i = torch.tensor(idx[3])
         v = [u.reshape(-1).tolist() for u in _ms3(algorithm_type, M[i - 2], M[i - 1], M[i], M[i + 1])]

@@ -56,6 +56,7 @@ class RawOutput:
     is_x0: bool = False     # `e_cond` is a materialised x0 (a guided flow or EDM prediction): it is only clamped, not converted
     apg: Optional[tuple] = None     # adaptive projected guidance of the combine: (eta, norm_threshold, momentum)
     cfgzero: bool = False           # CFG-Zero*: the combine against s*-scaled `e_uncond` (model_wrapper's cfg_zero_star)
+    cfgpp: bool = False             # CFG++: an update buffers U (e_uncond alone) and adds g*(G - U) (model_wrapper's cfg_pp)
 
 
 def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale):
@@ -149,8 +150,10 @@ class WrappedModel:
 
     def __init__(self, model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                  unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale=0.,
-                 apg_eta=None, apg_norm_threshold=0., apg_momentum=0., cfg_zero_star=False, cfg_zero_init_steps=0):
+                 apg_eta=None, apg_norm_threshold=0., apg_momentum=0., cfg_zero_star=False, cfg_zero_init_steps=0,
+                 cfg_pp=False):
         self.model = model
+        self.cfg_pp = cfg_pp
         self.guidance_rescale = guidance_rescale
         self.cfg_zero_star = bool(cfg_zero_star)
         self.cfg_zero_init_steps = cfg_zero_init_steps
@@ -217,6 +220,11 @@ class WrappedModel:
     @property
     def uses_cfg(self) -> bool:
         # (several conditions: guidance_scale is their tuple of scales, never equal to 1 -- always combined, no bypass)
+        # (CFG++ reads both halves at every evaluation: a scalar scale of 1 is combined, not bypassed)
+        return self._combines() or self.cfg_pp
+
+    def _combines(self) -> bool:
+        """The plain guided noise combines the two halves (the reference's test :323)."""
         return (self.guidance_type == "classifier-free" and self.unconditional_condition is not None
                 and (self._scale_vec is not None or self._one_scale() != 1.))
 
@@ -266,11 +274,12 @@ class WrappedModel:
             self._c_in = (key, torch.cat([uc, c]), (uc, c))
         return self._c_in[1]
 
-    def raw(self, x, t_continuous, t_input=None, x_in=None) -> RawOutput:
+    def raw(self, x, t_continuous, t_input=None, x_in=None, plain=False) -> RawOutput:
         """Run the network exactly as the reference does, return its un-combined output(s).
 
         `t_input`, when given, is the precomputed model-input time vector (`input_rows(B)` long,
-        same values as get_model_input_time would produce) so that no per-call arithmetic runs."""
+        same values as get_model_input_time would produce) so that no per-call arithmetic runs.
+        `plain`: the outputs of the plain guided noise (a direct call of this callable), never marked for CFG++."""
         param = PARAM_BY_NAME[self.model_type]
         if self.guidance_type == "uncond":
             return RawOutput(self._call_model(x, t_continuous, t_input=t_input), None, param, 1.0)
@@ -283,17 +292,18 @@ class WrappedModel:
             return RawOutput(outs[1], outs[0], param, 1.0, e_conds=tuple(outs[1:]), scales=self.cond_scales)
         if self.guidance_type == "classifier-free":
             gb = self._scales(x) if self._scale_vec is not None else None     # (checked before the network runs)
-            if not self.uses_cfg:
+            if not (self._combines() if plain else self.uses_cfg):
                 return RawOutput(self._call_model(x, t_continuous, cond=self.condition, t_input=t_input), None, param, 1.0)
+            cfgpp = self.cfg_pp and not plain
             if x_in is None:
                 x_in = ops.backend().duplicate(x)              # cat([x] * 2) :326 (the solver hands over a prebuilt one)
             t_in = None if t_input is not None else torch.cat([t_continuous] * 2)
             out_u, out_c = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(2)  # uncond first
             if gb is not None:
                 return RawOutput(out_c, out_u, param, 1.0, self.guidance_rescale, gb, apg=self.apg,
-                                 cfgzero=self.cfg_zero_star)
+                                 cfgzero=self.cfg_zero_star, cfgpp=cfgpp)
             return RawOutput(out_c, out_u, param, float(self._one_scale()), self.guidance_rescale, apg=self.apg,
-                             cfgzero=self.cfg_zero_star)
+                             cfgzero=self.cfg_zero_star, cfgpp=cfgpp)
         raise RuntimeError("raw() is not available with classifier guidance")
 
     def _alpha_sigma(self, t_continuous):
@@ -338,7 +348,7 @@ class WrappedModel:
                 gs = float(torch.tensor(sigma, dtype=torch.float32) * self.guidance_scale)
                 return ops.lincomb(o, [grad[rows]], 1.0, [-gs])
             return self._per_sample(pairs, x.shape[0], guided)
-        r = self.raw(x, t_continuous)
+        r = self.raw(x, t_continuous, plain=True)
         if r.e_uncond is None and r.param == PARAM_NOISE:
             return r.e_cond
         if r.apg is not None and r.e_uncond is not None:
@@ -377,7 +387,7 @@ class WrappedModel:
 def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, guidance_type="uncond",
                   condition=None, unconditional_condition=None, guidance_scale=1., classifier_fn=None,
                   classifier_kwargs={}, guidance_rescale=0., apg_eta=None, apg_norm_threshold=0., apg_momentum=0.,
-                  cfg_zero_star=False, cfg_zero_init_steps=0):
+                  cfg_zero_star=False, cfg_zero_init_steps=0, cfg_pp=False):
     """Wrap a network into `model_fn(x, t_continuous) -> noise`; same contract as the reference
     (:170-334): model_type in {noise, x_start, v, score}, guidance_type in {uncond, classifier,
     classifier-free}.
@@ -450,7 +460,36 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     evaluation. A direct call of this callable is never zeroed. Not available (ValueError): other guidance types, no
     unconditional_condition, several conditions, guidance_rescale != 0, apg_eta, DPM_Solver(reference_rounding=True),
     a cfg_zero_init_steps that is not an int >= 0 or that is set without cfg_zero_star=True, and cfg_zero_init_steps
-    > 0 with method="adaptive" (rejected steps leave "the first K evaluations" undefined)."""
+    > 0 with method="adaptive" (rejected steps leave "the first K evaluations" undefined).
+
+    cfg_pp=True (classifier-free guidance only; not in the reference; default False): CFG++ (Chung, Kim, Park, Nam and
+    Ye, ICLR 2025, arXiv:2406.08070). It changes the solver update, not the guided value: each update denoises with the
+    guided x0 and re-noises with the UNCONDITIONAL noise, so that the DDIM step is x_t = alpha_t*x0_g + sigma_t*eps_u.
+    Scales are those of CFG++ (about 0.2 to 1), not those of plain CFG (about 5 to 12); guidance_scale is a scalar or a
+    per-sample [B] tensor as above. DPM_Solver(fn, ns, algorithm_type="dpmsolver++").sample(x, method="multistep",
+    order=1 or 2, ...) then computes, at every evaluation, for every element, in fp32 with each op rounded and no
+    contraction (S = the state dtype):
+        U = round_S(T_u)   T_u: the x0 the unguided step buffers for the unconditional output alone (every
+                           parameterisation as without guidance)
+        G = round_S(T_g)   T_g: the x0 the classifier-free step buffers with this sample's scale (a per-sample scale of 1
+                           takes the conditional output; a scalar scale of 1 is combined, not bypassed: CFG++ always
+                           needs both halves)
+        d = G - U
+        order 1 (first-update coefficients a, c0):        x_t = (a*x + c0*U) + g*d
+        order 2 (multistep coefficients a, c0, c1, w0):   x_t = ((a*x + c0*U) + g*d) + c1*(w0*(G - U_prev))
+    with g = alpha_t, the fp32 alpha of the update's end time that c0 is formed from, and U_prev the previous update's U:
+    the multistep buffer holds U, not G. In exact arithmetic order 1 is alpha_t*G + sigma_t*eps_u, the paper's DDIM
+    CFG++, and order 2 the 2M CFG++ recurrence; in VE coordinates (x^ = x/alpha, lambda = -log(sigma/alpha), h the
+    step in lambda, r the ratio of the previous step to h):
+        x^' = G + e^-h*(x^ - U) - expm1(-h)/(2r)*(G - U_prev)       (solver_type="taylor": its c1, by the same rule)
+    A network blind to the condition (e_c == e_u) gives d = 0, and a CFG++ run then equals the plain DPM-Solver++ run at
+    any scale. denoise_to_zero returns G; a direct call of this callable returns the plain guided noise. Accepted:
+    sample() and inverse() with every skip type, lower_order_final, return_intermediate, correcting_xt_fn, capture()
+    and batch sharding, on every schedule and model type. Not available (ValueError before any launch): other guidance
+    types, no unconditional_condition, several conditions, guidance_rescale != 0, apg_eta, cfg_zero_star, a cfg_pp
+    that is not a bool, and in the solver algorithm_type="dpmsolver", order 3, singlestep, singlestep_fixed and adaptive
+    methods, UniPC, the direct update methods (dpm_solver_first_update, multistep_dpm_solver_*_update, ...), dynamic
+    thresholding and any correcting_x0_fn, and reference_rounding=True."""
     assert model_type in ["noise", "x_start", "v", "score", "flow", "edm"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
     flow_schedule = getattr(noise_schedule, "schedule", None) == "flow"
@@ -494,6 +533,19 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
         raise ValueError("cfg_zero_init_steps must be an int >= 0, got {!r}".format(cfg_zero_init_steps))
     if cfg_zero_init_steps and not cfg_zero_star:
         raise ValueError("cfg_zero_init_steps needs cfg_zero_star=True")
+    if not isinstance(cfg_pp, bool):
+        raise ValueError("cfg_pp must be a bool, got {!r}".format(cfg_pp))
+    if cfg_pp:
+        if guidance_type != "classifier-free" or unconditional_condition is None:
+            raise ValueError("cfg_pp needs guidance_type='classifier-free' and an unconditional_condition")
+        if isinstance(condition, (list, tuple)) and len(condition) >= 2:
+            raise ValueError("cfg_pp is not available with several conditions")
+        if guidance_rescale != 0:
+            raise ValueError("cfg_pp is not available with guidance_rescale")
+        if apg_eta is not None:
+            raise ValueError("cfg_pp is not available with adaptive projected guidance (apg_eta)")
+        if cfg_zero_star:
+            raise ValueError("cfg_pp is not available with cfg_zero_star")
     if cfg_zero_star:
         if guidance_type != "classifier-free" or unconditional_condition is None:
             raise ValueError("cfg_zero_star needs guidance_type='classifier-free' and an unconditional_condition")
@@ -505,7 +557,7 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
             raise ValueError("cfg_zero_star is not available with adaptive projected guidance (apg_eta)")
     return WrappedModel(model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                         unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale,
-                        apg_eta, apg_norm_threshold, apg_momentum, cfg_zero_star, cfg_zero_init_steps)
+                        apg_eta, apg_norm_threshold, apg_momentum, cfg_zero_star, cfg_zero_init_steps, cfg_pp)
 
 
 # =================================================================================================
@@ -583,6 +635,13 @@ class DPM_Solver:
             raise ValueError("adaptive projected guidance is not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "cfg_zero_star", False):
             raise ValueError("cfg_zero_star is not available with reference_rounding=True")
+        if getattr(model_fn, "cfg_pp", False):
+            if algorithm_type != "dpmsolver++":
+                raise ValueError("cfg_pp needs algorithm_type='dpmsolver++' (CFG++ re-noises a data prediction)")
+            if correcting_x0_fn is not None:
+                raise ValueError("cfg_pp is not available with dynamic thresholding or a correcting_x0_fn")
+            if self.reference_rounding:
+                raise ValueError("cfg_pp is not available with reference_rounding=True")
         self._rr_run = 0     # raw_round of the buffered values of the run in flight (reference_rounding)
         self._prep_cache = {}   # frozen launch descriptors of cached plan steps (ops.PreparedStep)
         self._prep_on = False
@@ -845,7 +904,7 @@ class DPM_Solver:
             # (and so is dynamic thresholding: a launch frozen without the clamp never serves a solver switched to it)
             pkey = (slot, raw.param, raw.guidance, raw.phi, raw.guidance_b is None, raw.e_uncond is None,
                     raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, raw.scales, self._dynamic_thresholding,
-                    raw.apg, raw.cfgzero)
+                    raw.apg, raw.cfgzero, raw.cfgpp)
             prep = self._prep_cache.get(pkey)
             if prep is not None:
                 r = prep.launch((x, xe, raw.e_cond, m1, m2, raw.e_cond, raw.e_uncond))
@@ -856,6 +915,8 @@ class DPM_Solver:
                     if m_new is None and prep.d.n_model == 0:
                         m_new = raw.e_cond                  # pure update on the raw noise: it IS the buffered value
                     return m_new, x_next
+        if raw.cfgpp and co is not None:
+            return self._cfgpp_step(raw, xe, alsig, co, x, m1, want_m, dup_out)
         x0 = self._pp if x0 is None else x0          # buffered value: x0 (dpmsolver++ / data_prediction_fn) or eps
         sd = xe.dtype if xe is not None else (x.dtype if x is not None else raw.e_cond.dtype)
         custom_fix = x0 and self.correcting_x0_fn is not None and not self._dynamic_thresholding
@@ -1004,6 +1065,27 @@ class DPM_Solver:
 
     _apg_materialise = False     # UniPC: its launch takes one network output, so an APG or CFG-Zero* value is
                                  # materialised first
+
+    def _cfgpp_step(self, raw: RawOutput, xe, alsig, co: P.Coeffs, x, m1, want_m: bool, dup_out: bool):
+        """A CFG++ update (dpm_step_cfgpp, one launch): returns (U, x_next), U the x0 of the unconditional output alone,
+        which the multistep loop buffers in place of the guided x0."""
+        if co.form not in (FORM_LIN1, ops.FORM_DIFF2) or co.c0_on_old or co.dev is not None:
+            raise ValueError("cfg_pp takes DPM-Solver++ multistep updates of order 1 or 2")
+        a = _guidance_args(self._conv_args(raw, xe, alsig, xe.dtype, True), None, raw)
+        self._fill_update(a, co, x, m1, None)
+        a.cfgpp_g, a.want_m_out = co.g, want_m
+        dup = self._dup_target(x) if dup_out else None
+        if dup is not None:
+            a.out, a.out2 = dup[1], dup[2]
+        m_new, x_next = ops.backend().step(a)
+        if dup is not None:
+            self._xin_pair = (x_next, dup[0])
+        return m_new, x_next
+
+    def _no_cfgpp(self, what: str) -> None:
+        if getattr(self._wrapped, "cfg_pp", False):
+            raise ValueError("cfg_pp is not available with {}: CFG++ runs inside sample() / inverse() with "
+                             "method='multistep' and order 1 or 2".format(what))
 
     def _apg_buffers(self, raw: RawOutput, xe):
         """(r_prev, r_out) of an APG evaluation. Without momentum, or outside a sample() / inverse() run: (None, None).
@@ -1163,6 +1245,7 @@ class DPM_Solver:
     # -- reference API: single updates (direct-call path; scalars computed per call) -------------
     def dpm_solver_first_update(self, x, s, t, model_s=None, return_intermediate=False):
         """DPM-Solver-1 / DDIM step s -> t (:547-592)."""
+        self._no_cfgpp("dpm_solver_first_update")
         x = self._state(x)
         co = P.first_update_coeffs(self.noise_schedule, self.algorithm_type, s, t)
         if model_s is None:
@@ -1180,6 +1263,7 @@ class DPM_Solver:
     def singlestep_dpm_solver_second_update(self, x, s, t, r1=0.5, model_s=None, return_intermediate=False,
                                             solver_type='dpmsolver'):
         """Singlestep DPM-Solver-2 s -> t (:594-673)."""
+        self._no_cfgpp("singlestep_dpm_solver_second_update")
         if solver_type not in ['dpmsolver', 'taylor']:
             raise ValueError("'solver_type' must be either 'dpmsolver' or 'taylor', got {}".format(solver_type))
         sp = P.singlestep_second(self.noise_schedule, self.algorithm_type, solver_type, s, t, r1)
@@ -1191,6 +1275,7 @@ class DPM_Solver:
     def singlestep_dpm_solver_third_update(self, x, s, t, r1=1. / 3., r2=2. / 3., model_s=None, model_s1=None,
                                            return_intermediate=False, solver_type='dpmsolver'):
         """Singlestep DPM-Solver-3 s -> t (:675-794)."""
+        self._no_cfgpp("singlestep_dpm_solver_third_update")
         if solver_type not in ['dpmsolver', 'taylor']:
             raise ValueError("'solver_type' must be either 'dpmsolver' or 'taylor', got {}".format(solver_type))
         sp = P.singlestep_third(self.noise_schedule, self.algorithm_type, solver_type, s, t, r1, r2)
@@ -1245,6 +1330,7 @@ class DPM_Solver:
 
     def multistep_dpm_solver_second_update(self, x, model_prev_list, t_prev_list, t, solver_type="dpmsolver"):
         """Multistep DPM-Solver-2 (:796-852)."""
+        self._no_cfgpp("multistep_dpm_solver_second_update")
         if solver_type not in ['dpmsolver', 'taylor']:
             raise ValueError("'solver_type' must be either 'dpmsolver' or 'taylor', got {}".format(solver_type))
         co = P.multistep_coeffs(self.noise_schedule, self.algorithm_type, solver_type, 2, t_prev_list, t)
@@ -1252,6 +1338,7 @@ class DPM_Solver:
 
     def multistep_dpm_solver_third_update(self, x, model_prev_list, t_prev_list, t, solver_type='dpmsolver'):
         """Multistep DPM-Solver-3 (:854-904); needs exactly three buffered values."""
+        self._no_cfgpp("multistep_dpm_solver_third_update")
         model_prev_2, model_prev_1, model_prev_0 = model_prev_list
         t_prev_2, t_prev_1, t_prev_0 = t_prev_list
         co = P.multistep_coeffs(self.noise_schedule, self.algorithm_type, solver_type, 3,
@@ -1261,6 +1348,7 @@ class DPM_Solver:
     def singlestep_dpm_solver_update(self, x, s, t, order, return_intermediate=False, solver_type='dpmsolver',
                                      r1=None, r2=None):
         """Order dispatch (:906-930)."""
+        self._no_cfgpp("singlestep_dpm_solver_update")
         if order == 1:
             return self.dpm_solver_first_update(x, s, t, return_intermediate=return_intermediate)
         elif order == 2:
@@ -1274,6 +1362,7 @@ class DPM_Solver:
 
     def multistep_dpm_solver_update(self, x, model_prev_list, t_prev_list, t, order, solver_type='dpmsolver'):
         """Order dispatch (:932-954)."""
+        self._no_cfgpp("multistep_dpm_solver_update")
         if order == 1:
             return self.dpm_solver_first_update(x, t_prev_list[-1], t, model_s=model_prev_list[-1])
         elif order == 2:
@@ -1288,6 +1377,7 @@ class DPM_Solver:
                             t_err=1e-5, solver_type='dpmsolver'):
         """Adaptive step size DPM-Solver-12 / -23 (:956-1010). Updates and the error estimate run on
         the fused kernels; the step-size controller is the reference's host logic."""
+        self._no_cfgpp("method='adaptive'")
         ns = self.noise_schedule
         x = self._state(x)
         device = x.device
@@ -1492,6 +1582,8 @@ class DPM_Solver:
                method='multistep', lower_order_final=True, denoise_to_zero=False, solver_type='dpmsolver',
                atol=0.0078, rtol=0.05, return_intermediate=False):
         """Integrate the diffusion ODE from t_start to t_end; arguments as in the reference."""
+        if getattr(self._wrapped, "cfg_pp", False) and (method != "multistep" or order not in (1, 2)):
+            self._no_cfgpp("method='{}' and order {}".format(method, order))
         t_0 = 1. / self.noise_schedule.total_N if t_end is None else t_end
         t_T = self.noise_schedule.T if t_start is None else t_start
         assert t_0 > 0 and t_T > 0, "Time range needs to be greater than 0. For discrete-time DPMs, it needs to be in [1 / N, 1], where N is the length of betas array"
@@ -1527,13 +1619,16 @@ class DPM_Solver:
                 if order not in (1, 2, 3):
                     raise ValueError("Solver order must be 1 or 2 or 3, got {}".format(order))
                 key = ("multistep", steps, order, skip_type, t_T, t_0, solver_type, lower_order_final)
+                cfgpp = getattr(self._wrapped, "cfg_pp", False)
+                if cfgpp:
+                    key = key + ("cfg_pp",)     # (the plan carries g)
 
                 def build():
                     ts = self.get_time_steps(skip_type=skip_type, t_T=t_T, t_0=t_0, N=steps, device='cpu')
                     assert ts.shape[0] - 1 == steps
                     marg = P.Marginals(ns, ts)
                     plan = P.multistep_plan(ns, self.algorithm_type, solver_type, ts, order, lower_order_final,
-                                            marginals=marg)
+                                            marginals=marg, cfg_pp=cfgpp)
                     # (alpha_t, sigma_t) per grid point: scalars of the eps->x0 / parameterisation step
                     return ts, plan, list(zip(marg.alpha_e.tolist(), marg.sigma.tolist()))
 

@@ -126,6 +126,8 @@ class UniPC(DPM_Solver):
                 raise ValueError("several conditions are not available with UniPC")
             if w.guidance_type == "classifier-free" and w.guidance_rescale != 0:
                 raise ValueError("guidance_rescale is not available with UniPC")
+            if w.cfg_pp:
+                raise ValueError("cfg_pp is not available with UniPC (CFG++ is a DPM-Solver++ multistep update)")
 
     def inverse(self, x, steps=20, t_start=None, t_end=None, order=2, skip_type='time_uniform', lower_order_final=True,
                 denoise_to_zero=False, use_corrector=True, return_intermediate=False):

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 107 /* 0.1.7: CFG-Zero* (dpm_cfgzero_scale, dpm_step_cfgzero) */
+#define DPM_B200_VERSION 108 /* 0.1.8: CFG++ (dpm_step_cfgpp) */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -370,6 +370,27 @@ DPM_API int dpm_cfgzero_scale(float* s_out, const void* e_cond, const void* e_un
                               dpm_stream_t stream);
 DPM_API int dpm_step_cfgzero(const dpm_step_desc* desc, const float* s_star, const float* guidance,
                              dpm_stream_t stream);
+
+/* ---- CFG++ (Chung, Kim, Park, Nam and Ye, "CFG++: Manifold-constrained Classifier Free Guidance for Diffusion
+ * Models", ICLR 2025, arXiv:2406.08070) -------------------------------------------------------------------------------
+ * A DPM-Solver++ update that denoises with the guided data prediction and re-noises with the unconditional noise. Per
+ * element, in fp32 with every op rounded (S = desc->state_dtype):
+ *   U = round_S(T_u)   T_u: the x0 dpm_step buffers for e_uncond alone (n_model == 1, same param and words)
+ *   G = round_S(T_g)   T_g: the x0 dpm_step buffers for the pair (e_cond, e_uncond) with the sample's scale w_b; a
+ *                      sample with a per-sample w_b == 1 takes e_cond alone (as dpm_step_guided); desc->guidance is
+ *                      always combined, 1 included
+ *   LIN1:  out = (a*x + c0*U) + g*(G - U)
+ *   DIFF2: out = ((a*x + c0*U) + g*(G - U)) + c1*(w0*(G - m1))      (m1: the previous update's U)
+ * m_out (optional) receives U, out2 (optional) a second copy of out. g is alpha_t of the update's end time: in exact
+ * arithmetic LIN1 is then alpha_t*G + sigma_t*eps_u (the paper's DDIM) and DIFF2 the 2M CFG++ recurrence; with
+ * e_cond == e_uncond, G == U and both are the plain update. guidance: NULL (w_b = desc->guidance) or the per-sample
+ * scales, fp32 [n/per_sample] in device memory (then desc->per_sample must divide n). Needs desc->form LIN1 or DIFF2
+ * with c0_on_old == 0, n_model == 2, predict_x0 == 1, thr == NULL, raw_round == 0 and dev_coef == NULL (DPM_ERR_ARG).
+ * Reads x, e_cond, e_uncond [, m1] and writes out, out2, m_out: 6*s (LIN1) / 7*s (DIFF2) bytes per element with a
+ * state and model type of s bytes. Served by packet kernels for the five dtype pairs (tails, unaligned views and
+ * per-sample scales over samples that do not hold whole 8-element packets by the generic kernel); never by the TMA
+ * variant. */
+DPM_API int dpm_step_cfgpp(const dpm_step_desc* desc, float g, const float* guidance, dpm_stream_t stream);
 
 /* ---- multi-condition classifier-free guidance (composable prompts, Liu et al. 2022) ----------------------------
  * The network runs once on cat([x] * (n_cond + 1)) with the conditions cat([uc, c_1, ..., c_n]) and returns
