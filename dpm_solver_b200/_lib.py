@@ -61,6 +61,11 @@ class AdaptiveCtl(C.Structure):
     ]
 
 
+class CondMap(C.Structure):
+    """struct dpm_cond_map"""
+    _fields_ = [("w", C.c_void_p), ("period", C.c_uint64), ("sample_stride", C.c_uint64)]
+
+
 _vp, _f, _u64, _i = C.c_void_p, C.c_float, C.c_uint64, C.c_int
 
 # name -> (restype, argtypes); every prototype of the header appears here and is checked at load
@@ -97,6 +102,8 @@ PROTOTYPES = {
     "dpm_step_guided": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _f, _f, _vp]),
     "dpm_cfg_rescale_ratio_guided": (C.c_int, [_vp, _vp, _vp, _vp, _u64, _u64, _i, _vp, C.c_size_t, _vp]),
     "dpm_step_multi": (C.c_int, [C.POINTER(StepDesc), C.POINTER(_vp), C.POINTER(_f), _i, C.POINTER(_vp), _vp]),
+    "dpm_step_multi_masked": (C.c_int, [C.POINTER(StepDesc), C.POINTER(_vp), C.POINTER(_f), C.POINTER(CondMap), _i,
+                                        C.POINTER(_vp), _vp]),
     "dpm_replicate": (C.c_int, [_vp, _vp, _u64, _i, _i, _vp]),
     "dpm_step_unipc": (C.c_int, [C.POINTER(StepDesc), C.POINTER(UniDesc), _vp]),
     "dpm_apg_workspace": (C.c_size_t, [_u64, _u64]),

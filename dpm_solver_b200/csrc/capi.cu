@@ -300,14 +300,10 @@ static MultiParams shifted_multi(const MultiParams& mp, uint64_t elems) {
   return t;
 }
 
-static int step_multi_impl(const dpm_step_desc* desc, const void* const* e_conds, const float* scales, int n_cond,
-                           void* const* replicas, cudaStream_t stream) {
-  if (desc == nullptr || e_conds == nullptr || scales == nullptr || n_cond < 2 || n_cond > kMaxCond ||
-      desc->n_model != 2 || desc->raw_round != 0) {
-    set_error("multi-condition step: needs desc, e_conds, scales, 2 <= n_cond <= %d, n_model == 2 and raw_round == 0",
-              kMaxCond);
-    return DPM_ERR_ARG;
-  }
+// the outputs, scales and replicas of a multi-condition launch (n_cond, desc, e_conds and scales checked by the
+// caller): DPM_ERR_ARG for a NULL output or replica, else mp filled and *aligned_all set (desc->n != 0)
+static int build_multi(const dpm_step_desc* desc, const void* const* e_conds, const float* scales, int n_cond,
+                       void* const* replicas, MultiParams* mp, bool* aligned_all) {
   for (int k = 0; k < n_cond; ++k) {
     if (e_conds[k] == nullptr || (replicas != nullptr && replicas[k] == nullptr)) {
       set_error("multi-condition step: conditional output or replica %d is NULL", k);
@@ -318,19 +314,34 @@ static int step_multi_impl(const dpm_step_desc* desc, const void* const* e_conds
   dpm_step_desc d = *desc;
   d.e_cond = e_conds[0];   // (checked for NULL by build_params like any conditional output; the kernels read mp.ec)
   d.out2 = nullptr;
-  MultiParams mp;
-  memset(&mp, 0, sizeof(mp));
+  memset(mp, 0, sizeof(*mp));
   Needs nd;
-  int rc = build_params(&d, &mp.k, &nd, false);
+  int rc = build_params(&d, &mp->k, &nd, false);
   if (rc != DPM_OK) return rc;
-  mp.n_cond = n_cond;
-  bool aligned_all = all_aligned(mp.k, nd);
+  mp->n_cond = n_cond;
+  bool al = all_aligned(mp->k, nd);
   for (int k = 0; k < n_cond; ++k) {
-    mp.ec[k] = e_conds[k];
-    mp.s[k] = scales[k];
-    mp.rep[k] = (replicas != nullptr && d.form != DPM_FORM_NONE) ? replicas[k] : nullptr;
-    aligned_all = aligned_all && aligned(mp.ec[k], d.model_dtype) && (mp.rep[k] == nullptr || aligned(mp.rep[k], d.state_dtype));
+    mp->ec[k] = e_conds[k];
+    mp->s[k] = scales[k];
+    mp->rep[k] = (replicas != nullptr && d.form != DPM_FORM_NONE) ? replicas[k] : nullptr;
+    al = al && aligned(mp->ec[k], d.model_dtype) && (mp->rep[k] == nullptr || aligned(mp->rep[k], d.state_dtype));
   }
+  *aligned_all = al;
+  return DPM_OK;
+}
+
+static int step_multi_impl(const dpm_step_desc* desc, const void* const* e_conds, const float* scales, int n_cond,
+                           void* const* replicas, cudaStream_t stream) {
+  if (desc == nullptr || e_conds == nullptr || scales == nullptr || n_cond < 2 || n_cond > kMaxCond ||
+      desc->n_model != 2 || desc->raw_round != 0) {
+    set_error("multi-condition step: needs desc, e_conds, scales, 2 <= n_cond <= %d, n_model == 2 and raw_round == 0",
+              kMaxCond);
+    return DPM_ERR_ARG;
+  }
+  MultiParams mp;
+  bool aligned_all = false;
+  int rc = build_multi(desc, e_conds, scales, n_cond, replicas, &mp, &aligned_all);
+  if (rc != DPM_OK || desc->n == 0) return rc;
   Tuning t{g_variant.load(), g_threads.load(), g_ctas.load()};
   bool body_done = false;
   if (mp.k.npk > 0 && aligned_all && mp.k.dev_coef == nullptr) {   // device-side scalars: generic kernel only
@@ -342,6 +353,54 @@ static int step_multi_impl(const dpm_step_desc* desc, const void* const* e_conds
     rc = launch_step_multi_scalar(mp, stream);
   } else if (mp.k.n % kPacket) {
     rc = launch_step_multi_scalar(shifted_multi(mp, (uint64_t)mp.k.npk * kPacket), stream);   // tail
+  }
+  return finish(rc);
+}
+
+static int step_multi_masked_impl(const dpm_step_desc* desc, const void* const* e_conds, const float* scales,
+                                  const dpm_cond_map* maps, int n_cond, void* const* replicas, cudaStream_t stream) {
+  if (desc == nullptr || e_conds == nullptr || scales == nullptr || maps == nullptr || n_cond < 1 ||
+      n_cond > kMaxCond || desc->n_model != 2 || desc->raw_round != 0) {
+    set_error("masked multi-condition step: needs desc, e_conds, scales, maps, 1 <= n_cond <= %d, n_model == 2 and "
+              "raw_round == 0", kMaxCond);
+    return DPM_ERR_ARG;
+  }
+  if (desc->per_sample == 0 || desc->n % desc->per_sample != 0) {
+    set_error("masked multi-condition step: per_sample must be nonzero and divide n");
+    return DPM_ERR_ARG;
+  }
+  for (int k = 0; k < n_cond; ++k) {
+    const dpm_cond_map& m = maps[k];
+    if (m.w != nullptr && (m.period == 0 || desc->per_sample % m.period != 0 ||
+                           (m.sample_stride != 0 && m.sample_stride != m.period))) {
+      set_error("masked multi-condition step: map %d needs a period dividing per_sample and a sample_stride of 0 or "
+                "the period", k);
+      return DPM_ERR_ARG;
+    }
+  }
+  MaskedParams q;
+  memset(&q, 0, sizeof(q));
+  bool aligned_all = false;
+  int rc = build_multi(desc, e_conds, scales, n_cond, replicas, &q.m, &aligned_all);
+  if (rc != DPM_OK || desc->n == 0) return rc;
+  for (int k = 0; k < n_cond; ++k) {
+    q.w[k] = maps[k].w;
+    q.period[k] = maps[k].w != nullptr ? maps[k].period : 1;
+    q.sstride[k] = maps[k].w != nullptr ? maps[k].sample_stride : 0;
+  }
+  Tuning t{g_variant.load(), g_threads.load(), g_ctas.load()};
+  bool body_done = false;
+  if (q.m.k.npk > 0 && aligned_all && q.m.k.dev_coef == nullptr) {   // device-side scalars: generic kernel only
+    const int r = launch_step_multi_masked(q, t, stream);
+    if (r < 0 || r > 1) return r;
+    body_done = (r == 0);
+  }
+  if (!body_done) {
+    rc = launch_step_multi_masked_scalar(q, stream);
+  } else if (q.m.k.n % kPacket) {
+    MaskedParams tail = q;
+    tail.m = shifted_multi(q.m, (uint64_t)q.m.k.npk * kPacket);
+    rc = launch_step_multi_masked_scalar(tail, stream);
   }
   return finish(rc);
 }
@@ -683,6 +742,11 @@ int dpm_duplicate(void* out, const void* x, uint64_t n, int dtype, dpm_stream_t 
 int dpm_step_multi(const dpm_step_desc* desc, const void* const* e_conds, const float* scales, int n_cond,
                    void* const* replicas, dpm_stream_t stream) {
   return step_multi_impl(desc, e_conds, scales, n_cond, replicas, static_cast<cudaStream_t>(stream));
+}
+
+int dpm_step_multi_masked(const dpm_step_desc* desc, const void* const* e_conds, const float* scales,
+                          const dpm_cond_map* maps, int n_cond, void* const* replicas, dpm_stream_t stream) {
+  return step_multi_masked_impl(desc, e_conds, scales, maps, n_cond, replicas, static_cast<cudaStream_t>(stream));
 }
 
 int dpm_step_unipc(const dpm_step_desc* desc, const dpm_unipc_desc* u, dpm_stream_t stream) {

@@ -94,6 +94,16 @@ struct MultiParams {
   int32_t n_cond;
 };
 
+// regional multi-condition guidance (dpm_step_multi_masked): MultiParams with one weight map per condition, the weight
+// of s[k] at global element i being w[k][b*sstride[k] + (i - b*k.per_sample) % period[k]], b = i / k.per_sample
+// (w[k] NULL: 1). MultiParams stays as it is, so k_step_multi keeps its code.
+struct MaskedParams {
+  MultiParams m;
+  const float* w[kMaxCond];
+  uint64_t period[kMaxCond];
+  uint64_t sstride[kMaxCond];
+};
+
 // UniPC (dpm_step_unipc): the corrector of step i and the predictor of step i+1 around the conversion of KParams, whose
 // own update fields (form, a, c*, w*) are not read. k.x is x~_i (also the evaluation state), k.m0 m_i when n_model == 0,
 // k.m1 / k.m2 / m3 the buffers m_{i-1} / m_{i-2} / m_{i-3}; out_c (optional) receives the corrected x_i.

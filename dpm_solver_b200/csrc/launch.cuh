@@ -118,6 +118,8 @@ int launch_select_copy(void* dst, const void* src, const float* state, uint64_t 
 int launch_duplicate(void* dst, const void* src, uint64_t bytes, cudaStream_t stream);
 int launch_step_multi(const MultiParams& mp, const Tuning& t, cudaStream_t stream);
 int launch_step_multi_scalar(const MultiParams& mp, cudaStream_t stream);
+int launch_step_multi_masked(const MaskedParams& q, const Tuning& t, cudaStream_t stream);
+int launch_step_multi_masked_scalar(const MaskedParams& q, cudaStream_t stream);
 int launch_step_unipc(const UniParams& up, const Tuning& t, cudaStream_t stream);
 int launch_step_unipc_scalar(const UniParams& up, cudaStream_t stream);
 int launch_step_cfgpp(const CfgppParams& q, const Tuning& t, cudaStream_t stream);

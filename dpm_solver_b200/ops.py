@@ -70,6 +70,12 @@ class StepArgs:
     e_conds: Optional[Tuple[torch.Tensor, ...]] = None
     scales: Optional[Tuple[float, ...]] = None
     replicas: Optional[Tuple[torch.Tensor, ...]] = None
+    # regional guidance (dpm_step_multi_masked; with e_conds, 1 <= K <= 4, per_sample set): one weight map per condition,
+    # None (all ones), (w, period, sample_stride) with w a contiguous fp32 tensor on the tensors' device, or an object
+    # whose weights(shape, layout, device) gives that triple for the launch's shape and storage order ('c' or 'cl'). The
+    # weight of scales[k] at element i (storage order) is w.view(-1)[b*sample_stride + (i - b*per_sample) % period],
+    # b = i // per_sample.
+    masks: Optional[Tuple[Optional[tuple], ...]] = None
     # UniPC (dpm_step_unipc): the launch's words (plan.UniCoeffs), m_{i-3}, and an optional preallocated tensor that
     # receives the corrected state x_i (required when the launch has no predictor). `x` is x~_i, `m1`/`m2` m_{i-1}/m_{i-2}.
     unipc: Optional[object] = None
@@ -330,14 +336,18 @@ class CudaBackend:
         return s
 
     def _step_multi(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
-        """dpm_step_multi: the K conditional outputs and scales of a multi-condition CFG step (d already filled)."""
+        """dpm_step_multi: the K conditional outputs and scales of a multi-condition CFG step (d already filled); with
+        `a.masks`, dpm_step_multi_masked (1 <= K <= 4)."""
         K = len(a.e_conds)
-        if not 2 <= K <= _lib.MAX_CONDITIONS or a.scales is None or len(a.scales) != K or a.n_model != 2:
-            raise ValueError("dpm_solver_b200: a multi-condition step takes 2..{} conditional outputs, one scale each, "
-                             "and n_model == 2".format(_lib.MAX_CONDITIONS))
+        k_min = 1 if a.masks is not None else 2
+        if not k_min <= K <= _lib.MAX_CONDITIONS or a.scales is None or len(a.scales) != K or a.n_model != 2 \
+                or a.masks is not None and len(a.masks) != K:
+            raise ValueError("dpm_solver_b200: a multi-condition step takes {}..{} conditional outputs, one scale (and "
+                             "with masks one mask) each, and n_model == 2".format(k_min, _lib.MAX_CONDITIONS))
         if a.replicas is not None and len(a.replicas) != K:
             raise ValueError("dpm_solver_b200: a multi-condition step takes one replica per condition")
         n, mdt = ref.numel(), a.e_cond.dtype
+        maps = None if a.masks is None else self._cond_maps(a, ref, layout, keep)
         ecs = [self._check(e, "e_conds[%d]" % k, ref.device, n, mdt, layout) for k, e in enumerate(a.e_conds)]
         keep.extend(ecs)
         reps = None
@@ -348,8 +358,32 @@ class CudaBackend:
                     raise ValueError("dpm_solver_b200: replicas must be dense and laid out like out")
             reps = (C.c_void_p * K)(*[r.data_ptr() for r in a.replicas])
         d.out2 = None
-        self._launch(ref.device, self._lib.dpm_step_multi, C.byref(d),
-                     (C.c_void_p * K)(*[e.data_ptr() for e in ecs]), (C.c_float * K)(*a.scales), C.c_int(K), reps)
+        ecp, sc = (C.c_void_p * K)(*[e.data_ptr() for e in ecs]), (C.c_float * K)(*a.scales)
+        if maps is None:
+            self._launch(ref.device, self._lib.dpm_step_multi, C.byref(d), ecp, sc, C.c_int(K), reps)
+        else:
+            self._launch(ref.device, self._lib.dpm_step_multi_masked, C.byref(d), ecp, sc, maps, C.c_int(K), reps)
+
+    @staticmethod
+    def _cond_maps(a: StepArgs, ref, layout, keep):
+        """The dpm_cond_map array of `a.masks`, each map checked against the launch's size and per_sample."""
+        n = ref.numel()
+        if a.per_sample <= 0 or n % a.per_sample:
+            raise ValueError("dpm_solver_b200: a masked multi-condition step needs per_sample dividing numel")
+        maps = (_lib.CondMap * len(a.masks))()
+        for k, m in enumerate(a.masks):
+            if m is None:
+                continue
+            w, period, stride = m if isinstance(m, tuple) else m.weights(tuple(ref.shape), layout, ref.device)
+            if not w.is_cuda or w.device != ref.device or w.dtype != torch.float32 or not w.is_contiguous():
+                raise TypeError("dpm_solver_b200: a weight map must be a contiguous fp32 tensor on the tensors' device")
+            if period <= 0 or a.per_sample % period or stride not in (0, period) \
+                    or w.numel() != (period if stride == 0 else period * (n // a.per_sample)):
+                raise ValueError("dpm_solver_b200: weight map {} does not fit period {} and sample stride {}".format(
+                    k, period, stride))
+            keep.append(w)
+            maps[k].w, maps[k].period, maps[k].sample_stride = w.data_ptr(), period, stride
+        return maps
 
     def _step_unipc(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
         """dpm_step_unipc: the UniPC words, m_{i-3} and the corrected-state output of a launch (d already filled)."""

@@ -53,16 +53,17 @@ class RawOutput:
     # and their fp32-rounded scales; `guidance` is then not read
     e_conds: Optional[tuple] = None
     scales: Optional[tuple] = None
+    masks: Optional[tuple] = None   # regional guidance: one _CondMask or None (all ones) per condition, with e_conds
     is_x0: bool = False     # `e_cond` is a materialised x0 (a guided flow or EDM prediction): it is only clamped, not converted
     apg: Optional[tuple] = None     # adaptive projected guidance of the combine: (eta, norm_threshold, momentum)
     cfgzero: bool = False           # CFG-Zero*: the combine against s*-scaled `e_uncond` (model_wrapper's cfg_zero_star)
     cfgpp: bool = False             # CFG++: an update buffers U (e_uncond alone) and adds g*(G - U) (model_wrapper's cfg_pp)
 
 
-def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale):
+def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale, masked=False):
     """model_wrapper's list or tuple of conditions -> (condition, guidance_scale, per-condition scales or None).
-    One condition is the tensor form (its scale as one python float); K >= 2 conditions keep their K scales, each read
-    on the host once and rounded to fp32 once."""
+    One condition is the tensor form (its scale as one python float); K >= 2 conditions, or any K with guidance masks,
+    keep their K scales, each read on the host once and rounded to fp32 once."""
     K = len(condition)
     if not 1 <= K <= ops._lib.MAX_CONDITIONS:
         raise ValueError("classifier-free guidance takes 1 to {} conditions, got {}".format(ops._lib.MAX_CONDITIONS, K))
@@ -77,13 +78,66 @@ def _multi_condition(condition, unconditional_condition, guidance_scale, guidanc
     if s.numel() != K:
         raise ValueError("{} guidance scales for {} conditions".format(s.numel(), K))
     scales = tuple(s.tolist())
-    if K == 1:
+    if K == 1 and not masked:
         return condition[0], scales[0], None
     if unconditional_condition is None:
         raise ValueError("classifier-free guidance with {} conditions needs an unconditional_condition".format(K))
     if guidance_rescale != 0:
         raise ValueError("guidance_rescale is not available with several conditions")
     return tuple(condition), scales, scales
+
+
+class _CondMask:
+    """One condition's guidance_mask. A mask that broadcasts to x's shape [B, C, *spatial] (batch extent 1 or B) becomes
+    the weight map of dpm_step_multi_masked, once per (tensor, version, shape, storage order): period 1 when it is
+    constant over every non-batch dim, a pixel map (period = spatial size) when it is constant over the channels of a
+    row-major x, else an element map in x's storage order (channels_last included). Values are taken in fp32. A
+    contiguous fp32 tensor on x's device that already has the map's layout is read in place, so a captured graph sees
+    values written into it."""
+
+    def __init__(self, mask: torch.Tensor):
+        self.mask = mask
+        self._cache = None
+
+    def check(self, shape) -> None:
+        """ValueError unless the mask broadcasts to `shape` (so its batch extent is 1 or shape[0])."""
+        m = self.mask
+        if m.dim() > len(shape) or any(a != 1 and a != b for a, b in zip(m.shape[::-1], tuple(shape)[::-1])):
+            raise ValueError("guidance_mask of shape {} does not broadcast to x's shape {}".format(
+                tuple(m.shape), tuple(shape)))
+
+    def weights(self, shape, layout: str, device):
+        """(w, period, sample_stride) for a launch over `shape` in storage order `layout` ('c' or 'cl') on `device`."""
+        key = (id(self.mask), self.mask._version, tuple(shape), layout, str(device))
+        if self._cache is None or self._cache[0] != key:
+            self.check(shape)
+            self._cache = (key, self._canonical(tuple(shape), layout, device))
+        return self._cache[1]
+
+    def _canonical(self, shape, layout, device):
+        B, d = shape[0], len(shape)
+        m = self.mask.detach()
+        m = m.reshape((1,) * (d - m.dim()) + tuple(m.shape)).to(device=device, dtype=torch.float32)
+        bm = m.shape[0]
+        per_sample = math.prod(shape[1:])
+        if all(v == 1 for v in m.shape[1:]):
+            w, period = m.reshape(bm, 1), 1
+        elif layout == "c" and d >= 3 and m.shape[1] == 1:
+            period = math.prod(shape[2:])
+            w = m.expand((bm, 1) + shape[2:]).reshape(bm, period)
+        else:
+            full = m.expand((bm,) + shape[1:])
+            if layout == "cl":
+                full = full.permute(0, *range(2, d), 1)      # channels_last storage order
+            w, period = full.reshape(bm, per_sample), per_sample
+        return w.contiguous(), period, (period if bm == B and B != 1 else 0)
+
+    def rows(self, rows, x_dims: int) -> "_CondMask":
+        """The mask of the batch rows `rows` of an x with `x_dims` dims (a mask shared by the batch is kept)."""
+        m = self.mask
+        if m.dim() < x_dims or m.shape[0] == 1:
+            return self
+        return _CondMask(m[rows])
 
 
 def _cfg_ratio(be, raw: RawOutput) -> Optional[torch.Tensor]:
@@ -106,7 +160,10 @@ def _guidance_args(a: StepArgs, ratio: Optional[torch.Tensor], raw: RawOutput, r
     if raw.e_conds is not None and a.n_model == 2:
         a.e_conds = raw.e_conds if rows is None else tuple(e[rows] for e in raw.e_conds)
         a.scales = raw.scales
-    if a.ratio is not None or a.guidance_b is not None:
+        if raw.masks is not None:
+            d = raw.e_cond.dim()
+            a.masks = raw.masks if rows is None else tuple(m if m is None else m.rows(rows, d) for m in raw.masks)
+    if a.ratio is not None or a.guidance_b is not None or a.masks is not None:
         a.per_sample = a.e_cond.numel() // a.e_cond.shape[0]
     return a
 
@@ -151,7 +208,7 @@ class WrappedModel:
     def __init__(self, model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                  unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale=0.,
                  apg_eta=None, apg_norm_threshold=0., apg_momentum=0., cfg_zero_star=False, cfg_zero_init_steps=0,
-                 cfg_pp=False):
+                 cfg_pp=False, guidance_mask=None):
         self.model = model
         self.cfg_pp = cfg_pp
         self.guidance_rescale = guidance_rescale
@@ -163,10 +220,13 @@ class WrappedModel:
         self.model_type = model_type
         self.model_kwargs = model_kwargs
         self.guidance_type = guidance_type
-        self.cond_scales = None     # K >= 2 conditions: their K scales (python floats, fp32-rounded)
+        self.cond_scales = None     # K >= 2 conditions (any K with masks): their K scales (python floats, fp32-rounded)
+        # regional guidance: one _CondMask or None per condition (model_wrapper's guidance_mask, normalised to a list)
+        self.cond_masks = None if guidance_mask is None else tuple(
+            None if m is None else _CondMask(m) for m in guidance_mask)
         if guidance_type == "classifier-free" and isinstance(condition, (list, tuple)):
             condition, guidance_scale, self.cond_scales = _multi_condition(
-                condition, unconditional_condition, guidance_scale, guidance_rescale)
+                condition, unconditional_condition, guidance_scale, guidance_rescale, self.cond_masks is not None)
         self.condition = condition
         self.unconditional_condition = unconditional_condition
         if isinstance(guidance_scale, (list, tuple)) and self.cond_scales is None:
@@ -202,7 +262,7 @@ class WrappedModel:
 
     @property
     def n_cond(self) -> int:
-        """Number of conditions of a multi-condition run (K >= 2), else 0."""
+        """Number of conditions of a multi-condition run (K >= 2, or K >= 1 with guidance masks), else 0."""
         return 0 if self.cond_scales is None else len(self.cond_scales)
 
     def _one_scale(self):
@@ -285,11 +345,15 @@ class WrappedModel:
             return RawOutput(self._call_model(x, t_continuous, t_input=t_input), None, param, 1.0)
         if self.guidance_type == "classifier-free" and self.cond_scales is not None:
             n = len(self.cond_scales) + 1
+            for m in self.cond_masks or ():
+                if m is not None:
+                    m.check(x.shape)                              # (before any launch)
             if x_in is None:
                 x_in = ops.backend().replicate(x, n)              # cat([x] * (K+1)) (the solver hands over a prebuilt one)
             t_in = None if t_input is not None else torch.cat([t_continuous] * n)
             outs = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(n)   # uncond first
-            return RawOutput(outs[1], outs[0], param, 1.0, e_conds=tuple(outs[1:]), scales=self.cond_scales)
+            return RawOutput(outs[1], outs[0], param, 1.0, e_conds=tuple(outs[1:]), scales=self.cond_scales,
+                             masks=self.cond_masks)
         if self.guidance_type == "classifier-free":
             gb = self._scales(x) if self._scale_vec is not None else None     # (checked before the network runs)
             if not (self._combines() if plain else self.uses_cfg):
@@ -387,7 +451,7 @@ class WrappedModel:
 def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, guidance_type="uncond",
                   condition=None, unconditional_condition=None, guidance_scale=1., classifier_fn=None,
                   classifier_kwargs={}, guidance_rescale=0., apg_eta=None, apg_norm_threshold=0., apg_momentum=0.,
-                  cfg_zero_star=False, cfg_zero_init_steps=0, cfg_pp=False):
+                  cfg_zero_star=False, cfg_zero_init_steps=0, cfg_pp=False, guidance_mask=None):
     """Wrap a network into `model_fn(x, t_continuous) -> noise`; same contract as the reference
     (:170-334): model_type in {noise, x_start, v, score}, guidance_type in {uncond, classifier,
     classifier-free}.
@@ -489,7 +553,34 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     types, no unconditional_condition, several conditions, guidance_rescale != 0, apg_eta, cfg_zero_star, a cfg_pp
     that is not a bool, and in the solver algorithm_type="dpmsolver", order 3, singlestep, singlestep_fixed and adaptive
     methods, UniPC, the direct update methods (dpm_solver_first_update, multistep_dpm_solver_*_update, ...), dynamic
-    thresholding and any correcting_x0_fn, and reference_rounding=True."""
+    thresholding and any correcting_x0_fn, and reference_rounding=True.
+
+    guidance_mask=m or [m1, ..., mK] (classifier-free guidance only; not in the reference; None, the default, changes
+    nothing): regional guidance, one weight mask per condition of condition=c or [c1, ..., cK] (K = 1 to 4), for
+    regional prompting and MultiDiffusion-style region composition (Bar-Tal et al. 2023). Each entry is a tensor or None
+    (all ones). A mask broadcasts to x's shape [B, C, *spatial] by torch's rules -- [H, W], [1, 1, H, W], [B, 1, H, W],
+    [B, C, H, W], [B, 1, 1, 1] (one weight per sample and condition), ... -- so its batch extent is 1 or B; this is
+    checked against x at the first evaluation and rejected (ValueError) before any launch. Values are taken as given in
+    fp32 (bool is 0/1); nothing checks them on the device and nothing synchronises. The network runs on all K+1 blocks,
+    as with several conditions (masks skip no network work). Per element i, in the network's output space after the
+    parameterisation converts each block, in fp32 with each op rounded and no contraction:
+        eps = eps_u;  for k = 1..K:  w = fl32(s_k)*m_k(i);  eps = eps + w*(eps_k - eps_u)
+    then eps -> x0, the thresholding clamp and the update as with several conditions. No term is bypassed: a zero
+    weight still evaluates 0*(eps_k - eps_u) (NaN where that difference is infinite, as a zero scale does). Masks of
+    ones give w == s_k, so the run equals the unmasked multi-condition run bit for bit for K >= 2, and for K = 1 the
+    one-condition CFG run when s != 1 (at s == 1 that run bypasses; this one combines). With masks that sum to 1 at
+    every element and one shared scale s, the result is, in exact arithmetic, ordinary CFG with scale s applied to the
+    mask-weighted average of the conditional outputs: the recipe for "average the regions". A contiguous fp32 mask on
+    x's device that already has its weight map's layout ([H, W] or [B, 1, H, W] for a row-major x, [B, 1, 1, 1], or a
+    [B, C, H, W] mask laid out like x) is read in place, so a captured graph sees values written into it; other masks
+    are converted once per (tensor, version, x shape, x memory format). guidance_scale is s or [s1, ..., sK] (one
+    python float or one-element tensor per condition). Accepted: everything several conditions accept -- every model
+    type and schedule, both algorithms, singlestep, multistep, singlestep_fixed, adaptive (host or device controller),
+    dynamic thresholding, denoise_to_zero, inverse(), return_intermediate, capture() and batch sharding (each rank
+    passes the masks of its own rows); a direct call of this callable returns the masked combine. Not available
+    (ValueError): other guidance types, no unconditional_condition, a mask count other than K, an entry that is neither
+    a tensor nor None, a per-sample guidance_scale (use a [B, 1, 1, 1] mask), guidance_rescale != 0, apg_eta,
+    cfg_zero_star, cfg_pp, UniPC and DPM_Solver(reference_rounding=True)."""
     assert model_type in ["noise", "x_start", "v", "score", "flow", "edm"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
     flow_schedule = getattr(noise_schedule, "schedule", None) == "flow"
@@ -546,6 +637,10 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
             raise ValueError("cfg_pp is not available with adaptive projected guidance (apg_eta)")
         if cfg_zero_star:
             raise ValueError("cfg_pp is not available with cfg_zero_star")
+    if guidance_mask is not None:
+        condition, guidance_scale, guidance_mask = _masked_arguments(
+            guidance_type, condition, unconditional_condition, guidance_scale, guidance_mask, guidance_rescale,
+            apg_eta, cfg_zero_star, cfg_pp)
     if cfg_zero_star:
         if guidance_type != "classifier-free" or unconditional_condition is None:
             raise ValueError("cfg_zero_star needs guidance_type='classifier-free' and an unconditional_condition")
@@ -557,7 +652,40 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
             raise ValueError("cfg_zero_star is not available with adaptive projected guidance (apg_eta)")
     return WrappedModel(model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                         unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale,
-                        apg_eta, apg_norm_threshold, apg_momentum, cfg_zero_star, cfg_zero_init_steps, cfg_pp)
+                        apg_eta, apg_norm_threshold, apg_momentum, cfg_zero_star, cfg_zero_init_steps, cfg_pp,
+                        guidance_mask)
+
+
+def _masked_arguments(guidance_type, condition, unconditional_condition, guidance_scale, guidance_mask,
+                      guidance_rescale, apg_eta, cfg_zero_star, cfg_pp):
+    """model_wrapper's arguments of a run with guidance masks, validated: (K conditions, their scales, K masks)."""
+    if guidance_type != "classifier-free" or unconditional_condition is None:
+        raise ValueError("guidance_mask needs guidance_type='classifier-free' and an unconditional_condition")
+    many = isinstance(condition, (list, tuple))
+    conds = list(condition) if many else [condition]
+    masks = list(guidance_mask) if isinstance(guidance_mask, (list, tuple)) else [guidance_mask]
+    if len(masks) != len(conds):
+        raise ValueError("{} guidance masks for {} conditions".format(len(masks), len(conds)))
+    if any(m is not None and not torch.is_tensor(m) for m in masks):
+        raise ValueError("each guidance_mask entry must be a tensor or None")
+    s = guidance_scale
+    per_sample = (torch.is_tensor(s) and (s.dim() >= 2 or (not many and s.numel() != 1))) or \
+        (isinstance(s, (list, tuple)) and any(torch.is_tensor(v) and v.numel() != 1 for v in s))
+    if per_sample:
+        raise ValueError("a per-sample guidance_scale is not available with guidance_mask; use a [B, 1, 1, 1] mask")
+    if guidance_rescale != 0:
+        raise ValueError("guidance_rescale is not available with guidance_mask")
+    if apg_eta is not None:
+        raise ValueError("adaptive projected guidance (apg_eta) is not available with guidance_mask")
+    if cfg_zero_star:
+        raise ValueError("cfg_zero_star is not available with guidance_mask")
+    if cfg_pp:
+        raise ValueError("cfg_pp is not available with guidance_mask")
+    if not many:
+        s = [float(s)] if torch.is_tensor(s) else [s]
+    elif isinstance(s, (list, tuple)):
+        s = [float(v) if torch.is_tensor(v) else v for v in s]
+    return conds, s, masks
 
 
 # =================================================================================================
@@ -631,6 +759,8 @@ class DPM_Solver:
             raise ValueError("a per-sample guidance_scale is not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "n_cond", 0) >= 2:
             raise ValueError("several conditions are not available with reference_rounding=True")
+        if self.reference_rounding and getattr(model_fn, "cond_masks", None) is not None:
+            raise ValueError("guidance_mask is not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "apg", None) is not None:
             raise ValueError("adaptive projected guidance is not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "cfg_zero_star", False):

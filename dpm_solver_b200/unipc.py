@@ -62,8 +62,8 @@ materialises the guided raw output g in fp32, then the UniPC launch converting g
 state. Zero-init evaluations (cfg_zero_init_steps) are one-output launches on a raw output of 0, counted as in
 DPM_Solver.
 
-Not available (ValueError before any launch): per-sample guidance scales, several conditions, guidance rescale,
-reference_rounding, plan_broadcast, orders outside 1..3, steps < order.
+Not available (ValueError before any launch): per-sample guidance scales, several conditions, guidance masks,
+guidance rescale, reference_rounding, plan_broadcast, orders outside 1..3, steps < order.
 """
 from __future__ import annotations
 
@@ -124,6 +124,8 @@ class UniPC(DPM_Solver):
                 raise ValueError("a per-sample guidance_scale is not available with UniPC")
             if w.n_cond >= 2:
                 raise ValueError("several conditions are not available with UniPC")
+            if w.cond_masks is not None:
+                raise ValueError("guidance_mask is not available with UniPC")
             if w.guidance_type == "classifier-free" and w.guidance_rescale != 0:
                 raise ValueError("guidance_rescale is not available with UniPC")
             if w.cfg_pp:

@@ -28,7 +28,8 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 108 /* 0.1.8: CFG++ (dpm_step_cfgpp) */
+#define DPM_B200_VERSION 108 /* 0.1.8: CFG++ (dpm_step_cfgpp); regional guidance (dpm_step_multi_masked) is an
+                                addition to this ABI: test for its symbol */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -122,7 +123,7 @@ typedef struct dpm_step_desc {
    * or NULL. clamp(x0,-s,s)/s, dynamic_thresholding_fn :423-424 */
   const float* thr;
   uint64_t n;          /* total elements                                                   */
-  uint64_t per_sample; /* elements per sample (C*H*W); only read when thr != NULL           */
+  uint64_t per_sample; /* elements per sample (C*H*W); read when thr != NULL, and by the masked step */
   int32_t state_dtype; /* dpm_dtype of x, xe, m*, m_out, out                               */
   int32_t model_dtype; /* dpm_dtype of e_cond, e_uncond                                    */
   int32_t form;        /* dpm_form                                                         */
@@ -410,6 +411,28 @@ DPM_API int dpm_step_cfgpp(const dpm_step_desc* desc, float g, const float* guid
 DPM_API int dpm_step_multi(const dpm_step_desc* desc, const void* const* e_conds, const float* scales, int n_cond,
                            void* const* replicas, dpm_stream_t stream);
 DPM_API int dpm_replicate(void* out, const void* x, uint64_t n, int copies, int dtype, dpm_stream_t stream);
+
+/* ---- regional classifier-free guidance: a weight map per condition (MultiDiffusion-style region composition) -----
+ * dpm_step_multi_masked: dpm_step_multi with the scale of condition k multiplied, per element, by a weight map:
+ *   eps = eps_u;  w = scales[k]*m_k(i);  eps = eps + w*(eps_k - eps_u),  k = 0 .. n_cond-1   (each op rounded to fp32,
+ *                                                                                               none skipped)
+ * The weight of global element i (storage order) is maps[k].w[b*sample_stride + (r % period)], b = i / per_sample,
+ * r = i - b*per_sample. maps[k].w == NULL means all ones (then w == scales[k] exactly, and the launch computes what
+ * dpm_step_multi computes). Three periods are meant: 1 (one weight per sample), the spatial size S of an
+ * NCHW-contiguous x (per_sample == C*S: a pixel map shared by the channels), and per_sample (a full element map in x's
+ * storage order); sample_stride is 0 (one map shared by the batch) or period. maps: HOST array of n_cond entries; the
+ * weights are fp32 in device memory, read at launch time (a captured graph sees values written into them).
+ * Needs 1 <= n_cond <= DPM_MAX_CONDITIONS, desc->per_sample != 0 dividing n, and period != 0 dividing per_sample;
+ * otherwise as dpm_step_multi (DPM_ERR_ARG before any launch). The packet kernels serve the five dtype pairs when
+ * samples hold whole packets and every map has period 1, or period % 8 == 0 with 16-byte-aligned weights; tails,
+ * unaligned views, other maps and pairs and dev_coef launches run on the generic kernel. */
+typedef struct dpm_cond_map {
+  const float* w;
+  uint64_t period;
+  uint64_t sample_stride;
+} dpm_cond_map;
+DPM_API int dpm_step_multi_masked(const dpm_step_desc* desc, const void* const* e_conds, const float* scales,
+                                  const dpm_cond_map* maps, int n_cond, void* const* replicas, dpm_stream_t stream);
 
 /* ---- UniPC multistep (Zhao et al. 2023, "UniPC: A Unified Predictor-Corrector Framework", arXiv:2302.04867) ------
  * One launch per network evaluation i: the corrector of step i and the predictor of step i+1 (dpm_solver_b200/unipc.py
