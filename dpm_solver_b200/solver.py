@@ -918,9 +918,10 @@ class DPM_Solver:
 
     def _device_tables(self, key, t_host, batch, device, n_eval=None):
         """Device copies of the time grid and of the model-input time matrix, cached with the plan
-        (they depend on the batch size and the device only)."""
+        (they depend on the batch size, the network's input rows and the device only)."""
         cache = self.__dict__.setdefault("_table_cache", {})
-        k = (self._schedule_key(), self.algorithm_type) + key + (batch, str(device), id(self._wrapped))
+        k = (self._schedule_key(), self.algorithm_type) + key + (batch, self._input_rows(batch), str(device),
+                                                                 id(self._wrapped))
         hit = cache.get(k)
         if hit is None:
             t_dev = self._upload(t_host, device)
@@ -938,7 +939,7 @@ class DPM_Solver:
     def _denoise_tables(self, t_0, batch, device):
         """(device label (1,), model-input time row or None, (alpha, sigma)) of the denoise-to-zero tail."""
         cache = self.__dict__.setdefault("_table_cache", {})
-        k = (self._schedule_key(), "d2z", float(t_0), batch, str(device), id(self._wrapped))
+        k = (self._schedule_key(), "d2z", float(t_0), batch, self._input_rows(batch), str(device), id(self._wrapped))
         hit = cache.get(k)
         if hit is None:
             th = torch.ones((1,)) * t_0                                   # fp32, as `torch.ones((1,)).to(device) * t_0`
@@ -948,6 +949,13 @@ class DPM_Solver:
                 cache.pop(next(iter(cache)))
             cache[k] = hit
         return hit
+
+    def _input_rows(self, batch: int) -> int:
+        """Rows of the network input for a batch: 2B under CFG, B when a one-element scale tensor now holds 1 and the
+        halves are bypassed. It can change between runs of one solver (the tensor edited in place, or the wrapper's
+        settings changed), so the model-input time tables are keyed by it."""
+        w = self._wrapped
+        return w.input_rows(batch) if isinstance(w, WrappedModel) and w.fusable else batch
 
     @staticmethod
     def _upload(t_host: torch.Tensor, device):

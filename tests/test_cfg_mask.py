@@ -70,11 +70,12 @@ def product_fn(model_type, K, scales, masks, net=None, batch=B):
                              guidance_scale=scales, guidance_mask=masks), pns
 
 
-def reference_composed(model_type, K, scales, masks, batch=B):
-    """model_fn(x, t_continuous) of the reference composition: w_k = fl32(s_k)*m_k, then eps_u + w_k*(eps_k - eps_u)."""
-    ref, rns, _ = schedules("sd")
+def reference_composed(model_type, K, scales, masks, batch=B, net=None, sched="sd"):
+    """model_fn(x, t_continuous) of the reference composition: w_k = fl32(s_k)*m_k, then eps_u + w_k*(eps_k - eps_u).
+    `net(x, t, c)` (default inner_net) on the VP schedule `sched` of tests/golden/cases.make_betas."""
+    ref, rns, _ = schedules(sched)
     uc = torch.zeros(batch, 1)
-    fs = [ref.model_wrapper(inner_net(), rns, model_type=model_type, guidance_type="classifier-free", condition=c,
+    fs = [ref.model_wrapper(net or inner_net(), rns, model_type=model_type, guidance_type="classifier-free", condition=c,
                             unconditional_condition=uc, guidance_scale=1.0) for c in [uc] + conds(K, batch)]
     ws = [torch.tensor(s, dtype=torch.float32) * (torch.ones(()) if m is None else m.float())
           for s, m in zip(scales, masks)]
