@@ -113,6 +113,9 @@ PROTOTYPES = {
     "dpm_cfgzero_scale": (C.c_int, [_vp, _vp, _vp, _i, _u64, _u64, _vp, C.c_size_t, _vp]),
     "dpm_step_cfgzero": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _vp]),
     "dpm_step_cfgpp": (C.c_int, [C.POINTER(StepDesc), _f, _vp, _vp]),
+    "dpm_tcfg_workspace": (C.c_size_t, [_u64, _u64]),
+    "dpm_tcfg_words": (C.c_int, [_vp, _vp, _vp, _i, _u64, _u64, _vp, C.c_size_t, _vp]),
+    "dpm_step_tcfg": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _vp]),
 }
 
 MAX_CONDITIONS = 4      # DPM_MAX_CONDITIONS

@@ -187,20 +187,25 @@ int launch_apg_words(float* words, const KParams& kp, const float* gscale, float
 // s*_b = fl32(<c_b, u_b> / (||u_b||^2 + 1e-8)) over the two raw network halves of sample b, fp64 sums of the widened
 // outputs. The chunking, thread ownership and summation order of k_apg_partial / k_apg_final, with two sums of raw
 // values in place of three of converted ones: no x, no marginals, no dev_coef. Algorithmic bytes: 2*s_model per element.
+// ---- TCFG (dpm_tcfg_words; "TCFG: Tangential Damping Classifier-free Guidance", CVPR 2025) -------------------------
+// The same pass with three sums, A = ||u||^2, B = <u, c>, C = ||c||^2, and k_tcfg_final in place of k_cfgzero_final:
+// the words (wu, wc) of u' = wu*u + wc*c, the projection of u on the first right singular vector of [u; c].
 struct ZParams {
   const void* ec;
   const void* eu;
-  double* partial;       // [n_samples * chunks][2]: <c, u>, ||u||^2
-  float* s_out;          // [n_samples]
+  double* partial;       // [n_samples * chunks][NS]: <c, u>, ||u||^2 (CFG-Zero*) or ||u||^2, <u, c>, ||c||^2 (TCFG)
+  float* s_out;          // [n_samples] s* (CFG-Zero*) or [n_samples][2] (wu, wc) (TCFG)
   uint64_t per_sample;
   uint64_t n_samples;
   uint32_t chunks;
   int32_t model_dtype;
 };
 
-// VEC: per_sample % 8 == 0 and both halves aligned, TE their type. Otherwise element-wise (load_any).
-template <typename TE, bool VEC>
+// VEC: per_sample % 8 == 0 and both halves aligned, TE their type. Otherwise element-wise (load_any). NS: the number of
+// sums, 2 (CFG-Zero*) or 3 (TCFG).
+template <typename TE, bool VEC, int NS>
 __global__ void __launch_bounds__(kAThreads) k_cfgzero_partial(const __grid_constant__ ZParams p) {
+  static_assert(NS == 2 || NS == 3, "two or three sums");
   __shared__ double warp_part[kAThreads / 32];
   const uint64_t sample = blockIdx.x / p.chunks;
   const uint32_t chunk = blockIdx.x % p.chunks;
@@ -210,10 +215,16 @@ __global__ void __launch_bounds__(kAThreads) k_cfgzero_partial(const __grid_cons
   const size_t e0 = sample * p.per_sample + c_begin;
   const int tid = threadIdx.x;
   constexpr int U = kAChunk / kPacket / kAThreads;   // 4
-  double scu = 0.0, suu = 0.0;
+  double s0 = 0.0, s1 = 0.0, s2 = 0.0;   // <c, u>, ||u||^2 (NS == 2); ||u||^2, <u, c>, ||c||^2 (NS == 3)
   auto term = [&](float c, float u) {
-    scu += (double)c * (double)u;
-    suu += (double)u * (double)u;
+    if constexpr (NS == 2) {
+      s0 += (double)c * (double)u;
+      s1 += (double)u * (double)u;
+    } else {
+      s0 += (double)u * (double)u;
+      s1 += (double)u * (double)c;
+      s2 += (double)c * (double)c;
+    }
   };
   // element (u, i) of this thread is chunk element (u*kAThreads + tid)*8 + i on both paths, as in k_apg_partial
 #pragma unroll
@@ -239,11 +250,13 @@ __global__ void __launch_bounds__(kAThreads) k_cfgzero_partial(const __grid_cons
       }
     }
   }
-  scu = apg_cta_sum(scu, warp_part);
-  suu = apg_cta_sum(suu, warp_part);
+  s0 = apg_cta_sum(s0, warp_part);
+  s1 = apg_cta_sum(s1, warp_part);
+  if constexpr (NS == 3) s2 = apg_cta_sum(s2, warp_part);
   if (tid == 0) {
-    double* o = p.partial + (size_t)blockIdx.x * 2;
-    o[0] = scu; o[1] = suu;
+    double* o = p.partial + (size_t)blockIdx.x * NS;
+    o[0] = s0; o[1] = s1;
+    if constexpr (NS == 3) o[2] = s2;
   }
 }
 
@@ -259,41 +272,93 @@ __global__ void __launch_bounds__(kAThreads) k_cfgzero_final(const __grid_consta
   p.s_out[b] = (float)(scu / (suu + 1e-8));   // diffusers' cfg_zero_star_scale epsilon
 }
 
-size_t cfgzero_workspace_bytes(uint64_t n_samples, uint64_t per_sample) {
-  if (per_sample == 0 || n_samples == 0) return 0;
-  const uint64_t chunks = (per_sample + kAChunk - 1) / kAChunk;
-  return (size_t)(n_samples * chunks) * 2 * sizeof(double);
+// The words of sample b from its merged sums, in fp64 with each op rounded. (p, q) is the top eigenvector of the Gram
+// matrix [[A, B], [B, C]], taken from the row without cancellation (h <= 0: row 1, else row 2); with the eigen identity
+// the projection <u, v1>*v1 is (p*p*u + p*q*c)/(p*p + q*q). n2 == 0 (A == C and B == 0: no unique top direction, both
+// outputs zero included) gives (1, 0), plain CFG; a sum that is not finite gives NaN words.
+__global__ void __launch_bounds__(kAThreads) k_tcfg_final(const __grid_constant__ ZParams p) {
+  const uint64_t b = (uint64_t)blockIdx.x * kAThreads + threadIdx.x;
+  if (b >= p.n_samples) return;
+  const double* part = p.partial + b * p.chunks * 3;
+  double A = 0.0, B = 0.0, C = 0.0;
+  for (uint32_t c = 0; c < p.chunks; ++c) {
+    A += part[c * 3];
+    B += part[c * 3 + 1];
+    C += part[c * 3 + 2];
+  }
+  float wu, wc;
+  if (!(isfinite(A) && isfinite(B) && isfinite(C))) {
+    wu = wc = __int_as_float(0x7fffffff);
+  } else {
+    const double h = 0.5 * (A - C);
+    const double r = sqrt(h * h + B * B);
+    double pv, qv;
+    if (C >= A) { pv = B; qv = (-h) + r; }
+    else        { pv = h + r; qv = B; }
+    const double pp = pv * pv;
+    const double n2 = pp + qv * qv;
+    if (n2 == 0.0) { wu = 1.f; wc = 0.f; }
+    else { wu = (float)(pp / n2); wc = (float)((pv * qv) / n2); }
+  }
+  p.s_out[2 * b] = wu;
+  p.s_out[2 * b + 1] = wc;
 }
 
-int launch_cfgzero_scale(float* s_out, const void* ec, const void* eu, int model_dtype, uint64_t per_sample,
-                         uint64_t n, void* ws, size_t ws_bytes, cudaStream_t stream) {
+static size_t zpass_workspace_bytes(uint64_t n_samples, uint64_t per_sample, int ns) {
+  if (per_sample == 0 || n_samples == 0) return 0;
+  const uint64_t chunks = (per_sample + kAChunk - 1) / kAChunk;
+  return (size_t)(n_samples * chunks) * ns * sizeof(double);
+}
+size_t cfgzero_workspace_bytes(uint64_t n_samples, uint64_t per_sample) {
+  return zpass_workspace_bytes(n_samples, per_sample, 2);
+}
+size_t tcfg_workspace_bytes(uint64_t n_samples, uint64_t per_sample) {
+  return zpass_workspace_bytes(n_samples, per_sample, 3);
+}
+
+// the sums pass over both halves, then `final` per sample: two launches, no allocation, no sync
+template <int NS>
+static int launch_zpass(void (*final)(const ZParams), const char* what, float* s_out, const void* ec, const void* eu,
+                        int model_dtype, uint64_t per_sample, uint64_t n, void* ws, size_t ws_bytes,
+                        cudaStream_t stream) {
   ZParams p;
   memset(&p, 0, sizeof(p));
   p.ec = ec; p.eu = eu; p.s_out = s_out; p.model_dtype = model_dtype;
   p.per_sample = per_sample; p.n_samples = n / per_sample;
   p.chunks = (uint32_t)((per_sample + kAChunk - 1) / kAChunk);
   p.partial = static_cast<double*>(ws);
-  if (ws == nullptr || ws_bytes < cfgzero_workspace_bytes(p.n_samples, per_sample) ||
+  if (ws == nullptr || ws_bytes < zpass_workspace_bytes(p.n_samples, per_sample, NS) ||
       (reinterpret_cast<uintptr_t>(ws) & 7)) {
-    set_error("cfg-zero* scale: workspace too small or not 8-byte aligned");
+    set_error("%s: workspace too small or not 8-byte aligned", what);
     return DPM_ERR_ARG;
   }
-  if (p.n_samples * p.chunks > 0x7fffffffull) { set_error("cfg-zero* scale: too many chunks"); return DPM_ERR_UNSUPPORTED; }
+  if (p.n_samples * p.chunks > 0x7fffffffull) { set_error("%s: too many chunks", what); return DPM_ERR_UNSUPPORTED; }
   const uintptr_t am = model_dtype == DPM_F32 ? 31 : 15;
   const bool vec = per_sample % kPacket == 0 && (reinterpret_cast<uintptr_t>(ec) & am) == 0 &&
                    (reinterpret_cast<uintptr_t>(eu) & am) == 0;
   typedef void (*ZKernel)(const ZParams);
-  ZKernel k = k_cfgzero_partial<float, false>;   // any dtype, alignment or sample size
+  ZKernel k = k_cfgzero_partial<float, false, NS>;   // any dtype, alignment or sample size
   if (vec) {
-    if (model_dtype == DPM_F32) k = k_cfgzero_partial<float, true>;
-    else if (model_dtype == DPM_BF16) k = k_cfgzero_partial<__nv_bfloat16, true>;
-    else if (model_dtype == DPM_F16) k = k_cfgzero_partial<__half, true>;
+    if (model_dtype == DPM_F32) k = k_cfgzero_partial<float, true, NS>;
+    else if (model_dtype == DPM_BF16) k = k_cfgzero_partial<__nv_bfloat16, true, NS>;
+    else if (model_dtype == DPM_F16) k = k_cfgzero_partial<__half, true, NS>;
   }
   k<<<(unsigned)(p.n_samples * p.chunks), kAThreads, 0, stream>>>(p);
-  k_cfgzero_final<<<(unsigned)((p.n_samples + kAThreads - 1) / kAThreads), kAThreads, 0, stream>>>(p);
+  final<<<(unsigned)((p.n_samples + kAThreads - 1) / kAThreads), kAThreads, 0, stream>>>(p);
   count_launch();
   count_launch();
   return DPM_OK;
+}
+
+int launch_cfgzero_scale(float* s_out, const void* ec, const void* eu, int model_dtype, uint64_t per_sample,
+                         uint64_t n, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  return launch_zpass<2>(k_cfgzero_final, "cfg-zero* scale", s_out, ec, eu, model_dtype, per_sample, n, ws, ws_bytes,
+                         stream);
+}
+
+int launch_tcfg_words(float* w_out, const void* ec, const void* eu, int model_dtype, uint64_t per_sample, uint64_t n,
+                      void* ws, size_t ws_bytes, cudaStream_t stream) {
+  return launch_zpass<3>(k_tcfg_final, "tcfg words", w_out, ec, eu, model_dtype, per_sample, n, ws, ws_bytes, stream);
 }
 
 }  // namespace dpm

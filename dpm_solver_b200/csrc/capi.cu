@@ -232,8 +232,10 @@ struct Apg {
 
 // gscale (optional): per-sample guidance of an n_model == 2 step, fp32 [n/per_sample]; rs then may be NULL
 // zs (optional): the CFG-Zero* scales s* of an n_model == 2 step, fp32 [n/per_sample]; gscale then may be NULL
+// td (optional): the TCFG words (wu, wc) of an n_model == 2 step, fp32 [n/per_sample][2]; likewise
 static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale* rs = nullptr,
-                     const float* gscale = nullptr, const Apg* apg = nullptr, const float* zs = nullptr) {
+                     const float* gscale = nullptr, const Apg* apg = nullptr, const float* zs = nullptr,
+                     const float* td = nullptr) {
   KParams p;
   Needs nd;
   if (d != nullptr && d->n == 0) return DPM_OK;  // empty tensors: nothing to do (pointers may be NULL)
@@ -262,6 +264,7 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale*
   }
   p.gscale = gscale;
   p.zs = zs;
+  p.td = td;
   Tuning t{g_variant.load(), g_threads.load(), g_ctas.load()};
 
   bool body_done = false;
@@ -275,6 +278,7 @@ static int step_impl(const dpm_step_desc* d, cudaStream_t stream, const Rescale*
                      p.gscale == nullptr &&  // per-sample guidance: the direct variant's <PG> kernels
                      p.apg_a == nullptr &&   // adaptive projected guidance: the direct variant's <APG> kernels
                      p.zs == nullptr &&      // CFG-Zero*: the direct variant's <PG> kernels
+                     p.td == nullptr &&      // TCFG: likewise
                      t.variant == 1;
     if (tma) r = launch_step_tma(p, t, stream);
     if (r == 1) r = launch_step_direct(p, t, stream);
@@ -642,6 +646,32 @@ int dpm_step_cfgzero(const dpm_step_desc* desc, const float* s_star, const float
     return DPM_ERR_ARG;
   }
   return step_impl(desc, static_cast<cudaStream_t>(stream), nullptr, guidance, nullptr, s_star);
+}
+
+size_t dpm_tcfg_workspace(uint64_t n_samples, uint64_t per_sample) {
+  return tcfg_workspace_bytes(n_samples, per_sample);
+}
+
+int dpm_tcfg_words(float* w_out, const void* e_cond, const void* e_uncond, int model_dtype, uint64_t per_sample,
+                   uint64_t n, void* workspace, size_t workspace_bytes, dpm_stream_t stream) {
+  if (n == 0) return DPM_OK;
+  if (!w_out || !e_cond || !e_uncond) { set_error("tcfg words: NULL tensor"); return DPM_ERR_ARG; }
+  if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) {
+    set_error("tcfg words: bad dtype or sizes");
+    return DPM_ERR_ARG;
+  }
+  return finish(launch_tcfg_words(w_out, e_cond, e_uncond, model_dtype, per_sample, n, workspace, workspace_bytes,
+                                  static_cast<cudaStream_t>(stream)));
+}
+
+int dpm_step_tcfg(const dpm_step_desc* desc, const float* words, const float* guidance, dpm_stream_t stream) {
+  if (desc != nullptr && desc->n == 0) return DPM_OK;
+  if (desc == nullptr || words == nullptr || desc->n_model != 2 || desc->raw_round != 0 || desc->per_sample == 0 ||
+      desc->n % desc->per_sample) {
+    set_error("tcfg step: needs words, n_model == 2, raw_round == 0 and per_sample dividing n");
+    return DPM_ERR_ARG;
+  }
+  return step_impl(desc, static_cast<cudaStream_t>(stream), nullptr, guidance, nullptr, nullptr, words);
 }
 
 int dpm_step_cfgpp(const dpm_step_desc* desc, float g, const float* guidance, dpm_stream_t stream) {

@@ -79,6 +79,10 @@ struct KParams {
   // the <PG = true> instantiations read it (kind kPgZeroStar); `gscale` may then be NULL (every sample's scale is
   // `guidance`).
   const float* zs;
+  // TCFG (dpm_step_tcfg): the per-sample words (wu_b, wc_b) of dpm_tcfg_words, fp32 [n/per_sample][2]. Only the
+  // <PG = true> instantiations read it (kind kPgTangential); `gscale` may then be NULL (every sample's scale is
+  // `guidance`).
+  const float* td;
 };
 
 // multi-condition classifier-free guidance (dpm_step_multi): eps = eps_u; eps = eps + s[k]*(eps_k - eps_u) for k < n_cond,
@@ -378,24 +382,36 @@ __device__ __forceinline__ float rescale_value(const KParams& p, float g, float 
 //   kPgCombine otherwise: the combine of the plain path
 //   kPgZeroStar p.zs set: CFG-Zero* (Fan et al. 2025) in the network's output space with r = s*_b of the sample:
 //              us = eu*s*, g = us + gs*(ec - us), each op rounded, then the parameterisation converts g
-enum { kPgAny = 1, kPgBypass = 2, kPgRescale = 3, kPgCombine = 4, kPgZeroStar = 5 };
+//   kPgTangential p.td set: TCFG (tangential damping, CVPR 2025) in the network's output space with r, r2 = the
+//              words wu_b, wc_b of the sample: us = eu*wu + ec*wc, g = us + gs*(ec - us), each op rounded, then the
+//              parameterisation converts g
+// Precedence: the bypass, then zs, td, ratio, the plain combine.
+enum { kPgAny = 1, kPgBypass = 2, kPgRescale = 3, kPgCombine = 4, kPgZeroStar = 5, kPgTangential = 6 };
 __host__ __device__ __forceinline__ int pg_kind(const KParams& p, float gs) {
-  return gs == 1.f ? kPgBypass : (p.zs != nullptr ? kPgZeroStar : (p.ratio != nullptr ? kPgRescale : kPgCombine));
+  if (gs == 1.f) return kPgBypass;
+  if (p.zs != nullptr) return kPgZeroStar;
+  if (p.td != nullptr) return kPgTangential;
+  return p.ratio != nullptr ? kPgRescale : kPgCombine;
 }
 template <int K>
-__device__ __forceinline__ float guided_value(const KParams& p, float xe, float ec, float eu, float r, float gs) {
+__device__ __forceinline__ float guided_value(const KParams& p, float xe, float ec, float eu, float r, float gs,
+                                              float r2) {
   if constexpr (K == kPgAny) {
     const int k = pg_kind(p, gs);
-    if (k == kPgBypass) return guided_value<kPgBypass>(p, xe, ec, eu, r, gs);
-    if (k == kPgRescale) return guided_value<kPgRescale>(p, xe, ec, eu, r, gs);
-    if (k == kPgZeroStar) return guided_value<kPgZeroStar>(p, xe, ec, eu, r, gs);
-    return guided_value<kPgCombine>(p, xe, ec, eu, r, gs);
+    if (k == kPgBypass) return guided_value<kPgBypass>(p, xe, ec, eu, r, gs, r2);
+    if (k == kPgRescale) return guided_value<kPgRescale>(p, xe, ec, eu, r, gs, r2);
+    if (k == kPgZeroStar) return guided_value<kPgZeroStar>(p, xe, ec, eu, r, gs, r2);
+    if (k == kPgTangential) return guided_value<kPgTangential>(p, xe, ec, eu, r, gs, r2);
+    return guided_value<kPgCombine>(p, xe, ec, eu, r, gs, r2);
   } else if constexpr (K == kPgBypass) {
     return convert_param(p, ec, xe);
   } else if constexpr (K == kPgRescale) {
     return convert_param(p, rescale_value(p, eu + gs * (ec - eu), r), xe);
   } else if constexpr (K == kPgZeroStar) {
     const float us = eu * r;
+    return convert_param(p, us + gs * (ec - us), xe);
+  } else if constexpr (K == kPgTangential) {
+    const float us = eu * r + ec * r2;
     return convert_param(p, us + gs * (ec - us), xe);
   } else {
     const float epc = convert_param(p, ec, xe);
@@ -406,13 +422,14 @@ __device__ __forceinline__ float guided_value(const KParams& p, float xe, float 
 
 // RS: guidance rescale (NE == 2). The combine then runs on the raw outputs, the rescale follows, and the
 // parameterisation converts the rescaled prediction -- the order of a rescaling network wrapped by :288-298.
-// PG: per-sample guidance (NE == 2, guided_value<PG>) with the sample's scale gs; 0 = off, else the kind.
+// PG: per-sample guidance (NE == 2, guided_value<PG>) with the sample's scale gs; 0 = off, else the kind. r2: the
+// second word of the sample (kPgTangential).
 template <int NE, bool RND = false, bool RS = false, int PG = 0>
 __device__ __forceinline__ float model_value(const KParams& p, float xe, float ec, float eu,
-                                             float thr, bool clamp, float r = 1.f, float gs = 1.f) {
+                                             float thr, bool clamp, float r = 1.f, float gs = 1.f, float r2 = 0.f) {
   float eps;
   if constexpr (PG != 0) {
-    eps = guided_value<PG>(p, xe, ec, eu, r, gs);
+    eps = guided_value<PG>(p, xe, ec, eu, r, gs, r2);
   } else if (RS) {
     eps = convert_param(p, rescale_value(p, eu + p.guidance * (ec - eu), r), xe);
   } else {

@@ -141,5 +141,8 @@ int launch_apg_words(float* words, const KParams& kp, const float* gscale, float
 size_t cfgzero_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
 int launch_cfgzero_scale(float* s_out, const void* ec, const void* eu, int model_dtype, uint64_t per_sample,
                          uint64_t n, void* ws, size_t ws_bytes, cudaStream_t stream);
+size_t tcfg_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
+int launch_tcfg_words(float* w_out, const void* ec, const void* eu, int model_dtype, uint64_t per_sample, uint64_t n,
+                      void* ws, size_t ws_bytes, cudaStream_t stream);
 
 }  // namespace dpm

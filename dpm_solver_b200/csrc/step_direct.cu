@@ -21,7 +21,8 @@ constexpr int kMaxThreads = 512;
 // like the per-sample thresholds.
 // PG (only with NE == 2, RND = false and RS = false): per-sample guidance (dpm_step_guided) with the scale p.gscale
 // and, when p.ratio is set, the rescale -- one kernel family for rescale on and off. With FAST = false it also serves
-// CFG-Zero* (dpm_step_cfgzero: p.zs set, p.gscale NULL for one scale p.guidance).
+// CFG-Zero* (dpm_step_cfgzero: p.zs set, p.gscale NULL for one scale p.guidance) and TCFG (dpm_step_tcfg: p.td set,
+// likewise).
 // APG (only with NE == 2, FAST = false and no other option; the kernel k_step_direct_apg): adaptive projected guidance
 // (dpm_step_apg) with the per-sample words p.apg_a / p.apg_b; reads the fp32 direction p.apg_r in place of e_uncond
 // when it is set.
@@ -145,17 +146,19 @@ __device__ __forceinline__ void step_direct_body(const KParams& p) {
             const float rpk = p.zs != nullptr ? __ldg(p.zs + b) : (p.ratio != nullptr ? __ldg(p.ratio + b) : 1.f);
             const float tpk = clamp ? __ldg(p.thr + b) : 1.f;
             // the kind of the combine is uniform per packet: one branch per packet, straight-line code per element
-            auto guided8 = [&](auto kind) {
+            auto guided8 = [&](auto kind, float r, float r2) {
 #pragma unroll
               for (int i = 0; i < 8; ++i)
                 fT[i] = model_value<NE, false, false, decltype(kind)::value>(p, fxe[i], fec[i], feu[i], tpk, clamp,
-                                                                             rpk, gpk);
+                                                                             r, gpk, r2);
             };
             const int kind = pg_kind(p, gpk);
-            if (kind == kPgBypass) guided8(std::integral_constant<int, kPgBypass>{});
-            else if (kind == kPgRescale) guided8(std::integral_constant<int, kPgRescale>{});
-            else if (kind == kPgZeroStar) guided8(std::integral_constant<int, kPgZeroStar>{});
-            else guided8(std::integral_constant<int, kPgCombine>{});
+            if (kind == kPgBypass) guided8(std::integral_constant<int, kPgBypass>{}, rpk, 0.f);
+            else if (kind == kPgRescale) guided8(std::integral_constant<int, kPgRescale>{}, rpk, 0.f);
+            else if (kind == kPgZeroStar) guided8(std::integral_constant<int, kPgZeroStar>{}, rpk, 0.f);
+            else if (kind == kPgTangential)   // TCFG's two words, loaded where they are used
+              guided8(std::integral_constant<int, kPgTangential>{}, __ldg(p.td + 2 * b), __ldg(p.td + 2 * b + 1));
+            else guided8(std::integral_constant<int, kPgCombine>{}, rpk, 0.f);
           } else {
             float thr8[8];
             const bool thr_uniform = p.pk_per_sample != 0;
@@ -227,7 +230,8 @@ __global__ void __launch_bounds__(kMaxThreads) k_step_direct_apg(const __grid_co
 // RND = true: reference-rounding mode (common.cuh) for the launches the <RND> vector kernels do not serve:
 // unaligned views, tails and fp32 network outputs.
 // RS = true: guidance rescale (n_model == 2) for unaligned views, tails and dev_coef launches.
-// PG = true: per-sample guidance (n_model == 2; rescale iff p.ratio is set) and CFG-Zero* (p.zs set), likewise.
+// PG = true: per-sample guidance (n_model == 2; rescale iff p.ratio is set), CFG-Zero* (p.zs set) and TCFG (p.td set),
+// likewise.
 // APG = true (the kernel k_step_scalar_apg): adaptive projected guidance (n_model == 2), likewise.
 template <bool RND, bool RS, bool PG, bool APG>
 __device__ __forceinline__ void step_scalar_body(const KParams& pc) {
@@ -265,9 +269,11 @@ __device__ __forceinline__ void step_scalar_body(const KParams& pc) {
                        clamp);
       } else if constexpr (PG) {
         const uint64_t b = (i + p.elem_offset) / p.per_sample;
-        const float r = p.zs != nullptr ? p.zs[b] : (p.ratio != nullptr ? p.ratio[b] : 1.f);
+        const float r = p.zs != nullptr ? p.zs[b]
+                        : (p.td != nullptr ? p.td[2 * b] : (p.ratio != nullptr ? p.ratio[b] : 1.f));
         mv = model_value<2, false, false, kPgAny>(p, xe, ec, eu, thr, clamp, r,
-                                                  p.gscale != nullptr ? p.gscale[b] : p.guidance);
+                                                  p.gscale != nullptr ? p.gscale[b] : p.guidance,
+                                                  p.td != nullptr ? p.td[2 * b + 1] : 0.f);
       } else if (RS) {
         mv = model_value<2, false, true>(p, xe, ec, eu, thr, clamp, p.ratio[(i + p.elem_offset) / p.per_sample]);
       } else {
@@ -312,9 +318,9 @@ typedef void (*StepKernel)(const KParams);
 // PG: per-sample guidance, NE == 2 only; serves rescaled and plain launches alike (so it is tested before RS).
 // APG: adaptive projected guidance, NE == 2 only, on the IEEE-division instantiations (tested first: it carries gscale
 // for its bypass).
-// CFG-Zero* (p.zs): the <PG> instantiations with FAST = false, with or without per-sample scales.
+// CFG-Zero* (p.zs) and TCFG (p.td): the <PG> instantiations with FAST = false, with or without per-sample scales.
 static StepKernel pick_direct(const KParams& p) {
-  const bool zs = p.zs != nullptr;
+  const bool zs = p.zs != nullptr || p.td != nullptr;
   const bool fast = fast_path_ok(p) && !zs, rnd = p.raw_round != 0, rs = p.ratio != nullptr;
   const bool pg = p.gscale != nullptr || zs;
   const bool apg = p.apg_a != nullptr;
@@ -382,7 +388,7 @@ int launch_step_scalar(const KParams& p, cudaStream_t stream) {
   uint32_t grid = (uint32_t)(blocks < cap ? blocks : cap);
   if (p.raw_round) k_step_scalar<true><<<grid, threads, 0, stream>>>(p);
   else if (p.apg_a) k_step_scalar_apg<<<grid, threads, 0, stream>>>(p);
-  else if (p.gscale || p.zs) k_step_scalar<false, false, true><<<grid, threads, 0, stream>>>(p);
+  else if (p.gscale || p.zs || p.td) k_step_scalar<false, false, true><<<grid, threads, 0, stream>>>(p);
   else if (p.ratio) k_step_scalar<false, true><<<grid, threads, 0, stream>>>(p);
   else k_step_scalar<false><<<grid, threads, 0, stream>>>(p);
   count_launch();

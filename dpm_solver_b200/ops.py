@@ -92,6 +92,9 @@ class StepArgs:
     # CFG-Zero* (dpm_step_cfgzero; n_model == 2, per_sample set): the per-sample scales s* of `cfgzero_scale()`, fp32
     # [B]; `guidance_b`, when set, gives the per-sample guidance scales (else `guidance`)
     cfgzero_s: Optional[torch.Tensor] = None
+    # TCFG (dpm_step_tcfg; n_model == 2, per_sample set): the per-sample words (wu, wc) of `tcfg_words()`, fp32 [B, 2];
+    # `guidance_b`, when set, gives the per-sample guidance scales (else `guidance`)
+    tcfg_w: Optional[torch.Tensor] = None
     # CFG++ (dpm_step_cfgpp; form LIN1 or DIFF2, n_model == 2, predict_x0): alpha_t of the update's end time, the weight
     # of G - U; None is off. m_out then receives U, the x0 of e_uncond alone; `guidance_b`, when set, gives the
     # per-sample scales (else `guidance`, always combined)
@@ -254,13 +257,20 @@ class CudaBackend:
                          C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()),
                          C.c_void_p(None if r is None else r.data_ptr()), C.c_float(a.alpha_t), C.c_float(a.sigma_t))
         elif a.cfgpp_g is not None:
-            if a.thr is not None or a.ratio is not None or a.cfgzero_s is not None:
+            if a.thr is not None or a.ratio is not None or a.cfgzero_s is not None or a.tcfg_w is not None:
                 raise ValueError("dpm_solver_b200: a CFG++ step takes one or per-sample scales, without thresholds, "
-                                 "rescale or CFG-Zero*")
+                                 "rescale, CFG-Zero* or TCFG")
             self._launch(ref.device, self._lib.dpm_step_cfgpp, C.byref(d), C.c_float(a.cfgpp_g),
                          C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()))
         elif a.cfgzero_s is not None:
+            if a.tcfg_w is not None:
+                raise ValueError("dpm_solver_b200: a step takes CFG-Zero* scales or TCFG words, not both")
             self._launch(ref.device, self._lib.dpm_step_cfgzero, C.byref(d), C.c_void_p(a.cfgzero_s.data_ptr()),
+                         C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()))
+        elif a.tcfg_w is not None:
+            if a.ratio is not None:
+                raise ValueError("dpm_solver_b200: a TCFG step takes no rescale")
+            self._launch(ref.device, self._lib.dpm_step_tcfg, C.byref(d), C.c_void_p(a.tcfg_w.data_ptr()),
                          C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()))
         elif a.guidance_b is not None:
             # (phi and 1 - phi as below; ignored without a ratio)
@@ -279,7 +289,7 @@ class CudaBackend:
     def _check_per_sample(a: StepArgs, ref) -> None:
         """The per-sample operands of a step: fp32 on the tensors' device, one value per sample (the APG words two)."""
         for v, what, k in ((a.ratio, "ratio", 1), (a.guidance_b, "guidance_b", 1), (a.apg_words, "apg_words", 2),
-                           (a.cfgzero_s, "cfgzero_s", 1)):
+                           (a.cfgzero_s, "cfgzero_s", 1), (a.tcfg_w, "tcfg_w", 2)):
             if v is None:
                 continue
             if not v.is_cuda or v.dtype != torch.float32 or not v.is_contiguous() or v.device != ref.device:
@@ -335,6 +345,27 @@ class CudaBackend:
                      C.c_uint64(n), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
         return s
 
+    def tcfg_words(self, e_cond: torch.Tensor, e_uncond: torch.Tensor) -> torch.Tensor:
+        """TCFG's per-sample words (wu_b, wc_b), u' = wu_b*u + wc_b*c the projection of the unconditional output on the
+        first right singular vector of [u_b; c_b], as fp32 [B, 2] on the device (dpm_tcfg_words): fp64 sums ||u||^2,
+        <u, c>, ||c||^2 in storage order, merged per chunk in order, then the closed form of the header. Both halves
+        keep a shared dense layout (a sample is one contiguous block in row-major and channels_last storage alike)."""
+        n, dev = e_cond.numel(), e_cond.device
+        layout = self._layout(e_cond)
+        if layout is None or self._layout(e_uncond) != layout:
+            layout = "c"
+        ec = self._check(e_cond, "e_cond", dev, n, layout=layout)
+        eu = self._check(e_uncond, "e_uncond", dev, n, e_cond.dtype, layout)
+        nb = e_cond.shape[0]
+        per_sample = n // nb
+        w = torch.empty(nb, 2, dtype=torch.float32, device=dev)
+        ws_bytes = int(self._lib.dpm_tcfg_workspace(nb, per_sample))
+        ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev)
+        self._launch(dev, self._lib.dpm_tcfg_words, C.c_void_p(w.data_ptr()), C.c_void_p(ec.data_ptr()),
+                     C.c_void_p(eu.data_ptr()), C.c_int(_DTYPE_CODE[e_cond.dtype]), C.c_uint64(per_sample),
+                     C.c_uint64(n), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
+        return w
+
     def _step_multi(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
         """dpm_step_multi: the K conditional outputs and scales of a multi-condition CFG step (d already filled); with
         `a.masks`, dpm_step_multi_masked (1 <= K <= 4)."""
@@ -388,9 +419,9 @@ class CudaBackend:
     def _step_unipc(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
         """dpm_step_unipc: the UniPC words, m_{i-3} and the corrected-state output of a launch (d already filled)."""
         if a.e_conds is not None or a.guidance_b is not None or a.ratio is not None or a.apg_words is not None \
-                or a.cfgzero_s is not None or a.cfgpp_g is not None:
-            raise ValueError("dpm_solver_b200: a UniPC step takes one guidance scale, without rescale, APG, CFG-Zero* "
-                             "or CFG++")
+                or a.cfgzero_s is not None or a.cfgpp_g is not None or a.tcfg_w is not None:
+            raise ValueError("dpm_solver_b200: a UniPC step takes one guidance scale, without rescale, APG, CFG-Zero*, "
+                             "CFG++ or TCFG")
         w, u = a.unipc, _lib.UniDesc()
         n = ref.numel()
         if a.m3 is not None:
@@ -472,9 +503,10 @@ class CudaBackend:
         """Per-sample s_b = max(quantile(|x0_b|, q), max_val) -> fp32 [B].
         return_stats=True also returns the pipeline's per-sample header words (int32 [B, 8]:
         lo key, hi key, #below, #inside, path (1 bracket / 2 exact fallback), ...) for diagnostics."""
-        if a.guidance_b is not None or a.e_conds is not None or a.apg_words is not None or a.cfgzero_s is not None:
+        if a.guidance_b is not None or a.e_conds is not None or a.apg_words is not None or a.cfgzero_s is not None \
+                or a.tcfg_w is not None:
             raise ValueError("dpm_solver_b200: the quantile takes one guidance scale; materialise a per-sample, "
-                             "multi-condition, APG or CFG-Zero* combine first")
+                             "multi-condition, APG, CFG-Zero* or TCFG combine first")
         d, keep, ref, _, _ = self._fill(a)
         if a.per_sample <= 0 or ref.numel() % a.per_sample:
             raise ValueError("dpm_solver_b200: per_sample must divide numel")
@@ -681,11 +713,12 @@ class PreparedStep:
         if a.thr is not None or a.raw_round or a.ratio is not None or a.guidance_b is not None \
                 or a.e_conds is not None or a.coef_dev is not None or a.unipc is not None \
                 or a.apg_words is not None or a.cfgzero_s is not None or a.cfgpp_g is not None \
-                or a.out is not None and a.out2 is None:
+                or a.tcfg_w is not None or a.out is not None and a.out2 is None:
             # (a rescaled step reads a fresh ratio tensor every evaluation, an APG one fresh words, a CFG-Zero* one fresh
-            # scales s*, a CFG++ one goes through its own entry point, a guided one a scales tensor the
-            # descriptor does not carry, a multi-condition one K outputs and scales it does not carry, one with device
-            # coefficients a block the descriptor would point into without owning it: never frozen)
+            # scales s*, a TCFG one fresh words (wu, wc), a CFG++ one goes through its own entry point, a guided one a
+            # scales tensor the descriptor does not carry, a multi-condition one K outputs and scales it does not
+            # carry, one with device coefficients a block the descriptor would point into without owning it: never
+            # frozen)
             return None
         ref = a.reference_tensor()
         if not ref.is_contiguous():

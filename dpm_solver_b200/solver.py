@@ -58,6 +58,7 @@ class RawOutput:
     apg: Optional[tuple] = None     # adaptive projected guidance of the combine: (eta, norm_threshold, momentum)
     cfgzero: bool = False           # CFG-Zero*: the combine against s*-scaled `e_uncond` (model_wrapper's cfg_zero_star)
     cfgpp: bool = False             # CFG++: an update buffers U (e_uncond alone) and adds g*(G - U) (model_wrapper's cfg_pp)
+    tcfg: bool = False              # TCFG: the combine against the damped `e_uncond` (model_wrapper's tcfg)
 
 
 def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale, masked=False):
@@ -208,9 +209,10 @@ class WrappedModel:
     def __init__(self, model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                  unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale=0.,
                  apg_eta=None, apg_norm_threshold=0., apg_momentum=0., cfg_zero_star=False, cfg_zero_init_steps=0,
-                 cfg_pp=False, guidance_mask=None):
+                 cfg_pp=False, guidance_mask=None, tcfg=False):
         self.model = model
         self.cfg_pp = cfg_pp
+        self.tcfg = tcfg
         self.guidance_rescale = guidance_rescale
         self.cfg_zero_star = bool(cfg_zero_star)
         self.cfg_zero_init_steps = cfg_zero_init_steps
@@ -365,9 +367,9 @@ class WrappedModel:
             out_u, out_c = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(2)  # uncond first
             if gb is not None:
                 return RawOutput(out_c, out_u, param, 1.0, self.guidance_rescale, gb, apg=self.apg,
-                                 cfgzero=self.cfg_zero_star, cfgpp=cfgpp)
+                                 cfgzero=self.cfg_zero_star, cfgpp=cfgpp, tcfg=self.tcfg)
             return RawOutput(out_c, out_u, param, float(self._one_scale()), self.guidance_rescale, apg=self.apg,
-                             cfgzero=self.cfg_zero_star, cfgpp=cfgpp)
+                             cfgzero=self.cfg_zero_star, cfgpp=cfgpp, tcfg=self.tcfg)
         raise RuntimeError("raw() is not available with classifier guidance")
 
     def _alpha_sigma(self, t_continuous):
@@ -434,6 +436,7 @@ class WrappedModel:
         xo = x.to(r.e_cond.dtype) if needs_x else None
         ratio = _cfg_ratio(be, r)      # over the whole batch: each sample's ratio reads its own values only
         zs = be.cfgzero_scale(r.e_cond, r.e_uncond) if r.cfgzero and r.e_uncond is not None else None   # likewise
+        tw = be.tcfg_words(r.e_cond, r.e_uncond) if r.tcfg and r.e_uncond is not None else None         # likewise
 
         def convert(rows, alpha, sigma):
             a = StepArgs(form=FORM_NONE, n_model=2 if r.e_uncond is not None else 1, e_cond=r.e_cond[rows],
@@ -442,6 +445,8 @@ class WrappedModel:
             _guidance_args(a, None if ratio is None else ratio[rows], r, rows)
             if zs is not None:
                 a.cfgzero_s, a.per_sample = zs[rows], a.e_cond.numel() // a.e_cond.shape[0]
+            if tw is not None:
+                a.tcfg_w, a.per_sample = tw[rows], a.e_cond.numel() // a.e_cond.shape[0]
             if needs_x:
                 a.xe = xo[rows]
             return be.step(a)[0]
@@ -451,7 +456,7 @@ class WrappedModel:
 def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, guidance_type="uncond",
                   condition=None, unconditional_condition=None, guidance_scale=1., classifier_fn=None,
                   classifier_kwargs={}, guidance_rescale=0., apg_eta=None, apg_norm_threshold=0., apg_momentum=0.,
-                  cfg_zero_star=False, cfg_zero_init_steps=0, cfg_pp=False, guidance_mask=None):
+                  cfg_zero_star=False, cfg_zero_init_steps=0, cfg_pp=False, guidance_mask=None, tcfg=False):
     """Wrap a network into `model_fn(x, t_continuous) -> noise`; same contract as the reference
     (:170-334): model_type in {noise, x_start, v, score}, guidance_type in {uncond, classifier,
     classifier-free}.
@@ -580,7 +585,47 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     passes the masks of its own rows); a direct call of this callable returns the masked combine. Not available
     (ValueError): other guidance types, no unconditional_condition, a mask count other than K, an entry that is neither
     a tensor nor None, a per-sample guidance_scale (use a [B, 1, 1, 1] mask), guidance_rescale != 0, apg_eta,
-    cfg_zero_star, cfg_pp, UniPC and DPM_Solver(reference_rounding=True)."""
+    cfg_zero_star, cfg_pp, UniPC and DPM_Solver(reference_rounding=True).
+
+    tcfg=True (classifier-free guidance only; not in the reference; default False; anything other than a bool is a
+    ValueError): tangential-damping CFG ("TCFG: Tangential Damping Classifier-free Guidance", CVPR 2025; diffusers'
+    TangentialClassifierFreeGuidance guider, ComfyUI's TCFG node). The damping works in the network's raw output space,
+    as cfg_zero_star does: the noise of a "noise" network, the velocity of a "flow" one, whatever the network returns
+    for "x_start", "v", "score" and "edm" -- the space of diffusers' guider. ComfyUI damps x - denoised, which is
+    sigma*eps or sigma*v for noise and flow networks; the damping is invariant to a per-sample factor common to both
+    outputs, so it gives the same words there.
+    Definition: per sample b, with c and u the conditional and unconditional outputs flattened over all non-batch
+    dimensions in storage order, M the 2 x D matrix with rows u and c and v1 its first right singular vector, the damped
+    unconditional output is u' = <u, v1>*v1 (diffusers and ComfyUI compute it with torch.linalg.svd), and the guided
+    raw output g = u' + w_b*(c - u') is then converted by the parameterisation as it converts a single output.
+    This library evaluates u' in closed form from the 2 x 2 Gram matrix, u' = wu_b*u + wc_b*c. A = ||u||^2,
+    B = <u, c>, C = ||c||^2 are fp64 sums of the fp32-widened outputs, in the chunking, thread ownership and chunk-merge
+    order of the CFG-Zero* pass, so the words of sample b depend on sample b's values only. Then, in fp64 with each
+    operation rounded:
+        h = 0.5*(A - C);  r = sqrt(h*h + B*B)
+        if C >= A:  p = B;      q = (-h) + r
+        else:       p = h + r;  q = B
+        pp = p*p;  n2 = pp + q*q
+        wu = fl32(pp / n2);  wc = fl32((p*q) / n2)
+    (p, q) is the top eigenvector of the Gram matrix, taken from the row without cancellation, and the closed form is
+    the eigen identity. n2 == 0 happens only when A == C and B == 0 (both outputs zero included): the top singular
+    direction is then not unique and the words are (1, 0), plain CFG. A sum that is not finite gives NaN words. Then
+    per element, in fp32 with each operation rounded and no contraction, in this order:
+        us = u*wu + c*wc;   g = us + w*(c - us);   value = convert(g)
+    diffusers casts u' to the model's dtype and combines in it; this library combines in fp32, as cfg_zero_star and
+    plain CFG do. Consequences: a network blind to the condition (c == u) gives A = B = C, r = |B| exactly and the
+    words exactly (0.5, 0.5), so us == u and g == u for normal operands: such a run equals the unguided run by value,
+    at any scale and in every state dtype. Rank-1 pairs (c = k*u) give u' = u in exact arithmetic, plain CFG. A scalar
+    guidance_scale of 1 keeps the bypass (one network half, the conditional output alone, no words pass); a per-sample
+    scale of 1 gives that row c. Cost per guided evaluation: the words pass (2 launches reading both halves once) and
+    the fused step; with dynamic thresholding, and under UniPC, g is materialised once in fp32 (+1 launch) first.
+    Accepted: scalar or per-sample [B] scales, every model type and schedule (VP discrete, linear and cosine, flow,
+    EDM), both algorithms, singlestep, multistep, singlestep_fixed and adaptive (host or device controller), dynamic
+    thresholding, correcting_x0_fn / correcting_xt_fn, denoise_to_zero, inverse(), return_intermediate, capture(),
+    batch sharding (the words are per sample: no collective) and UniPC. A direct call of this callable returns the
+    converted TCFG value. Not available (ValueError before any launch and any network call): other guidance types, no
+    unconditional_condition, several conditions, guidance_mask, guidance_rescale != 0, apg_eta, cfg_zero_star, cfg_pp
+    and DPM_Solver(reference_rounding=True)."""
     assert model_type in ["noise", "x_start", "v", "score", "flow", "edm"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
     flow_schedule = getattr(noise_schedule, "schedule", None) == "flow"
@@ -637,6 +682,23 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
             raise ValueError("cfg_pp is not available with adaptive projected guidance (apg_eta)")
         if cfg_zero_star:
             raise ValueError("cfg_pp is not available with cfg_zero_star")
+    if not isinstance(tcfg, bool):
+        raise ValueError("tcfg must be a bool, got {!r}".format(tcfg))
+    if tcfg:
+        if guidance_type != "classifier-free" or unconditional_condition is None:
+            raise ValueError("tcfg needs guidance_type='classifier-free' and an unconditional_condition")
+        if isinstance(condition, (list, tuple)) and len(condition) >= 2:
+            raise ValueError("tcfg is not available with several conditions")
+        if guidance_mask is not None:
+            raise ValueError("tcfg is not available with guidance_mask")
+        if guidance_rescale != 0:
+            raise ValueError("tcfg is not available with guidance_rescale")
+        if apg_eta is not None:
+            raise ValueError("tcfg is not available with adaptive projected guidance (apg_eta)")
+        if cfg_zero_star:
+            raise ValueError("tcfg is not available with cfg_zero_star")
+        if cfg_pp:
+            raise ValueError("tcfg is not available with cfg_pp")
     if guidance_mask is not None:
         condition, guidance_scale, guidance_mask = _masked_arguments(
             guidance_type, condition, unconditional_condition, guidance_scale, guidance_mask, guidance_rescale,
@@ -653,7 +715,7 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     return WrappedModel(model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                         unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale,
                         apg_eta, apg_norm_threshold, apg_momentum, cfg_zero_star, cfg_zero_init_steps, cfg_pp,
-                        guidance_mask)
+                        guidance_mask, tcfg)
 
 
 def _masked_arguments(guidance_type, condition, unconditional_condition, guidance_scale, guidance_mask,
@@ -765,6 +827,8 @@ class DPM_Solver:
             raise ValueError("adaptive projected guidance is not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "cfg_zero_star", False):
             raise ValueError("cfg_zero_star is not available with reference_rounding=True")
+        if self.reference_rounding and getattr(model_fn, "tcfg", False):
+            raise ValueError("tcfg is not available with reference_rounding=True")
         if getattr(model_fn, "cfg_pp", False):
             if algorithm_type != "dpmsolver++":
                 raise ValueError("cfg_pp needs algorithm_type='dpmsolver++' (CFG++ re-noises a data prediction)")
@@ -1042,7 +1106,7 @@ class DPM_Solver:
             # (and so is dynamic thresholding: a launch frozen without the clamp never serves a solver switched to it)
             pkey = (slot, raw.param, raw.guidance, raw.phi, raw.guidance_b is None, raw.e_uncond is None,
                     raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, raw.scales, self._dynamic_thresholding,
-                    raw.apg, raw.cfgzero, raw.cfgpp)
+                    raw.apg, raw.cfgzero, raw.cfgpp, raw.tcfg)
             prep = self._prep_cache.get(pkey)
             if prep is not None:
                 r = prep.launch((x, xe, raw.e_cond, m1, m2, raw.e_cond, raw.e_uncond))
@@ -1114,6 +1178,18 @@ class DPM_Solver:
                              per_sample=raw.e_cond.numel() // raw.e_cond.shape[0], cfgzero_s=cfz)
                 raw = RawOutput(be.step(a)[0], None, raw.param, 1.0)
                 cfz = None
+        tcw = None          # TCFG's per-sample words (wu, wc) of a fused evaluation
+        if raw.tcfg and raw.e_uncond is not None:
+            # the words pass over both raw halves (+2 launches), then the fused step; with dynamic thresholding, and
+            # under UniPC, g is materialised once in fp32 (+1 launch) and handed on as one network output, as for
+            # CFG-Zero*
+            tcw = be.tcfg_words(raw.e_cond, raw.e_uncond)
+            if (x0 and self._dynamic_thresholding) or self._apg_materialise:
+                a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
+                             guidance=raw.guidance, state_dtype=torch.float32, guidance_b=raw.guidance_b,
+                             per_sample=raw.e_cond.numel() // raw.e_cond.shape[0], tcfg_w=tcw)
+                raw = RawOutput(be.step(a)[0], None, raw.param, 1.0)
+                tcw = None
         ratio = _cfg_ratio(be, raw)     # guidance rescale: one streaming pass over both halves (+2 launches)
         if code:
             # reference-rounding mode (raw 16-bit NOISE outputs, fp32 state): bits 0-1 make the fused kernel take the
@@ -1165,6 +1241,8 @@ class DPM_Solver:
         a = apg_a if apg_a is not None else _guidance_args(self._conv_args(raw, xe, alsig, sd, x0), ratio, raw)
         if cfz is not None:
             a.cfgzero_s, a.per_sample = cfz, raw.e_cond.numel() // raw.e_cond.shape[0]
+        if tcw is not None:
+            a.tcfg_w, a.per_sample = tcw, raw.e_cond.numel() // raw.e_cond.shape[0]
         if alsig is _DEV:
             if co is None or co.dev is None:
                 raise RuntimeError("device-side scalars need the coefficient block of the consuming launch")

@@ -62,6 +62,10 @@ materialises the guided raw output g in fp32, then the UniPC launch converting g
 state. Zero-init evaluations (cfg_zero_init_steps) are one-output launches on a raw output of 0, counted as in
 DPM_Solver.
 
+TCFG (model_wrapper's tcfg) runs with a scalar scale, as CFG-Zero* does: per evaluation the words pass (2 launches),
+one launch that materialises the guided raw output g = us + w*(c - us), us = wu*u + wc*c, in fp32, then the UniPC
+launch converting g as a single network output at its own state.
+
 Not available (ValueError before any launch): per-sample guidance scales, several conditions, guidance masks,
 guidance rescale, reference_rounding, plan_broadcast, orders outside 1..3, steps < order.
 """
@@ -88,7 +92,7 @@ class _Launch:
 
 
 class UniPC(DPM_Solver):
-    _apg_materialise = True     # APG: the buffered value (+1 launch), then this launch on it; CFG-Zero*: g (+1 launch)
+    _apg_materialise = True     # APG: the buffered value (+1 launch), then this launch on it; CFG-Zero*, TCFG: g (+1)
 
     def __init__(self, model_fn, noise_schedule, algorithm_type="dpmsolver++", variant="bh2", correcting_x0_fn=None,
                  correcting_xt_fn=None, thresholding_max_val=1., dynamic_thresholding_ratio=0.995, state_dtype=None):

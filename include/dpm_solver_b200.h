@@ -28,8 +28,8 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 108 /* 0.1.8: CFG++ (dpm_step_cfgpp); regional guidance (dpm_step_multi_masked) is an
-                                addition to this ABI: test for its symbol */
+#define DPM_B200_VERSION 108 /* 0.1.8: CFG++ (dpm_step_cfgpp); regional guidance (dpm_step_multi_masked) and TCFG
+                                (dpm_tcfg_words, dpm_step_tcfg) are additions to this ABI: test for their symbols */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -371,6 +371,34 @@ DPM_API int dpm_cfgzero_scale(float* s_out, const void* e_cond, const void* e_un
                               dpm_stream_t stream);
 DPM_API int dpm_step_cfgzero(const dpm_step_desc* desc, const float* s_star, const float* guidance,
                              dpm_stream_t stream);
+
+/* ---- TCFG ("TCFG: Tangential Damping Classifier-free Guidance", CVPR 2025) ------------------------------------------
+ * Classifier-free guidance against the unconditional output projected, per sample, on the first right singular vector
+ * v1 of the 2 x per_sample matrix [u; c], in the network's raw output space. Per sample b (c = e_cond, u = e_uncond,
+ * both flattened in storage order), A = ||u_b||^2, B = <u_b, c_b>, C = ||c_b||^2 (fp64 sums of the fp32-widened
+ * outputs, in the chunking and merge order of dpm_cfgzero_scale), then in fp64 with each op rounded:
+ *   h = 0.5*(A - C);  r = sqrt(h*h + B*B)
+ *   C >= A:  p = B,  q = (-h) + r;   else:  p = h + r,  q = B
+ *   pp = p*p;  n2 = pp + q*q;  wu_b = fl32(pp / n2);  wc_b = fl32((p*q) / n2)
+ * so that u' = <u, v1>*v1 = wu_b*u + wc_b*c. n2 == 0 (A == C and B == 0, both outputs zero included) gives (1, 0);
+ * a sum that is not finite gives NaN words. Per element, three rounded fp32 ops in this order, then the
+ * parameterisation converts g as it converts a single output:
+ *   us = u*wu_b + c*wc_b,  g = us + w_b*(c - us)
+ * A sample with w_b == 1 gets the converted c alone.
+ * dpm_tcfg_words: (wu_b, wc_b) -> w_out[2*b], w_out[2*b + 1] for b < n/per_sample, fp32 device memory. Reads the two
+ *   halves only (2*s_model bytes per element). workspace: dpm_tcfg_workspace(n/per_sample, per_sample) bytes of 8-byte
+ *   aligned device memory (contents irrelevant). Two launches.
+ * dpm_step_tcfg: dpm_step with g in place of the combine. guidance: NULL (w_b = desc->guidance) or the per-sample
+ *   scales, fp32 [n/per_sample] in device memory. Needs desc->n_model == 2, desc->raw_round == 0, desc->per_sample != 0
+ *   dividing n and words != NULL (DPM_ERR_ARG). Served like dpm_step_cfgzero: the IEEE-division instantiations of the
+ *   direct vector kernels for per-sample guidance, the generic kernel for tails, unaligned views and dev_coef
+ *   launches, never the TMA variant. Call the words pass and then the step on one stream; neither synchronises or
+ *   allocates. Both entry points were added within version 108: test for their symbols. */
+DPM_API size_t dpm_tcfg_workspace(uint64_t n_samples, uint64_t per_sample);
+DPM_API int dpm_tcfg_words(float* w_out, const void* e_cond, const void* e_uncond, int model_dtype,
+                           uint64_t per_sample, uint64_t n, void* workspace, size_t workspace_bytes,
+                           dpm_stream_t stream);
+DPM_API int dpm_step_tcfg(const dpm_step_desc* desc, const float* words, const float* guidance, dpm_stream_t stream);
 
 /* ---- CFG++ (Chung, Kim, Park, Nam and Ye, "CFG++: Manifold-constrained Classifier Free Guidance for Diffusion
  * Models", ICLR 2025, arXiv:2406.08070) -------------------------------------------------------------------------------
