@@ -66,7 +66,7 @@ class CondMap(C.Structure):
     _fields_ = [("w", C.c_void_p), ("period", C.c_uint64), ("sample_stride", C.c_uint64)]
 
 
-_vp, _f, _u64, _i = C.c_void_p, C.c_float, C.c_uint64, C.c_int
+_vp, _f, _u64, _i, _i64 = C.c_void_p, C.c_float, C.c_uint64, C.c_int, C.c_int64
 
 # name -> (restype, argtypes); every prototype of the header appears here and is checked at load
 PROTOTYPES = {
@@ -116,9 +116,13 @@ PROTOTYPES = {
     "dpm_tcfg_workspace": (C.c_size_t, [_u64, _u64]),
     "dpm_tcfg_words": (C.c_int, [_vp, _vp, _vp, _i, _u64, _u64, _vp, C.c_size_t, _vp]),
     "dpm_step_tcfg": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _vp]),
+    "dpm_fdg_supported": (C.c_int, [_u64, _u64, _i, _i]),
+    "dpm_fdg_guided": (C.c_int, [_vp, _vp, _vp, _i, _u64, _u64, _u64, _i64, _i64, _i64, _i64, _i, _vp, _u64, _u64,
+                                 _vp]),
 }
 
 MAX_CONDITIONS = 4      # DPM_MAX_CONDITIONS
+FDG_MAX_LEVELS = 5      # DPM_FDG_MAX_LEVELS
 
 _lib = None
 

@@ -674,6 +674,19 @@ int dpm_step_tcfg(const dpm_step_desc* desc, const float* words, const float* gu
   return step_impl(desc, static_cast<cudaStream_t>(stream), nullptr, guidance, nullptr, nullptr, words);
 }
 
+int dpm_fdg_supported(uint64_t H, uint64_t W, int levels, int model_dtype) {
+  return fdg_supported(H, W, levels, model_dtype);
+}
+
+int dpm_fdg_guided(void* g_out, const void* e_cond, const void* e_uncond, int model_dtype, uint64_t planes, uint64_t H,
+                   uint64_t W, int64_t sample_stride, int64_t plane_stride, int64_t h_stride, int64_t w_stride,
+                   int levels, const float* scales, uint64_t scale_stride, uint64_t planes_per_sample,
+                   dpm_stream_t stream) {
+  return finish(launch_fdg_guided(g_out, e_cond, e_uncond, model_dtype, planes, H, W, sample_stride, plane_stride,
+                                  h_stride, w_stride, levels, scales, scale_stride, planes_per_sample,
+                                  static_cast<cudaStream_t>(stream)));
+}
+
 int dpm_step_cfgpp(const dpm_step_desc* desc, float g, const float* guidance, dpm_stream_t stream) {
   return step_cfgpp_impl(desc, g, guidance, static_cast<cudaStream_t>(stream));
 }

@@ -10,6 +10,7 @@ from __future__ import annotations
 import ctypes as C
 import dataclasses
 from dataclasses import dataclass
+import math
 from typing import Optional, Tuple
 
 import torch
@@ -117,6 +118,42 @@ _raw_stream = getattr(torch._C, "_cuda_getCurrentRawStream", None)
 if _raw_stream is None:  # older torch: go through the Stream object
     def _raw_stream(idx):
         return torch.cuda.current_stream(idx).cuda_stream
+
+
+def fdg_check(shape, levels: int, dtype=torch.float32) -> None:
+    """ValueError unless frequency-decoupled guidance serves outputs of `shape` with `levels` levels: at least 4 dims,
+    and planes of the last two that dpm_fdg_supported accepts (the library's one statement of the size rule)."""
+    if len(shape) < 4:
+        raise ValueError("frequency-decoupled guidance needs x with at least 4 dims [B, C, ..., H, W], got shape "
+                         "{}".format(tuple(shape)))
+    if dtype not in _DTYPE_CODE:
+        raise TypeError("dpm_solver_b200: unsupported dtype {} for frequency-decoupled guidance".format(dtype))
+    lib = _lib.lib()
+    if lib.dpm_fdg_supported(int(shape[-2]), int(shape[-1]), int(levels), _DTYPE_CODE[dtype]) != 0:
+        raise ValueError("frequency-decoupled guidance with x of shape {}: {}".format(
+            tuple(shape), lib.dpm_last_error().decode("utf-8", "replace")))
+
+
+def _dense(t: torch.Tensor) -> bool:
+    """True when the elements of `t` fill its storage span exactly once in some order of its dims (row-major,
+    channels_last, transposed or otherwise permuted views): an output allocated with its strides has no gaps."""
+    expect = 1
+    for st, n in sorted((st, n) for n, st in zip(t.shape, t.stride()) if n != 1):
+        if st != expect:
+            return False
+        expect *= n
+    return True
+
+
+def _plane_strides(t: torch.Tensor):
+    """(sample_stride, plane_stride, h_stride, w_stride) in elements of a [B, *mid, H, W] tensor whose planes are
+    indexed by one stride over the flattened mid dims (row-major and 4-D channels_last alike), else None."""
+    mid = [(n, st) for n, st in zip(t.shape[1:-2], t.stride()[1:-2]) if n != 1]
+    for (n0, s0), (n1, s1) in zip(mid, mid[1:]):
+        if s0 != s1 * n1:
+            return None
+    plane = mid[-1][1] if mid else 0
+    return t.stride(0), plane, t.stride(-2), t.stride(-1)
 
 
 class CudaBackend:
@@ -365,6 +402,41 @@ class CudaBackend:
                      C.c_void_p(eu.data_ptr()), C.c_int(_DTYPE_CODE[e_cond.dtype]), C.c_uint64(per_sample),
                      C.c_uint64(n), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
         return w
+
+    def fdg_guided(self, e_cond: torch.Tensor, e_uncond: torch.Tensor, scales, levels: int) -> torch.Tensor:
+        """Frequency-decoupled guidance (dpm_fdg_guided, one launch): g over the planes of the last two dims, in the
+        outputs' dtype and dense layout. `scales`: `levels` python floats shared by the batch, or an fp32 [B, levels]
+        tensor on the outputs' device (one row per sample)."""
+        dev = e_cond.device
+        fdg_check(e_cond.shape, levels, e_cond.dtype)
+        for t, what in ((e_cond, "e_cond"), (e_uncond, "e_uncond")):
+            if not t.is_cuda or t.device != dev:
+                raise RuntimeError(f"dpm_solver_b200: `{what}` is on {t.device}; expected {dev} (CUDA only)")
+            if t.dtype != e_cond.dtype or t.shape != e_cond.shape:
+                raise ValueError(f"dpm_solver_b200: `{what}` is {t.dtype} {tuple(t.shape)}, expected "
+                                 f"{e_cond.dtype} {tuple(e_cond.shape)}")
+        ec, eu = e_cond, e_uncond
+        strides = _plane_strides(ec) if _dense(ec) else None
+        if strides is None or eu.stride() != ec.stride():
+            ec, eu = ec.contiguous(), eu.contiguous()       # (any other layout: the same bits, at a copy's cost)
+            strides = _plane_strides(ec)
+        g = torch.empty_strided(ec.shape, ec.stride(), dtype=ec.dtype, device=dev)
+        B, H, W = ec.shape[0], ec.shape[-2], ec.shape[-1]
+        pps = math.prod(ec.shape[1:-2])
+        if torch.is_tensor(scales):
+            if not scales.is_cuda or scales.device != dev or scales.dtype != torch.float32 \
+                    or tuple(scales.shape) != (B, levels) or not scales.is_contiguous():
+                raise ValueError("dpm_solver_b200: per-sample FDG scales must be a contiguous fp32 [{}, {}] tensor on "
+                                 "{}".format(B, levels, dev))
+            sp, stride = C.c_void_p(scales.data_ptr()), levels
+        else:
+            host = (C.c_float * levels)(*scales)
+            sp, stride = C.cast(host, C.c_void_p), 0
+        self._launch(dev, self._lib.dpm_fdg_guided, C.c_void_p(g.data_ptr()), C.c_void_p(ec.data_ptr()),
+                     C.c_void_p(eu.data_ptr()), C.c_int(_DTYPE_CODE[ec.dtype]), C.c_uint64(B * pps), C.c_uint64(H),
+                     C.c_uint64(W), *(C.c_int64(v) for v in strides), C.c_int(levels), sp, C.c_uint64(stride),
+                     C.c_uint64(pps))
+        return g
 
     def _step_multi(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
         """dpm_step_multi: the K conditional outputs and scales of a multi-condition CFG step (d already filled); with

@@ -59,6 +59,9 @@ class RawOutput:
     cfgzero: bool = False           # CFG-Zero*: the combine against s*-scaled `e_uncond` (model_wrapper's cfg_zero_star)
     cfgpp: bool = False             # CFG++: an update buffers U (e_uncond alone) and adds g*(G - U) (model_wrapper's cfg_pp)
     tcfg: bool = False              # TCFG: the combine against the damped `e_uncond` (model_wrapper's tcfg)
+    # frequency-decoupled guidance (model_wrapper's fdg_scales): (scales, levels), the scales `levels` python floats or
+    # an fp32 [B, levels] tensor on the outputs' device; the solver turns the pair into one output g (dpm_fdg_guided)
+    fdg: Optional[tuple] = None
 
 
 def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale, masked=False):
@@ -186,6 +189,47 @@ def _apg_args(be, raw: RawOutput, xe, marg, sdtype, x0: bool, ns, coef_dev=None,
     return a
 
 
+def _fdg_scales(fdg_scales):
+    """model_wrapper's fdg_scales -> (levels, shared, tensor): the N shared scales as python floats, each rounded to
+    fp32 once (a list or tuple of numbers), or None and the tensor `WrappedModel.fdg_args` converts once per (tensor,
+    version, device, B) or reads in place (a 1-D tensor, a [B, N] tensor, or a list or tuple holding tensors, which are
+    stacked on their device). The host never reads a tensor's values."""
+    s = fdg_scales
+    if isinstance(s, (list, tuple)) and any(torch.is_tensor(v) for v in s):
+        if any(not torch.is_tensor(v) or v.numel() != 1 for v in s) or len({v.device for v in s}) != 1:
+            raise ValueError("fdg_scales as a list or tuple of tensors takes N one-element tensors on one device")
+        s = torch.stack([v.detach().reshape(()) for v in s])
+    if torch.is_tensor(s):
+        if s.dim() not in (1, 2):
+            raise ValueError("fdg_scales must be a list, a tuple, a 1-D tensor of N scales or a [B, N] tensor, got "
+                             "shape {}".format(tuple(s.shape)))
+        if s.is_complex():
+            raise ValueError("fdg_scales must be real, got {}".format(s.dtype))
+        levels, shared = s.shape[-1], False
+    elif isinstance(s, (list, tuple)):
+        if any(isinstance(v, (list, tuple)) for v in s):
+            raise ValueError("fdg_scales as a list or tuple takes N numbers")
+        levels, shared = len(s), True
+    else:
+        raise ValueError("fdg_scales must be a list, a tuple, a 1-D tensor of N scales or a [B, N] tensor, got "
+                         "{!r}".format(type(s).__name__))
+    if not 1 <= levels <= ops._lib.FDG_MAX_LEVELS:
+        raise ValueError("fdg_scales takes 1 to {} levels, got {}".format(ops._lib.FDG_MAX_LEVELS, levels))
+    if shared:
+        return levels, tuple(torch.tensor([float(v) for v in s], dtype=torch.float32).tolist()), None
+    return levels, None, s
+
+
+def _fdg_output(be, raw: RawOutput) -> RawOutput:
+    """A frequency-decoupled guidance evaluation as one network output: g in the outputs' dtype (1 launch), which the
+    parameterisation then converts as it converts a single output."""
+    fn = getattr(be, "fdg_guided", None)
+    if fn is None:
+        raise RuntimeError("fdg_scales needs an executor with fdg_guided; {} has none".format(
+            getattr(be, "name", type(be).__name__)))
+    return RawOutput(fn(raw.e_cond, raw.e_uncond, *raw.fdg), None, raw.param, 1.0)
+
+
 def _scale_vector(guidance_scale, guidance_type):
     """model_wrapper's guidance_scale as per-sample scales (a 1-D tensor, or None for one scale). A python number, a
     0-dim or a one-element tensor is one scale, as before; any other tensor must be 1-D."""
@@ -209,10 +253,14 @@ class WrappedModel:
     def __init__(self, model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                  unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale=0.,
                  apg_eta=None, apg_norm_threshold=0., apg_momentum=0., cfg_zero_star=False, cfg_zero_init_steps=0,
-                 cfg_pp=False, guidance_mask=None, tcfg=False):
+                 cfg_pp=False, guidance_mask=None, tcfg=False, fdg_scales=None):
         self.model = model
         self.cfg_pp = cfg_pp
         self.tcfg = tcfg
+        # frequency-decoupled guidance: its number of levels (0: off), shared scales or the per-sample tensor
+        self.fdg_levels, self._fdg_shared, self._fdg_vec = (0, None, None) if fdg_scales is None else \
+            _fdg_scales(fdg_scales)
+        self._fdg_dev = None
         self.guidance_rescale = guidance_rescale
         self.cfg_zero_star = bool(cfg_zero_star)
         self.cfg_zero_init_steps = cfg_zero_init_steps
@@ -283,7 +331,8 @@ class WrappedModel:
     def uses_cfg(self) -> bool:
         # (several conditions: guidance_scale is their tuple of scales, never equal to 1 -- always combined, no bypass)
         # (CFG++ reads both halves at every evaluation: a scalar scale of 1 is combined, not bypassed)
-        return self._combines() or self.cfg_pp
+        # (frequency-decoupled guidance always combines both halves, whatever its scales)
+        return self._combines() or self.cfg_pp or self.fdg_levels > 0
 
     def _combines(self) -> bool:
         """The plain guided noise combines the two halves (the reference's test :323)."""
@@ -310,6 +359,29 @@ class WrappedModel:
             # the source is kept alive next to the key so that its id cannot be recycled
             self._gs = (key, s.detach().to(device=x.device, dtype=torch.float32).contiguous(), s)
         return self._gs[1]
+
+    def fdg_args(self, x) -> tuple:
+        """(scales, levels) of a frequency-decoupled guidance evaluation at x: the shared python floats, or fp32
+        [B, N] on x's device. A contiguous fp32 [B, N] tensor already there is read in place (values written into it
+        between graph replays take effect); any other form is converted once per (tensor, version, device, B). Checks
+        x against the size rule, and the per-sample rows against x's batch (ValueError); never reads device values on
+        the host."""
+        L = self.fdg_levels
+        ops.fdg_check(x.shape, L)
+        if self._fdg_shared is not None:
+            return self._fdg_shared, L
+        s, B = self._fdg_vec, x.shape[0]
+        if s.dim() == 2:
+            if s.shape[0] != B:
+                raise ValueError("fdg_scales has {} rows for a batch of {}".format(s.shape[0], B))
+            if s.device == x.device and s.dtype == torch.float32 and s.is_contiguous():
+                return s, L
+        key = (id(s), s._version, str(x.device), B)
+        if self._fdg_dev is None or self._fdg_dev[0] != key:
+            # the source is kept alive next to the key so that its id cannot be recycled
+            v = s.detach().to(device=x.device, dtype=torch.float32)
+            self._fdg_dev = (key, v.expand(B, L).contiguous(), s)
+        return self._fdg_dev[1], L
 
     @property
     def fusable(self) -> bool:
@@ -358,13 +430,16 @@ class WrappedModel:
                              masks=self.cond_masks)
         if self.guidance_type == "classifier-free":
             gb = self._scales(x) if self._scale_vec is not None else None     # (checked before the network runs)
-            if not (self._combines() if plain else self.uses_cfg):
+            fdg = self.fdg_args(x) if self.fdg_levels else None               # likewise
+            if not ((self._combines() or self.fdg_levels > 0) if plain else self.uses_cfg):
                 return RawOutput(self._call_model(x, t_continuous, cond=self.condition, t_input=t_input), None, param, 1.0)
             cfgpp = self.cfg_pp and not plain
             if x_in is None:
                 x_in = ops.backend().duplicate(x)              # cat([x] * 2) :326 (the solver hands over a prebuilt one)
             t_in = None if t_input is not None else torch.cat([t_continuous] * 2)
             out_u, out_c = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(2)  # uncond first
+            if fdg is not None:
+                return RawOutput(out_c, out_u, param, 1.0, fdg=fdg)
             if gb is not None:
                 return RawOutput(out_c, out_u, param, 1.0, self.guidance_rescale, gb, apg=self.apg,
                                  cfgzero=self.cfg_zero_star, cfgpp=cfgpp, tcfg=self.tcfg)
@@ -415,6 +490,8 @@ class WrappedModel:
                 return ops.lincomb(o, [grad[rows]], 1.0, [-gs])
             return self._per_sample(pairs, x.shape[0], guided)
         r = self.raw(x, t_continuous, plain=True)
+        if r.fdg is not None:
+            r = _fdg_output(be, r)        # g, then converted as one network output
         if r.e_uncond is None and r.param == PARAM_NOISE:
             return r.e_cond
         if r.apg is not None and r.e_uncond is not None:
@@ -456,7 +533,8 @@ class WrappedModel:
 def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, guidance_type="uncond",
                   condition=None, unconditional_condition=None, guidance_scale=1., classifier_fn=None,
                   classifier_kwargs={}, guidance_rescale=0., apg_eta=None, apg_norm_threshold=0., apg_momentum=0.,
-                  cfg_zero_star=False, cfg_zero_init_steps=0, cfg_pp=False, guidance_mask=None, tcfg=False):
+                  cfg_zero_star=False, cfg_zero_init_steps=0, cfg_pp=False, guidance_mask=None, tcfg=False,
+                  fdg_scales=None):
     """Wrap a network into `model_fn(x, t_continuous) -> noise`; same contract as the reference
     (:170-334): model_type in {noise, x_start, v, score}, guidance_type in {uncond, classifier,
     classifier-free}.
@@ -625,7 +703,55 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     batch sharding (the words are per sample: no collective) and UniPC. A direct call of this callable returns the
     converted TCFG value. Not available (ValueError before any launch and any network call): other guidance types, no
     unconditional_condition, several conditions, guidance_mask, guidance_rescale != 0, apg_eta, cfg_zero_star, cfg_pp
-    and DPM_Solver(reference_rounding=True)."""
+    and DPM_Solver(reference_rounding=True).
+
+    fdg_scales=[w_0, ..., w_{N-1}] (classifier-free guidance only; not in the reference; default None: off):
+    frequency-decoupled guidance (Sadat, Vontobel, Salehi and Weber, "Guidance in the Frequency Domain Enables
+    High-Fidelity Sampling at Low CFG Scales", 2025; diffusers' FrequencyDecoupledGuidance guider). c - u is split into
+    the N levels of a Laplacian pyramid over the last two dims (H, W) of x, and level l gets scale w_l: w_0 the finest
+    (highest-frequency) level, w_{N-1} the coarsest, diffusers' order ([10.0, 5.0] is its default); 1 <= N <= 5.
+    Accepted forms: a list or a tuple of N numbers or one-element tensors, or a 1-D tensor of N values (shared by the
+    batch), or a [B, N] tensor with one row per sample. Numbers are rounded to fp32 once when the wrapper is built.
+    A contiguous fp32 [B, N] tensor on x's device is read in place (a capture() replay sees values written into it);
+    any other tensor form is converted on the device once per (tensor, version, device, B), so in-place writes to it
+    take effect at the next evaluation. The host never reads a tensor's values. guidance_scale must stay at its default (fdg_scales replaces it); both halves are
+    always combined, whatever the scales. The combine runs in the network's raw output space, as cfg_zero_star and tcfg
+    do; every conversion is a per-sample affine map shared by both halves and the operator is linear in c - u, so the
+    space does not change the result in exact arithmetic.
+    Planes: every non-batch index other than the last two names one plane, so x needs at least 4 dims; H and W must each
+    be divisible by 2^(N-1) with a quotient of at least 3, and H*W at most 16384 (128 x 128: SD 1.x/2.x latents are
+    64 x 64, SDXL / SD3-size latents 128 x 128); the library states the rule once (dpm_fdg_supported). Violations raise
+    ValueError against x before the network runs.
+    Definition, per plane and sample, fp32 with each product rounded, sums left to right, no contraction, and
+    delta_l = fl32(w_l - w_{l-1}):
+        d = c - u;  G_0 = d;  G_{l+1} = Down(G_l)                        (l < N-1)
+        E_{N-1} = delta_{N-1}*G_{N-1};  E_l = delta_l*G_l + Up(E_{l+1})  (l = N-2 .. 1)
+        g = (u + w_0*d) + Up(E_1)   (N >= 2);   g = u + w_0*d   (N == 1)
+    Down (n even -> n/2): out[i] = sum_k h_k*a[R(2i-2+k)], h = [1, 5, 10, 10, 5, 1]/32. Up (m -> 2m):
+    out[2i] = (1*a[R(i-2)] + 21*a[R(i-1)] + 35*a[R(i)] + 7*a[R(i+1)])/64, out[2i+1] = (7*a[R(i-1)] + 35*a[R(i)] +
+    21*a[R(i+1)] + 1*a[R(i+2)])/64, with the exact fp32 weights; R reflects without repeating the edge (R(j) = -j for
+    j < 0, 2(n-1) - j for j > n-1). In 2-D both filters run along W on every row first, then along H. Down is the 5 x 5
+    binomial blur with reflect borders followed by half-pixel bilinear 1/2 (kornia's pyrdown, as diffusers' guider uses
+    it); Up is bilinear x2 followed by the blur in the interior and reflects on the coarse grid at the borders. In exact
+    arithmetic this is diffusers' per-level form u_l + w_l*(c_l - u_l) on the pyramids of c and u, reconstructed; it
+    needs one pyramid, of d only. Bit agreement with kornia is not claimed.
+    g is stored in the network's output dtype and then converted by the parameterisation as a single output, so the
+    update runs on the packet step kernels of that dtype pair. For 16-bit networks this rounds g once more, the size of
+    the network output's own rounding. Consequences: N == 1 is the CFG combine u + w*(c - u) op for op (a noise network
+    with fp32 outputs and w != 1 gives the plain CFG run bit for bit; at w == 1 plain CFG bypasses to c and this does
+    not); equal scales give the N == 1 value (up to the sign of a zero); a condition-blind network (c == u) gives g = u,
+    the unguided run, in every state dtype. Cost per guided evaluation: one pyramid launch (c and u read once, g written
+    once), then the one-output step.
+    Accepted: shared or [B, N] scales, every model type and schedule (VP discrete, linear and cosine, flow, EDM), both
+    algorithms, singlestep, multistep, singlestep_fixed and adaptive (host or device controller), dynamic thresholding,
+    correcting_x0_fn / correcting_xt_fn, denoise_to_zero, inverse(), return_intermediate, capture(), batch sharding (per
+    plane: no collective; split [B, N] scales like the batch) and UniPC. A direct call of this callable returns the
+    converted FDG value. Not available (ValueError before any launch and any network call): other guidance types, no
+    unconditional_condition, several conditions, guidance_mask, guidance_rescale != 0, apg_eta, cfg_zero_star, cfg_pp,
+    tcfg, a guidance_scale other than the default (a per-sample one included: use [B, N] fdg_scales), N outside 1..5, a
+    [B, N] tensor whose B does not match x, an x the size rule refuses and DPM_Solver(reference_rounding=True).
+    Not offered: diffusers' per-level parallel_weights (APG-style projection), per-level guidance rescale, a guidance
+    interval."""
     assert model_type in ["noise", "x_start", "v", "score", "flow", "edm"]
     assert guidance_type in ["uncond", "classifier", "classifier-free"]
     flow_schedule = getattr(noise_schedule, "schedule", None) == "flow"
@@ -699,6 +825,29 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
             raise ValueError("tcfg is not available with cfg_zero_star")
         if cfg_pp:
             raise ValueError("tcfg is not available with cfg_pp")
+    if fdg_scales is not None:
+        if guidance_type != "classifier-free" or unconditional_condition is None:
+            raise ValueError("fdg_scales needs guidance_type='classifier-free' and an unconditional_condition")
+        if isinstance(condition, (list, tuple)) and len(condition) >= 2:
+            raise ValueError("fdg_scales is not available with several conditions")
+        if guidance_mask is not None:
+            raise ValueError("fdg_scales is not available with guidance_mask")
+        if guidance_rescale != 0:
+            raise ValueError("fdg_scales is not available with guidance_rescale")
+        if apg_eta is not None:
+            raise ValueError("fdg_scales is not available with adaptive projected guidance (apg_eta)")
+        if cfg_zero_star:
+            raise ValueError("fdg_scales is not available with cfg_zero_star")
+        if cfg_pp:
+            raise ValueError("fdg_scales is not available with cfg_pp")
+        if tcfg:
+            raise ValueError("fdg_scales is not available with tcfg")
+        if torch.is_tensor(guidance_scale) and guidance_scale.numel() != 1:
+            raise ValueError("fdg_scales replaces guidance_scale: give per-sample scales as a [B, N] fdg_scales tensor")
+        if torch.is_tensor(guidance_scale) or guidance_scale != 1.:
+            raise ValueError("fdg_scales replaces guidance_scale, which must stay at its default 1.0, got {!r}".format(
+                guidance_scale))
+        _fdg_scales(fdg_scales)                       # (the form and the number of levels)
     if guidance_mask is not None:
         condition, guidance_scale, guidance_mask = _masked_arguments(
             guidance_type, condition, unconditional_condition, guidance_scale, guidance_mask, guidance_rescale,
@@ -715,7 +864,7 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     return WrappedModel(model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                         unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale,
                         apg_eta, apg_norm_threshold, apg_momentum, cfg_zero_star, cfg_zero_init_steps, cfg_pp,
-                        guidance_mask, tcfg)
+                        guidance_mask, tcfg, fdg_scales)
 
 
 def _masked_arguments(guidance_type, condition, unconditional_condition, guidance_scale, guidance_mask,
@@ -829,6 +978,8 @@ class DPM_Solver:
             raise ValueError("cfg_zero_star is not available with reference_rounding=True")
         if self.reference_rounding and getattr(model_fn, "tcfg", False):
             raise ValueError("tcfg is not available with reference_rounding=True")
+        if self.reference_rounding and getattr(model_fn, "fdg_levels", 0):
+            raise ValueError("fdg_scales is not available with reference_rounding=True")
         if getattr(model_fn, "cfg_pp", False):
             if algorithm_type != "dpmsolver++":
                 raise ValueError("cfg_pp needs algorithm_type='dpmsolver++' (CFG++ re-noises a data prediction)")
@@ -1097,6 +1248,12 @@ class DPM_Solver:
         `slot` names a step of a CACHED coefficient plan (sample() loops): its launch descriptor is frozen after
         the first run (ops.PreparedStep) and later runs only patch tensor pointers -- the steady-state host path."""
         be = ops.backend()
+        fdg = raw.fdg is not None
+        if fdg:
+            # frequency-decoupled guidance: the pyramid pass over both raw halves (+1 launch) gives g in the network's
+            # dtype, handed on as one network output of the same parameterisation; everything below is the one-output
+            # path (the fused step with out / out2, the quantile, UniPC, device coefficients)
+            raw = _fdg_output(be, raw)
         pkey = None
         if slot is not None and self._prep_on:
             # (phi is part of the key: a rescaled evaluation is never served by a launch frozen without the rescale)
@@ -1106,7 +1263,7 @@ class DPM_Solver:
             # (and so is dynamic thresholding: a launch frozen without the clamp never serves a solver switched to it)
             pkey = (slot, raw.param, raw.guidance, raw.phi, raw.guidance_b is None, raw.e_uncond is None,
                     raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, raw.scales, self._dynamic_thresholding,
-                    raw.apg, raw.cfgzero, raw.cfgpp, raw.tcfg)
+                    raw.apg, raw.cfgzero, raw.cfgpp, raw.tcfg, fdg)
             prep = self._prep_cache.get(pkey)
             if prep is not None:
                 r = prep.launch((x, xe, raw.e_cond, m1, m2, raw.e_cond, raw.e_uncond))
@@ -1281,6 +1438,12 @@ class DPM_Solver:
 
     _apg_materialise = False     # UniPC: its launch takes one network output, so an APG or CFG-Zero* value is
                                  # materialised first
+
+    def _check_fdg(self, x) -> None:
+        """Frequency-decoupled guidance: x's shape against the size rule and the per-sample rows, before any launch."""
+        w = self._wrapped
+        if isinstance(w, WrappedModel) and w.fdg_levels:
+            w.fdg_args(x)
 
     def _cfgpp_step(self, raw: RawOutput, xe, alsig, co: P.Coeffs, x, m1, want_m: bool, dup_out: bool):
         """A CFG++ update (dpm_step_cfgpp, one launch): returns (U, x_next), U the x0 of the unconditional output alone,
@@ -1813,6 +1976,7 @@ class DPM_Solver:
         if method == 'adaptive' and self._apg_momentum() != 0:
             raise ValueError("apg_momentum != 0 is not available with method='adaptive': its evaluations, the device "
                              "controller's surplus iterations included, define no momentum sequence")
+        self._check_fdg(x)
         device = x.device
         intermediates = []
         ns = self.noise_schedule

@@ -66,6 +66,9 @@ TCFG (model_wrapper's tcfg) runs with a scalar scale, as CFG-Zero* does: per eva
 one launch that materialises the guided raw output g = us + w*(c - us), us = wu*u + wc*c, in fp32, then the UniPC
 launch converting g as a single network output at its own state.
 
+Frequency-decoupled guidance (model_wrapper's fdg_scales), shared or per-sample [B, N] scales: per evaluation the
+pyramid pass (1 launch) gives g in the network's dtype, then the UniPC launch converts g as a single network output.
+
 Not available (ValueError before any launch): per-sample guidance scales, several conditions, guidance masks,
 guidance rescale, reference_rounding, plan_broadcast, orders outside 1..3, steps < order.
 """
@@ -152,6 +155,7 @@ class UniPC(DPM_Solver):
         t_T = self.noise_schedule.T if t_start is None else t_start
         assert t_0 > 0 and t_T > 0, "Time range needs to be greater than 0. For discrete-time DPMs, it needs to be in [1 / N, 1], where N is the length of betas array"
         self._check_supported(steps, order)
+        self._check_fdg(x)
         ns, device, hook = self.noise_schedule, x.device, self.correcting_xt_fn
         intermediates = []
         self._xin_pair = None

@@ -28,8 +28,9 @@
 extern "C" {
 #endif
 
-#define DPM_B200_VERSION 108 /* 0.1.8: CFG++ (dpm_step_cfgpp); regional guidance (dpm_step_multi_masked) and TCFG
-                                (dpm_tcfg_words, dpm_step_tcfg) are additions to this ABI: test for their symbols */
+#define DPM_B200_VERSION 108 /* 0.1.8: CFG++ (dpm_step_cfgpp); regional guidance (dpm_step_multi_masked), TCFG
+                                (dpm_tcfg_words, dpm_step_tcfg) and frequency-decoupled guidance (dpm_fdg_supported,
+                                dpm_fdg_guided) are additions to this ABI: test for their symbols */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -399,6 +400,40 @@ DPM_API int dpm_tcfg_words(float* w_out, const void* e_cond, const void* e_uncon
                            uint64_t per_sample, uint64_t n, void* workspace, size_t workspace_bytes,
                            dpm_stream_t stream);
 DPM_API int dpm_step_tcfg(const dpm_step_desc* desc, const float* words, const float* guidance, dpm_stream_t stream);
+
+/* ---- frequency-decoupled guidance (S. Sadat, T. Vontobel, F. Salehi and R. M. Weber, "Guidance in the Frequency
+ * Domain Enables High-Fidelity Sampling at Low CFG Scales", 2025) ----------------------------------------------------
+ * Classifier-free guidance with one scale per level of a Laplacian pyramid, in the network's raw output space. Per
+ * plane (the last two dims, H x W, of one sample and one index of the other non-batch dims), N = levels scales
+ * w_0 (finest) .. w_{N-1} (coarsest), delta_l = fl32(w_l - w_{l-1}), every op fp32, each product rounded, no
+ * contraction:
+ *   d = c - u;  G_0 = d;  G_{l+1} = Down(G_l)  (l < N-1)
+ *   E_{N-1} = delta_{N-1}*G_{N-1};  E_l = delta_l*G_l + Up(E_{l+1})  (l = N-2 .. 1)
+ *   g = (u + w_0*d) + Up(E_1)  (N >= 2);  g = u + w_0*d  (N == 1);  stored rounded to model_dtype
+ * Filters are 1-D, applied to every row (along W) first, then to every column; R(j) = -j for j < 0, 2(n-1) - j for
+ * j > n-1 (reflect without repeating the edge); each term fl(weight*a) with the exact fp32 weights, summed left to right:
+ *   Down, n (even) -> n/2:  out[i] = sum_{k=0..5} h_k*a[R(2i-2+k)],  h = [1, 5, 10, 10, 5, 1]/32
+ *   Up, m -> 2m:  out[2i]   = (1*a[R(i-2)] + 21*a[R(i-1)] + 35*a[R(i)] + 7*a[R(i+1)])/64
+ *                 out[2i+1] = (7*a[R(i-1)] + 35*a[R(i)] + 21*a[R(i+1)] + 1*a[R(i+2)])/64
+ * This is the per-level form u_l + w_l*(c_l - u_l) of the Laplacian pyramids of c and u, reconstructed, in exact
+ * arithmetic; it needs one pyramid, of d only.
+ * dpm_fdg_supported: DPM_OK when a plane of H x W with `levels` levels is served, else DPM_ERR_ARG with the reason in
+ *   dpm_last_error(): 1 <= levels <= DPM_FDG_MAX_LEVELS, H and W divisible by 2^(levels-1) with a quotient of at
+ *   least 3, H*W <= DPM_FDG_MAX_PLANE. The size rule lives here only.
+ * dpm_fdg_guided: g_out <- g for `planes` planes. Plane p is sample s = p / planes_per_sample, index q = p %
+ *   planes_per_sample; its element (h, w) is at s*sample_stride + q*plane_stride + h*h_stride + w*w_stride (elements,
+ *   the same for g_out, e_cond and e_uncond). scales: scale_stride == 0 -> `levels` shared scales in HOST memory, passed
+ *   by value; else per-sample scales in device memory, sample s's at scales[s*scale_stride .. + levels). One launch,
+ *   one CTA per plane, every level in shared memory: reads c and u once and writes g once (3*s_model bytes per
+ *   element). Dense row-major planes with 16-byte aligned bases take 128-bit accesses; any other strides give the same
+ *   bits. Does not synchronise or allocate. */
+#define DPM_FDG_MAX_LEVELS 5
+#define DPM_FDG_MAX_PLANE 16384   /* H*W: 128 x 128 */
+DPM_API int dpm_fdg_supported(uint64_t H, uint64_t W, int levels, int model_dtype);
+DPM_API int dpm_fdg_guided(void* g_out, const void* e_cond, const void* e_uncond, int model_dtype, uint64_t planes,
+                           uint64_t H, uint64_t W, int64_t sample_stride, int64_t plane_stride, int64_t h_stride,
+                           int64_t w_stride, int levels, const float* scales, uint64_t scale_stride,
+                           uint64_t planes_per_sample, dpm_stream_t stream);
 
 /* ---- CFG++ (Chung, Kim, Park, Nam and Ye, "CFG++: Manifold-constrained Classifier Free Guidance for Diffusion
  * Models", ICLR 2025, arXiv:2406.08070) -------------------------------------------------------------------------------
