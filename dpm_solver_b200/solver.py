@@ -192,14 +192,17 @@ def _apg_args(be, raw: RawOutput, xe, marg, sdtype, x0: bool, ns, coef_dev=None,
 def _fdg_scales(fdg_scales):
     """model_wrapper's fdg_scales -> (levels, shared, tensor): the N shared scales as python floats, each rounded to
     fp32 once (a list or tuple of numbers), or None and the tensor `WrappedModel.fdg_args` converts once per (tensor,
-    version, device, B) or reads in place (a 1-D tensor, a [B, N] tensor, or a list or tuple holding tensors, which are
-    stacked on their device). The host never reads a tensor's values."""
+    version, device, B) or reads in place (a 1-D tensor, a [B, N] tensor, or a list or tuple holding tensors, kept as a
+    tuple and stacked on their device). The host never reads a tensor's values."""
     s = fdg_scales
     if isinstance(s, (list, tuple)) and any(torch.is_tensor(v) for v in s):
         if any(not torch.is_tensor(v) or v.numel() != 1 for v in s) or len({v.device for v in s}) != 1:
             raise ValueError("fdg_scales as a list or tuple of tensors takes N one-element tensors on one device")
-        s = torch.stack([v.detach().reshape(()) for v in s])
-    if torch.is_tensor(s):
+        if any(v.is_complex() for v in s):
+            raise ValueError("fdg_scales must be real, got {}".format(next(v.dtype for v in s if v.is_complex())))
+        # the tensors themselves, not a stacked copy: fdg_args restacks them after an in-place write to any of them
+        levels, shared, s = len(s), False, tuple(s)
+    elif torch.is_tensor(s):
         if s.dim() not in (1, 2):
             raise ValueError("fdg_scales must be a list, a tuple, a 1-D tensor of N scales or a [B, N] tensor, got "
                              "shape {}".format(tuple(s.shape)))
@@ -371,15 +374,17 @@ class WrappedModel:
         if self._fdg_shared is not None:
             return self._fdg_shared, L
         s, B = self._fdg_vec, x.shape[0]
-        if s.dim() == 2:
+        listed = isinstance(s, tuple)            # N one-element tensors
+        if not listed and s.dim() == 2:
             if s.shape[0] != B:
                 raise ValueError("fdg_scales has {} rows for a batch of {}".format(s.shape[0], B))
             if s.device == x.device and s.dtype == torch.float32 and s.is_contiguous():
                 return s, L
-        key = (id(s), s._version, str(x.device), B)
+        key = (tuple((id(v), v._version) for v in (s if listed else (s,))), str(x.device), B)
         if self._fdg_dev is None or self._fdg_dev[0] != key:
             # the source is kept alive next to the key so that its id cannot be recycled
-            v = s.detach().to(device=x.device, dtype=torch.float32)
+            v = torch.stack([t.detach().reshape(()) for t in s]) if listed else s.detach()
+            v = v.to(device=x.device, dtype=torch.float32)
             self._fdg_dev = (key, v.expand(B, L).contiguous(), s)
         return self._fdg_dev[1], L
 

@@ -1,6 +1,7 @@
-"""Random CFG-Zero*, CFG++ and regional-guidance `sample()` configurations for the end-to-end tests on the device
-(tests/test_gpu_guidance_random_configs.py) and their CPU side (tests/test_guidance_draws_vs_reference.py): the draw
-(apg_configs.draw_apg's base, one feature per configuration), a `GuidanceRig` and the CPU oracle.
+"""Random CFG-Zero*, CFG++, regional-guidance, TCFG and frequency-decoupled-guidance `sample()` configurations for the
+end-to-end tests on the device (tests/test_gpu_guidance_random_configs.py) and their CPU side
+(tests/test_guidance_draws_vs_reference.py): the draw (apg_configs.draw_apg's base, one feature per configuration), a
+`GuidanceRig` and the CPU oracle.
 
 The base is draw_apg's: VP, flow and EDM schedules, 35 to 16384 elements per sample (some not multiples of 8), B from 1
 to 4, a channels_last x_T, a network whose outputs keep their input's layout or are channels_last or row-major, 16-bit
@@ -12,13 +13,23 @@ state and model dtypes, inverse(), denoise_to_zero, t_start / t_end, skip types 
   * mask: K = 1..4 conditions, each with a mask of one of MASK_KINDS, held as fp32 (read in place when canonical),
     channels_last, bf16 or on the CPU (converted); values 0, negatives and quarters. UniPC is drawn now and then and
     must be refused.
+  * tcfg: one scale from {1 (the bypass), 3.5, 7.5}, a one-element tensor scale, or per-sample scales with rows at 1;
+    DPM_Solver (every method) or UniPC; thresholding now and then (both materialise g in fp32 before the step).
+  * fdg: planes that reach each CTA shape of k_fdg_guided, its shared-memory opt-in and its scalar loads (FDG_PLANES),
+    or the base's shape; `levels` from what the plane admits, and now and then one level more, which the size rule
+    refuses; the scales as N floats, N one-element tensors, a 1-D tensor, an fp32 [B, N] tensor read in place, a bf16
+    or CPU [B, N] tensor (converted), or a [B + 1, N] tensor (refused); now and then equal scales, whose run must be
+    the N == 1 run.
 
 The oracle of a configuration, on CPU tensors:
-  * the product's host logic on the numpy executor `MaskOracle(exact=True)` (which is also the CFG++, CFG-Zero* and APG
-    executor): y, every intermediate and the trace of network calls -- what the device must give bit for bit;
+  * the product's host logic on the numpy executor -- `MaskOracle(exact=True)` (which is also the CFG++, CFG-Zero* and
+    APG executor), or for tcfg and fdg `FDGOracle()` (TCFG's words in the device's summation order): y, every
+    intermediate and the trace of network calls -- what the device must give bit for bit;
   * where the unmodified reference can express the configuration, the executor against it with as many network calls:
-    cfgzero bit for bit through cfgzero_oracle.guided_net, cfgpp within CFGPP_TOL of cfgpp_oracle.cfgpp_fp64, mask bit
-    for bit against test_cfg_mask.reference_composed;
+    cfgzero, tcfg and fdg bit for bit through cfgzero_oracle / tcfg_oracle / fdg_oracle.guided_net behind a
+    guidance_type="uncond" wrapper, cfgpp within CFGPP_TOL of cfgpp_oracle.cfgpp_fp64 (plus, for an x_start network,
+    the rounding bound of its x0 conversion: _reference_cfgpp), mask bit for bit against
+    test_cfg_mask.reference_composed;
   * a configuration the product refuses is {"error": exception}.
 """
 import contextlib
@@ -30,16 +41,23 @@ import torch
 
 from apg_configs import APGRig, draw_apg, per_sample, reference_schedule
 from cfg_mask_oracle import MaskOracle
+from fdg_oracle import FDGOracle
 from gpu_configs import backend, really_channels_last, rel_err, same_bits, sample_kwargs
 
-FEATURES = ("cfgzero", "cfgpp", "mask")
+FEATURES = ("cfgzero", "cfgpp", "mask", "tcfg", "fdg")
 BEYOND = 1000                 # a cfg_zero_init_steps above any run's number of evaluations: every evaluation is 0
 CFGPP_TOL = 1e-5              # tests/test_cfg_pp.py's bound against the fp64 transcription
+XSTART_ROUNDING = 3           # x_start under CFG++: multiples of what its fp32 x0 conversion alone moves a run
 MASK_KINDS = ("hw", "11hw", "b1hw", "b111", "bchw", "chw", "bc11", "none")
 MASK_FORMS = ("f32", "f32", "cl", "bf16", "cpu")
 VP = ("sd", "ddpm_linear", "vp_linear")
 CFGPP_REFUSALS =("dpmsolver", "order3", "singlestep", "adaptive", "unipc", "thresholding")
-CHUNKS, PER_CHUNK, SEED = 6, 20, 9900     # the device test: 6 chunks of 20 configurations
+# k_fdg_guided's paths: 64 x 64 (CTA shape 0, 5 levels), 72 x 64 (shape 1), 64 x 128 (shape 1 past 48 KiB of shared
+# memory), 126 x 130 (shape 2, H*W % 8 != 0: scalar loads), 6 x 6 (the smallest plane with 2 levels), 24 x 40
+FDG_PLANES = [(4, 64, 64), (3, 72, 64), (2, 64, 128), (1, 126, 130), (2, 6, 6), (3, 24, 40)]
+FDG_FORMS = ("floats", "listed", "vec", "rows", "rows", "bf16", "cpu")     # (+ "bad_rows" now and then: refused)
+FDG_VALUES = [7.0, 3.5, 1.5, 1.0, 0.0, -1.0, 10.0, 2.5]                  # (exact in bf16)
+CHUNKS, PER_CHUNK, SEED = 10, 20, 9900    # the device test: 10 chunks of 20 configurations
 
 
 def draw_guidance(rng):
@@ -48,7 +66,9 @@ def draw_guidance(rng):
     f = c["feature"] = rng.choice(FEATURES)
     B = c["B"]
     c["zero_init"], c["K"], c["masks"], c["cfgpp_refusal"] = 0, 0, None, None
-    if c["schedule"] in ("flow", "edm") and rng.random() < {"cfgzero": 0.25, "cfgpp": 0.25, "mask": 0.5}[f]:
+    c["fdg_levels"], c["fdg_form"], c["fdg_w"], c["fdg_equal"] = 0, None, None, False
+    if c["schedule"] in ("flow", "edm") and rng.random() < {"cfgzero": 0.25, "cfgpp": 0.25, "mask": 0.5, "tcfg": 0.25,
+                                                             "fdg": 0.25}[f]:
         c.update(schedule=rng.choice(VP), model_type=rng.choice(["noise", "x_start", "v", "score"]))
     if f in ("cfgzero", "cfgpp"):
         ones = [1.0, 3.5, 7.5] if f == "cfgzero" else [0.2, 0.6, 1.0, 7.5]
@@ -65,6 +85,23 @@ def draw_guidance(rng):
             c.update(guidance="float", cfg=7.5, scales=None)             # (UniPC refuses per-sample scales)
         if c["sampler"] == "dpm" and c["method"] == "adaptive" and c["zero_init"] and rng.random() < 0.6:
             c["zero_init"] = 0                                           # (refused; keep most adaptive draws)
+    elif f == "tcfg":
+        g = rng.random()
+        if g < 0.35:
+            rows = [rng.choice([7.5, 1.0, 3.5]) for _ in range(B)]
+            if B > 1 and 1.0 not in rows:
+                rows[rng.randrange(B)] = 1.0
+            c.update(guidance="per_sample", cfg=None, scales=rows)
+        elif g < 0.55:
+            c.update(guidance="tensor0", cfg=rng.choice([1.0, 3.5, 7.5]), scales=None)
+        else:
+            c.update(guidance="float", cfg=rng.choice([1.0, 3.5, 7.5]), scales=None)
+        if c["sampler"] == "unipc" and c["guidance"] == "per_sample" and rng.random() < 0.7:
+            c.update(guidance="float", cfg=7.5, scales=None)             # (UniPC refuses per-sample scales)
+        if c["algo"] == "dpmsolver++" and rng.random() < 0.15:
+            c["thresholding"] = True
+    elif f == "fdg":
+        draw_fdg(rng, c)
     elif f == "cfgpp":
         c.update(sampler="dpm", method="multistep", order=rng.choice([1, 2]), algo="dpmsolver++", thresholding=False,
                  reference_rounding=False, steps=max(c["steps"], 3))
@@ -86,6 +123,66 @@ def draw_guidance(rng):
         c["masks"] = [(rng.choice(MASK_KINDS), rng.choice(MASK_FORMS)) for _ in range(K)]
         c.update(guidance="multi", cfg=None, scales=[rng.choice([7.5, -2.0, 0.0, 1.5, 3.0, 1.0]) for _ in range(K)])
     return c
+
+
+def fdg_max_levels(shape):
+    """The most levels the size rule admits for the plane of `shape` (H and W divisible by 2^(levels-1), quotients of
+    at least 3, at most 5 levels)."""
+    H, W = shape[-2:]
+    L = 1
+    while L < 5 and H % (2 << (L - 1)) == 0 and W % (2 << (L - 1)) == 0 and H >> L >= 3 and W >> L >= 3:
+        L += 1
+    return L
+
+
+def draw_fdg(rng, c):
+    """The fdg part of a draw: the plane, the layouts on it, the levels and the scales."""
+    if not c["thresholding"] or rng.random() < 0.5:
+        c["shape"] = rng.choice(FDG_PLANES + [(2, 3, 6, 4), c["shape"]])
+    c["steps"] = min(c["steps"], 12)
+    three = len(c["shape"]) == 3
+    c["x_channels_last"] = three and rng.random() < 0.3
+    c["net_layout"] = rng.choice(["keep", "keep", "cl", "row"]) if three else "keep"
+    c["channels_last"] = c["net_layout"] == "cl"
+    c["x2_channels_last"] = three and not c["channels_last"] and rng.random() < 0.15
+    c.update(guidance="fdg", cfg=None, scales=None)
+    mx = fdg_max_levels(c["shape"])
+    L = c["fdg_levels"] = mx + 1 if rng.random() < 0.1 else rng.choice([1, mx, mx] + list(range(1, mx + 1)))
+    c["fdg_form"] = "bad_rows" if rng.random() < 0.05 else rng.choice(FDG_FORMS)
+    c["fdg_equal"] = rng.random() < 0.15
+    rows = []
+    for _ in range(c["B"] if c["fdg_form"] not in ("floats", "listed", "vec") else 1):
+        rows.append([rng.choice(FDG_VALUES)] * L if c["fdg_equal"] else [rng.choice(FDG_VALUES) for _ in range(L)])
+    c["fdg_w"] = rows * c["B"] if len(rows) == 1 else rows
+
+
+def make_fdg_scales(c, device):
+    """The configuration's fdg_scales in its form: N floats, N one-element tensors, a 1-D tensor, an fp32 [B, N]
+    tensor on `device` (read in place there), a bf16 one on `device` or an fp32 one on the CPU (both converted), or an
+    fp32 [B + 1, N] tensor."""
+    rows, form = c["fdg_w"], c["fdg_form"]
+    if form == "floats":
+        return list(rows[0])
+    if form == "listed":
+        return [torch.tensor([v], device=device) for v in rows[0]]
+    if form == "vec":
+        return torch.tensor(rows[0], device=device)
+    if form == "bad_rows":
+        rows = rows + rows[:1]
+    t = torch.tensor(rows, dtype=torch.float32)
+    return t if form == "cpu" else t.to(device=device, dtype=torch.bfloat16 if form == "bf16" else torch.float32)
+
+
+def fdg_values(c):
+    """The scales as the kernel reads them: N python floats (the shared forms) or an fp32 [B, N] CPU tensor."""
+    if c["fdg_form"] in ("floats", "listed", "vec"):
+        return list(c["fdg_w"][0])
+    return torch.tensor(c["fdg_w"], dtype=torch.float32)
+
+
+def executor(c):
+    """The numpy executor of `c`: FDGOracle (which also runs TCFG) for tcfg and fdg, MaskOracle(exact=True) else."""
+    return FDGOracle() if c["feature"] in ("tcfg", "fdg") else MaskOracle(exact=True)
 
 
 def mask_shape(kind, B, shape):
@@ -115,15 +212,21 @@ def make_masks(c, device):
 
 
 class GuidanceRig(APGRig):
-    """APGRig with CFG-Zero*, CFG++ or regional guidance in model_wrapper. `masks` replaces the drawn masks."""
+    """APGRig with CFG-Zero*, CFG++, regional guidance, TCFG or frequency-decoupled guidance in model_wrapper. `masks`
+    replaces the drawn masks, `fdg` the drawn fdg_scales."""
 
-    def __init__(self, mod, c, device="cpu", masks=None):
+    def __init__(self, mod, c, device="cpu", masks=None, fdg=None):
         super().__init__(mod, dict(c, guidance="none"), device)
         self.c = c
         B, dev = c["B"], self.device
         kw = dict(model_type=c["model_type"], guidance_type="classifier-free",
                   unconditional_condition=torch.zeros(B, 1, device=dev))
-        self.masks = None
+        self.masks = self.fdg = None
+        if c["feature"] == "fdg":
+            self.fdg = make_fdg_scales(c, dev) if fdg is None else fdg
+            self.fn = mod.model_wrapper(self.net, self.ns, condition=torch.ones(B, 1, device=dev), fdg_scales=self.fdg,
+                                        **kw)
+            return
         if c["feature"] == "mask":
             self.masks = make_masks(c, dev) if masks is None else masks
             cond = [torch.full((B, 1), float(k + 1), device=dev) for k in range(c["K"])]
@@ -133,9 +236,13 @@ class GuidanceRig(APGRig):
         scale = c["cfg"]
         if c["guidance"] == "per_sample":
             scale = torch.tensor(c["scales"], dtype=torch.float32, device=dev)
+        elif c["guidance"] == "tensor0":
+            scale = torch.tensor(c["cfg"])
         self.scale = scale
         if c["feature"] == "cfgzero":
             kw.update(cfg_zero_star=True, cfg_zero_init_steps=c["zero_init"])
+        elif c["feature"] == "tcfg":
+            kw["tcfg"] = True
         else:
             kw["cfg_pp"] = True
         self.fn = mod.model_wrapper(self.net, self.ns, condition=torch.ones(B, 1, device=dev), guidance_scale=scale,
@@ -147,15 +254,18 @@ def refused(c):
     if c["schedule"] == "flow" and c["model_type"] in ("v", "score"):
         return True
     if c["reference_rounding"]:
-        return True          # (UniPC refuses it, and DPM_Solver does with each of the three features)
+        return True          # (UniPC refuses it, and DPM_Solver does with each of the five features)
     unipc = c["sampler"] == "unipc"
     if unipc and c["steps"] < c["order"]:
         return True
     f = c["feature"]
-    if f == "cfgzero":
+    if f == "fdg":
+        # (the size rule, more than 5 levels, and a [B', N] tensor for a batch of B)
+        return c["fdg_levels"] > fdg_max_levels(c["shape"]) or c["fdg_form"] == "bad_rows"
+    if f in ("cfgzero", "tcfg"):
         if unipc:
             return c["guidance"] == "per_sample" and c["B"] > 1
-        return c["method"] == "adaptive" and c["zero_init"] > 0
+        return f == "cfgzero" and c["method"] == "adaptive" and c["zero_init"] > 0
     if f == "cfgpp":
         return (unipc or c["algo"] != "dpmsolver++" or c["method"] != "multistep" or c["order"] not in (1, 2)
                 or c["thresholding"])
@@ -169,27 +279,42 @@ def _fp32(c):
 
 
 def reference_expressible(c):
-    """cfgzero: fp32 DPM_Solver, not adaptive, a network the reference's wrappers take on its schedule; cfgpp: fp32, a
-    network with a closed-form x0, no denoise_to_zero; mask: fp32 DPM_Solver on a VP schedule, not adaptive. Never
-    inverse()."""
+    """cfgzero, tcfg and fdg: fp32 DPM_Solver, not adaptive, a network the reference's wrappers take on its schedule;
+    cfgpp: fp32, a network with a closed-form x0, no denoise_to_zero; mask: fp32 DPM_Solver on a VP schedule, not
+    adaptive. Never inverse()."""
     if refused(c) or not _fp32(c) or c["inverse"] or c["sampler"] != "dpm" or c["method"] == "adaptive":
         return False
     sched, mt = c["schedule"], c["model_type"]
-    if c["feature"] == "cfgzero":
+    if c["feature"] in ("cfgzero", "tcfg", "fdg"):
         return mt == sched if sched in ("flow", "edm") else mt in ("noise", "x_start", "v", "score")
     if c["feature"] == "cfgpp":
         return mt in ("noise", "x_start", "v", "score", "flow") and sched != "edm" and not c["denoise_to_zero"]
     return sched not in ("flow", "edm") and mt in ("noise", "x_start", "v", "score")
 
 
-def _reference_cfgzero(c, rig, x):
+def _guided_net(c, rig):
+    """A network for the reference's guidance_type="uncond" wrapper that returns the guided output of rig.net."""
+    B = c["B"]
+    uc, cond = torch.zeros(B, 1), torch.ones(B, 1)
+    if c["feature"] == "fdg":
+        import fdg_oracle
+        return fdg_oracle.guided_net(rig.net, uc, cond, fdg_values(c))
+    # (one scale as per-sample scales: a scale of 1 then gives out_c itself, as the product's bypass does, not
+    # us + 1*(out_c - us))
+    w = torch.tensor(c["scales"] or [c["cfg"]] * B, dtype=torch.float32)
+    if c["feature"] == "tcfg":
+        import tcfg_oracle
+        return tcfg_oracle.guided_net(rig.net, uc, cond, w)
     from cfgzero_oracle import guided_net
+    return guided_net(rig.net, uc, cond, w, c["zero_init"])
+
+
+def _reference_uncond(c, rig, x):
+    """The reference driving _guided_net(c, rig) through guidance_type="uncond" (cfgzero, tcfg, fdg)."""
     from gpu_configs import reference
     ref = reference()
-    B = c["B"]
-    w = c["cfg"] if c["guidance"] == "float" else torch.tensor(c["scales"], dtype=torch.float32)
     rns = reference_schedule(c)
-    g = guided_net(rig.net, torch.zeros(B, 1), torch.ones(B, 1), w, c["zero_init"])
+    g = _guided_net(c, rig)
     thr = c["thresholding"]
     if c["schedule"] in ("flow", "edm"):
         from edm_oracle import reference_solver as edm_solver
@@ -221,8 +346,9 @@ def _reference_mask(c, rig, x):
         return s.sample(x, **sample_kwargs(c)), n[0]
 
 
-def _reference_cfgpp(c, rig, x):
-    """cfgpp_fp64 on the product's grid and fp32 marginals, the network's halves converted to x0 in fp64."""
+def _cfgpp_fp64(c, rig, x, rounded=False):
+    """(y, evaluations): cfgpp_fp64 on the product's grid and fp32 marginals, the network's halves converted to x0 in
+    fp64; `rounded`: an x_start output converted as the product converts it, in fp32 (see _reference_cfgpp)."""
     import dpm_solver_b200 as new
     from cfgpp_oracle import cfgpp_fp64
     from dpm_solver_b200 import plan as P
@@ -237,8 +363,14 @@ def _reference_cfgpp(c, rig, x):
     w = np.float64(c["cfg"]) if c["guidance"] == "float" else \
         np.array(c["scales"], np.float64).reshape((B,) + (1,) * len(c["shape"]))
     n = [0]
+    f32 = np.float32
 
     def x0(out, xx, i):
+        if mt == "x_start" and rounded:
+            # eps = (x - alpha*o)/sigma, then x0 = (x - sigma*eps)/alpha, each op rounded to fp32
+            xf, a, s_ = xx.astype(f32), f32(al[i]), f32(sg[i])
+            e = ((xf - a * out.astype(f32)) / s_).astype(f32)
+            return ((xf - s_ * e) / a).astype(f32).astype(np.float64)
         out = out.astype(np.float64)
         if mt == "noise":
             return (xx - sg[i] * out) / al[i]
@@ -261,10 +393,34 @@ def _reference_cfgpp(c, rig, x):
     return torch.from_numpy(y), n[0]
 
 
+def _reference_cfgpp(c, rig, x):
+    """(y, evaluations, tolerance): _cfgpp_fp64 and the relative distance the product may lie from it.
+
+    That is CFGPP_TOL, plus for an x_start network the rounding of its conversion. The product takes an x_start output
+    o to x0 as the reference's data prediction does: eps = (x - alpha*o)/sigma (:292), then x0 = (x - sigma*eps)/alpha
+    (:439), each op in fp32. x - sigma*eps cancels down to alpha*o, so x0 carries an error of about u*|x|/alpha
+    (u = 2^-24), where the transcription takes x0 = o exactly; the guided x0 carries (1 + 2|w|) times that, and the
+    update after grid point i scales it by alpha_{i+1}. Where alpha_i is small -- a flow schedule starts at
+    alpha_T = 1/N -- this amounts to 1e-4 of the result at a few steps, against 1e-6 for a velocity or noise network.
+    The replay `rounded` measures it on the run itself: the same conversion rounded to fp32, the rest in fp64. The
+    product rounds that conversion, and the state it reads, independently of the replay, so it may lie up to
+    XSTART_ROUNDING times the replay's distance away (at most about twice, over the draws and grids tried)."""
+    y, n = _cfgpp_fp64(c, rig, x)
+    tol = CFGPP_TOL
+    if c["model_type"] == "x_start":
+        tol += XSTART_ROUNDING * rel_err(_cfgpp_fp64(c, rig, x, rounded=True)[0], y)
+    return y, n, tol
+
+
 def reference_run(c, rig):
-    """(y, number of evaluations) of the reference form of `c` on rig's network."""
+    """(y, number of evaluations, tolerance) of the reference form of `c` on rig's network; the tolerance is None where
+    the product must match it bit for bit."""
     x = rig.x()
-    return {"cfgzero": _reference_cfgzero, "cfgpp": _reference_cfgpp, "mask": _reference_mask}[c["feature"]](c, rig, x)
+    if c["feature"] == "cfgpp":
+        return _reference_cfgpp(c, rig, x)
+    run = {"cfgzero": _reference_uncond, "tcfg": _reference_uncond, "fdg": _reference_uncond,
+           "mask": _reference_mask}[c["feature"]]
+    return run(c, rig, x) + (None,)
 
 
 def cpu_oracle(c):
@@ -272,18 +428,22 @@ def cpu_oracle(c):
     compared; {"error": exception} when the product refuses the configuration."""
     import dpm_solver_b200 as new
     out = {}
-    with backend(MaskOracle(exact=True)):
+    with backend(executor(c)):
         try:
             rig = GuidanceRig(new, c)
             out["y"], out["inter"], out["calls"] = rig.sample(rig.solver(), rig.x(), trace=True)
         except (ValueError, AssertionError) as e:
             return {"error": e}
+        if c["fdg_equal"]:
+            # equal scales: the pyramid terms vanish, so the run is the one-level run's bit for bit
+            one = GuidanceRig(new, dict(c, fdg_levels=1, fdg_w=[r[:1] for r in c["fdg_w"]]))
+            assert same_bits(out["y"], one.sample(one.solver(), one.x())[0]), c
         if reference_expressible(c):
-            yr, n = reference_run(c, GuidanceRig(new, c))
+            yr, n, tol = reference_run(c, GuidanceRig(new, c))
             assert len(out["calls"]) == n, (c, len(out["calls"]), n)
-            if c["feature"] == "cfgpp":
+            if tol is not None:
                 out["pinned"] = rel_err(out["y"], yr)
-                assert out["pinned"] <= CFGPP_TOL, (c, out["pinned"])
+                assert out["pinned"] <= tol, (c, out["pinned"], tol)
             else:
                 assert same_bits(out["y"], yr), (c, rel_err(out["y"], yr))
                 out["pinned"] = 0.0
@@ -317,6 +477,8 @@ def tally_static(c):
             keys.append("layout change:row-major outputs of a channels_last state")
     if c["net_layout"] == "cl" and not c["x_channels_last"] and really_channels_last(c):
         keys.append("layout change:channels_last outputs of a row-major state")
+    if f in ("tcfg", "fdg"):
+        keys += [f + ":" + k for k in keys if k.startswith("layout change:")]
     if c["sampler"] == "dpm":
         keys.append("method:" + c["method"])
     if c["inverse"]:
@@ -327,6 +489,27 @@ def tally_static(c):
         keys.append("t_start/t_end")
     if f == "cfgzero":
         keys.append("zero-init:" + {0: "none", BEYOND: "all"}.get(c["zero_init"], "partial"))
+    elif f == "tcfg":
+        bypass = c["guidance"] != "per_sample" and c["cfg"] == 1.0 or c["scales"] == [1.0]
+        if bypass:
+            keys.append("tcfg:bypass")
+        elif c["sampler"] == "unipc" or (c["thresholding"] and c["algo"] == "dpmsolver++"):
+            keys.append("tcfg:materialised")
+        if c["guidance"] == "per_sample" and c["B"] > 1 and 1.0 in c["scales"]:
+            keys.append("tcfg:per-sample row at 1")
+    elif f == "fdg":
+        H, W = c["shape"][-2:]
+        # (g follows the network's outputs: channels_last ones, asked for or kept from a channels_last x, are strided
+        # planes)
+        strided = (x_cl and c["net_layout"] == "keep") or (c["net_layout"] == "cl" and really_channels_last(c))
+        keys += ["fdg:levels=%d" % c["fdg_levels"],
+                 "fdg:scales:" + {"bf16": "converted", "cpu": "converted"}.get(c["fdg_form"], c["fdg_form"])]
+        if (H * W) % 8 or strided:
+            keys.append("fdg:scalar path")
+        if ps // (H * W) > 1:
+            keys.append("fdg:planes>1 per sample")
+        if c["fdg_equal"] and c["fdg_levels"] > 1:
+            keys.append("fdg:equal scales")
     elif f == "cfgpp":
         keys.append("cfgpp:order%d" % c["order"])
         if c["cfg"] == 1.0:
@@ -352,9 +535,14 @@ REQUIRED = (["feature:" + f for f in FEATURES] + ["schedule:vp", "schedule:flow"
              "layout change:row-major outputs of a channels_last state",
              "layout change:channels_last outputs of a row-major state"] +
             ["method:" + m for m in ("multistep", "singlestep", "singlestep_fixed", "adaptive")] +
-            ["inverse", "d2z", "t_start/t_end"])
+            ["inverse", "d2z", "t_start/t_end"] +
+            ["tcfg:bypass", "tcfg:per-sample row at 1", "tcfg:materialised"] +
+            ["fdg:levels=1", "fdg:levels=5", "fdg:scalar path", "fdg:planes>1 per sample", "fdg:equal scales"] +
+            ["fdg:scales:" + k for k in ("floats", "listed", "vec", "rows", "converted")] +
+            [f + ":layout change:" + k for f in ("tcfg", "fdg") for k in ("row-major outputs of a channels_last state",
+                                                                          "channels_last outputs of a row-major state")])
 REQUIRED_ON_DEVICE = ["rejected", "captured", "captured:zero-init", "captured:rewritten-mask", "second_stream",
-                      "pinned"]
+                      "pinned", "fdg:frozen step served", "fdg:frozen step fell back", "captured:fdg rows rewritten"]
 
 
 def configurations(chunk):

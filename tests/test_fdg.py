@@ -449,16 +449,23 @@ def test_size_rule_lives_in_the_library():
 
 
 def test_tensor_scales_are_converted_per_version(fdg_backend):
-    """A 1-D tensor and a list of one-element tensors are read as tensors: an in-place write to the 1-D tensor takes
-    effect at the next run, and both give the run of the same numbers."""
+    """A 1-D tensor and a list of one-element tensors are read as tensors: an in-place write to the 1-D tensor or to
+    any one of the listed tensors takes effect at the next run, and both give the run of the same numbers."""
     import dpm_solver_b200 as new
     ns = product_schedule("noise")
     want = new.DPM_Solver(wrap("noise", ns, SCALES), ns).sample(x_T(), steps=3, order=2)
     t = torch.tensor(SCALES)
     s = new.DPM_Solver(wrap("noise", ns, t), ns)
     assert torch.equal(s.sample(x_T(), steps=3, order=2), want)
-    listed = new.DPM_Solver(wrap("noise", ns, [torch.tensor(v) for v in SCALES]), ns)
+    ts = [torch.tensor(v) for v in SCALES[:2]] + [torch.tensor([SCALES[2]], dtype=torch.float64)]
+    listed = new.DPM_Solver(wrap("noise", ns, ts), ns)
     assert torch.equal(listed.sample(x_T(), steps=3, order=2), want)
     t.copy_(torch.tensor([2.0, 1.0, 0.5]))
     want2 = new.DPM_Solver(wrap("noise", ns, [2.0, 1.0, 0.5]), ns).sample(x_T(), steps=3, order=2)
     assert torch.equal(s.sample(x_T(), steps=3, order=2), want2)
+    for k, v in ((0, 2.0), (1, 1.0), (2, 0.5)):          # one listed tensor at a time, each write seen at once
+        ts[k].fill_(v)
+        scales = [float(u) for u in ts]
+        want_k = new.DPM_Solver(wrap("noise", ns, scales), ns).sample(x_T(), steps=3, order=2)
+        assert torch.equal(listed.sample(x_T(), steps=3, order=2), want_k), k
+    assert torch.equal(listed.sample(x_T(), steps=3, order=2), want2)

@@ -1,14 +1,16 @@
-"""CFG-Zero*, CFG++ and regional guidance in `sample()`, `UniPC.sample()` and `inverse()` on the device over random
-configurations, bit for bit (tests/guidance_configs.py): paths A-E of tests/test_gpu_apg_random_configs.py -- A the first
-call against the exact CPU executor (every intermediate and the trace of network calls), B the same call again, with no
-guided evaluation of these features frozen as a `PreparedStep`, C another input on the same solver against a fresh
-solver (the zero-init count starts over), D `capture()` replays (zero-init included; a mask read in place is rewritten
-after capture and the replay must follow it), E a fresh solver on a second stream. A refused configuration raises on the
-device and launches nothing. A module-wide tally requires every path of interest to have been met by the fixed seeds."""
+"""CFG-Zero*, CFG++, regional guidance, TCFG and frequency-decoupled guidance in `sample()`, `UniPC.sample()` and
+`inverse()` on the device over random configurations, bit for bit (tests/guidance_configs.py): paths A-E of
+tests/test_gpu_apg_random_configs.py -- A the first call against the exact CPU executor (every intermediate and the
+trace of network calls), B the same call again (no guided evaluation frozen as a `PreparedStep`, except FDG's, which is
+one network output g: its frozen steps are served, and fall back when x comes in another layout), C another input on
+the same solver against a fresh solver (the zero-init count starts over), D `capture()` replays (zero-init included; a
+mask or an FDG [B, N] scale tensor read in place is rewritten after capture and the replay must follow it), E a fresh
+solver on a second stream. A refused configuration raises on the device and launches nothing. A module-wide tally
+requires every path of interest to have been met by the fixed seeds."""
 import pytest
 import torch
 
-from gpu_configs import DT, same_bits
+from gpu_configs import DT, really_channels_last, same_bits
 from guidance_configs import CHUNKS, PER_CHUNK, REQUIRED, REQUIRED_ON_DEVICE, SEED, GuidanceRig, configurations, \
     cpu_oracle, refused, tally_static
 from oracle import ref_loader
@@ -101,8 +103,25 @@ def check_configuration(c, be, filler):
     expect(Bv[2] == A[2], "B: trace of network calls")
     equal_runs(Bv, A, "B vs A")
     expect(all(same_bits(a, b) for a, b in zip([A[0]] + A[1], keepA)), "B overwrote a tensor run A returned")
+    fdg = c["feature"] == "fdg"
     if unipc:
         expect(spy.dup + spy.plain + spy.fell_back == 0 and not s._prep_cache, "B: a UniPC run used a PreparedStep")
+    elif fdg:
+        # a frozen FDG step holds the one output g (a new allocation each evaluation: only its pointer is patched in)
+        expect(all(k[5] and k[-1] for k in s._prep_cache), "B: an FDG step was frozen without g")
+        if spy.dup + spy.plain and not bad:
+            hit("fdg:frozen step served")
+        if (s._prep_cache and x.is_contiguous() and len(c["shape"]) == 3
+                and really_channels_last(dict(c, channels_last=True))):
+            # the same solver on x in channels_last: g and the state in another layout than the frozen steps'
+            xc = x.contiguous(memory_format=torch.channels_last)
+            with LaunchSpy() as spy:
+                Bc = rig.sample(s, xc, trace=True)
+            fresh = GuidanceRig(new, c, "cuda:0")
+            equal_runs(Bc, fresh.sample(fresh.solver(), xc.clone(), trace=True), "B: channels_last x vs fresh solver")
+            expect(spy.fell_back > 0, "B: no frozen step fell back for a channels_last x")
+            if spy.fell_back and not bad:
+                hit("fdg:frozen step fell back")
     else:
         # (key field [5]: e_uncond is None -- a frozen step holds one network output, never a guided pair)
         expect(all(k[5] for k in s._prep_cache), "B: a guided step was frozen")
@@ -112,7 +131,8 @@ def check_configuration(c, be, filler):
     fresh = GuidanceRig(new, c, "cuda:0")
     Cw = fresh.sample(fresh.solver(), x2.clone(), trace=True)
     equal_runs(Cv, Cw, "C vs fresh solver")
-    expect(Cv[2] == Cw[2] and len(Cv[2]) == len(A[2]), "C: trace of network calls (the zero-init count)")
+    # (the adaptive method's number of evaluations follows its input: x2 may take other steps than x)
+    expect(Cv[2] == Cw[2] and (adaptive or len(Cv[2]) == len(A[2])), "C: trace of network calls (the zero-init count)")
     # ---- D: graph capture and replay ----
     if not adaptive and not c["inverse"]:
         g = s.capture(x, **rig.kwargs())
@@ -135,6 +155,14 @@ def check_configuration(c, be, filler):
                 expect(same_bits(got, new_rig.sample(new_rig.solver(), x)[0]),
                        "D: replay after rewriting a mask vs a fresh eager run")
                 hit("captured:rewritten-mask")
+        if fdg and c["fdg_form"] == "rows":
+            # an fp32 [B, N] tensor on the device is read in place: the replay follows a rewrite
+            rig.fdg.mul_(-0.5).add_(0.75)
+            got = g(x).clone()
+            new_rig = GuidanceRig(new, c, "cuda:0", fdg=rig.fdg.clone())
+            expect(same_bits(got, new_rig.sample(new_rig.solver(), x)[0]),
+                   "D: replay after rewriting the FDG scales vs a fresh eager run")
+            hit("captured:fdg rows rewritten")
         del g
     # ---- E: a fresh solver on a second stream ----
     side = torch.cuda.Stream()

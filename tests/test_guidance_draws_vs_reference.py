@@ -1,11 +1,14 @@
 """The CPU side of tests/test_gpu_guidance_random_configs.py, pinned where there is no device: the exact executor's result
-for every CFG-Zero*, CFG++ and regional-guidance configuration the device test draws, against the unmodified reference
-wherever it can express the configuration (CFG-Zero* and masks bit for bit, CFG++ within CFGPP_TOL of the fp64
-transcription, each with as many evaluations); the refused configurations are exactly the documented ones; and the
-fixed seeds reach every path the device test must meet."""
+for every CFG-Zero*, CFG++, regional-guidance, TCFG and FDG configuration the device test draws, against the unmodified
+reference wherever it can express the configuration (CFG-Zero*, masks, TCFG and FDG bit for bit, CFG++ within CFGPP_TOL
+of the fp64 transcription, plus the rounding bound of an x_start network's x0 conversion, each with as many
+evaluations); an FDG run with equal scales is its one-level run; the
+refused configurations are exactly the documented ones; and the fixed seeds reach every path the device test must
+meet."""
 import pytest
 
-from guidance_configs import CHUNKS, REQUIRED, configurations, cpu_oracle, reference_expressible, refused, tally_static
+from guidance_configs import CHUNKS, FEATURES, REQUIRED, configurations, cpu_oracle, reference_expressible, refused, \
+    tally_static
 from oracle import ref_loader
 
 pytestmark = pytest.mark.skipif(not ref_loader.available(), reason="oracle/_ref not built and no reference tree")
@@ -34,5 +37,5 @@ def test_tally_of_the_drawn_configurations():
     if len(CHUNKS_RUN) < CHUNKS:
         pytest.skip("needs every chunk of test_oracle_of_every_drawn_configuration in the same session")
     print("\ntally: %s" % dict(sorted(TALLY.items())))
-    pinned = ["pinned:" + f for f in ("cfgzero", "cfgpp", "mask")]
+    pinned = ["pinned:" + f for f in FEATURES]
     assert not [k for k in REQUIRED + pinned + ["rejected"] if not TALLY.get(k)]
