@@ -116,6 +116,9 @@ PROTOTYPES = {
     "dpm_tcfg_workspace": (C.c_size_t, [_u64, _u64]),
     "dpm_tcfg_words": (C.c_int, [_vp, _vp, _vp, _i, _u64, _u64, _vp, C.c_size_t, _vp]),
     "dpm_step_tcfg": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _vp]),
+    "dpm_perpneg_workspace": (C.c_size_t, [_u64, _u64]),
+    "dpm_perpneg_words": (C.c_int, [_vp, _vp, C.POINTER(_vp), C.POINTER(_f), _i, _i, _u64, _u64, _vp, C.c_size_t,
+                                    _vp]),
     "dpm_fdg_supported": (C.c_int, [_u64, _u64, _i, _i]),
     "dpm_fdg_guided": (C.c_int, [_vp, _vp, _vp, _i, _u64, _u64, _u64, _i64, _i64, _i64, _i64, _i, _vp, _u64, _u64,
                                  _vp]),

@@ -361,4 +361,170 @@ int launch_tcfg_words(float* w_out, const void* ec, const void* eu, int model_dt
   return launch_zpass<3>(k_tcfg_final, "tcfg words", w_out, ec, eu, model_dtype, per_sample, n, ws, ws_bytes, stream);
 }
 
+// ---- Perp-Neg (dpm_perpneg_words; Armandpour, Sadeghian, Zheng, Sadeghian and Zhou, arXiv:2304.04968) -------------
+// The K-way sibling of the CFG-Zero* pass: over u = e_uncond and e_1..e_K, d_k = e_k - u in fp64 and the K fp64 sums
+// N = ||d_1||^2, P_k = <d_k, d_1> (k = 2..K), in k_cfgzero_partial's chunking, thread ownership, warp butterflies and
+// chunk merge. k_perpneg_final then folds the sums with the host scales into one word per sample,
+// w_1 = fl32(s_1 - s_2*c_2 - ... - s_K*c_K), c_k = P_k/N (0 when N == 0), which dpm_step_multi_masked reads as condition
+// 1's period-1 weight map. Algorithmic bytes: (K+1)*s_model per element. (This file builds with -fmad=false: no
+// product below is contracted into an fma.)
+constexpr int kPNMax = 4;   // DPM_MAX_CONDITIONS
+
+struct PNParams {
+  const void* eu;
+  const void* ec[kPNMax];
+  double* partial;       // [n_samples * chunks][K]: N, P_2 .. P_K
+  float* w_out;          // [n_samples]
+  uint64_t per_sample;
+  uint64_t n_samples;
+  uint32_t chunks;
+  int32_t model_dtype;
+  int32_t n_cond;
+  float scales[kPNMax];  // fl32(s_1) .. fl32(s_K)
+};
+
+// VEC: per_sample % 8 == 0 and all K+1 blocks aligned, TE their type. Otherwise element-wise (load_any).
+template <typename TE, bool VEC, int K>
+__global__ void __launch_bounds__(kAThreads) k_perpneg_partial(const __grid_constant__ PNParams p) {
+  static_assert(K >= 2 && K <= kPNMax, "two to four conditions");
+  __shared__ double warp_part[kAThreads / 32];
+  const uint64_t sample = blockIdx.x / p.chunks;
+  const uint32_t chunk = blockIdx.x % p.chunks;
+  const uint64_t c_begin = (uint64_t)chunk * kAChunk;
+  const uint64_t c_end = c_begin + kAChunk < p.per_sample ? c_begin + kAChunk : p.per_sample;
+  const uint32_t cnt = (uint32_t)(c_end - c_begin);
+  const size_t e0 = sample * p.per_sample + c_begin;
+  const int tid = threadIdx.x;
+  constexpr int U = kAChunk / kPacket / kAThreads;   // 4
+  double s[K];   // N, P_2 .. P_K
+#pragma unroll
+  for (int k = 0; k < K; ++k) s[k] = 0.0;
+  auto term = [&](float u, const float (&e)[K]) {
+    const double d1 = (double)e[0] - (double)u;
+    s[0] += d1 * d1;
+#pragma unroll
+    for (int k = 1; k < K; ++k) s[k] += ((double)e[k] - (double)u) * d1;
+  };
+  // element (u, i) of this thread is chunk element (u*kAThreads + tid)*8 + i on both paths, as in k_cfgzero_partial
+#pragma unroll
+  for (int it = 0; it < U; ++it) {
+    const uint32_t pk = it * kAThreads + tid;
+    if (VEC) {
+      if (pk * kPacket < cnt) {
+        const size_t e = e0 + (size_t)pk * kPacket;
+        Raw<TE> ru, rc[K];
+        ldg_pk(ru, static_cast<const TE*>(p.eu) + e);
+#pragma unroll
+        for (int k = 0; k < K; ++k) ldg_pk(rc[k], static_cast<const TE*>(p.ec[k]) + e);
+        float fu[8], fc[K][8];
+        unpack(ru, fu);
+#pragma unroll
+        for (int k = 0; k < K; ++k) unpack(rc[k], fc[k]);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          float ev[K];
+#pragma unroll
+          for (int k = 0; k < K; ++k) ev[k] = fc[k][i];
+          term(fu[i], ev);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const uint32_t j = pk * kPacket + i;
+        if (j < cnt) {
+          float ev[K];
+#pragma unroll
+          for (int k = 0; k < K; ++k) ev[k] = load_any(p.ec[k], p.model_dtype, e0 + j);
+          term(load_any(p.eu, p.model_dtype, e0 + j), ev);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < K; ++k) s[k] = apg_cta_sum(s[k], warp_part);
+  if (tid == 0) {
+    double* o = p.partial + (size_t)blockIdx.x * K;
+#pragma unroll
+    for (int k = 0; k < K; ++k) o[k] = s[k];
+  }
+}
+
+// The word of sample b from its merged sums, in fp64 left to right with each op rounded: t = s_1, then
+// t = t - s_k*c_k for k = 2..K, rounded to fp32 once. A sum that is not finite gives k_tcfg_final's NaN.
+__global__ void __launch_bounds__(kAThreads) k_perpneg_final(const __grid_constant__ PNParams p) {
+  const uint64_t b = (uint64_t)blockIdx.x * kAThreads + threadIdx.x;
+  if (b >= p.n_samples) return;
+  const int K = p.n_cond;
+  const double* part = p.partial + b * p.chunks * K;
+  double s[kPNMax] = {0.0, 0.0, 0.0, 0.0};
+  for (uint32_t c = 0; c < p.chunks; ++c) {
+#pragma unroll
+    for (int k = 0; k < kPNMax; ++k)
+      if (k < K) s[k] += part[c * K + k];
+  }
+  bool finite = true;
+#pragma unroll
+  for (int k = 0; k < kPNMax; ++k)
+    if (k < K) finite = finite && isfinite(s[k]);
+  float w = __int_as_float(0x7fffffff);
+  if (finite) {
+    double t = (double)p.scales[0];
+#pragma unroll
+    for (int k = 1; k < kPNMax; ++k) {
+      if (k < K) {
+        const double ck = s[0] == 0.0 ? 0.0 : s[k] / s[0];
+        t = t - (double)p.scales[k] * ck;
+      }
+    }
+    w = (float)t;
+  }
+  p.w_out[b] = w;
+}
+
+size_t perpneg_workspace_bytes(uint64_t n_samples, uint64_t per_sample) {
+  return zpass_workspace_bytes(n_samples, per_sample, kPNMax);
+}
+
+template <int K>
+static void launch_perpneg_partial(const PNParams& p, bool vec, cudaStream_t stream) {
+  typedef void (*PKernel)(const PNParams);
+  PKernel k = k_perpneg_partial<float, false, K>;   // any dtype, alignment or sample size
+  if (vec) {
+    if (p.model_dtype == DPM_F32) k = k_perpneg_partial<float, true, K>;
+    else if (p.model_dtype == DPM_BF16) k = k_perpneg_partial<__nv_bfloat16, true, K>;
+    else if (p.model_dtype == DPM_F16) k = k_perpneg_partial<__half, true, K>;
+  }
+  k<<<(unsigned)(p.n_samples * p.chunks), kAThreads, 0, stream>>>(p);
+}
+
+// the sums pass over the K+1 blocks, then the word per sample: two launches, no allocation, no sync
+int launch_perpneg_words(float* w_out, const void* eu, const void* const* ec, const float* scales, int n_cond,
+                         int model_dtype, uint64_t per_sample, uint64_t n, void* ws, size_t ws_bytes,
+                         cudaStream_t stream) {
+  PNParams p;
+  memset(&p, 0, sizeof(p));
+  p.eu = eu; p.w_out = w_out; p.model_dtype = model_dtype; p.n_cond = n_cond;
+  for (int k = 0; k < n_cond; ++k) { p.ec[k] = ec[k]; p.scales[k] = scales[k]; }
+  p.per_sample = per_sample; p.n_samples = n / per_sample;
+  p.chunks = (uint32_t)((per_sample + kAChunk - 1) / kAChunk);
+  p.partial = static_cast<double*>(ws);
+  if (ws == nullptr || ws_bytes < perpneg_workspace_bytes(p.n_samples, per_sample) ||
+      (reinterpret_cast<uintptr_t>(ws) & 7)) {
+    set_error("perpneg words: workspace too small or not 8-byte aligned");
+    return DPM_ERR_ARG;
+  }
+  if (p.n_samples * p.chunks > 0x7fffffffull) { set_error("perpneg words: too many chunks"); return DPM_ERR_UNSUPPORTED; }
+  const uintptr_t am = model_dtype == DPM_F32 ? 31 : 15;
+  bool vec = per_sample % kPacket == 0 && (reinterpret_cast<uintptr_t>(eu) & am) == 0;
+  for (int k = 0; k < n_cond; ++k) vec = vec && (reinterpret_cast<uintptr_t>(ec[k]) & am) == 0;
+  if (n_cond == 2) launch_perpneg_partial<2>(p, vec, stream);
+  else if (n_cond == 3) launch_perpneg_partial<3>(p, vec, stream);
+  else launch_perpneg_partial<4>(p, vec, stream);
+  k_perpneg_final<<<(unsigned)((p.n_samples + kAThreads - 1) / kAThreads), kAThreads, 0, stream>>>(p);
+  count_launch();
+  count_launch();
+  return DPM_OK;
+}
+
 }  // namespace dpm

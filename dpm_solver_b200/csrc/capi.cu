@@ -674,6 +674,27 @@ int dpm_step_tcfg(const dpm_step_desc* desc, const float* words, const float* gu
   return step_impl(desc, static_cast<cudaStream_t>(stream), nullptr, guidance, nullptr, nullptr, words);
 }
 
+size_t dpm_perpneg_workspace(uint64_t n_samples, uint64_t per_sample) {
+  return perpneg_workspace_bytes(n_samples, per_sample);
+}
+
+int dpm_perpneg_words(float* w_out, const void* e_uncond, const void* const* e_conds, const float* scales, int n_cond,
+                      int model_dtype, uint64_t per_sample, uint64_t n, void* workspace, size_t workspace_bytes,
+                      dpm_stream_t stream) {
+  if (n_cond < 2 || n_cond > DPM_MAX_CONDITIONS) {
+    set_error("perpneg words: n_cond must be 2..%d, got %d", DPM_MAX_CONDITIONS, n_cond);
+    return DPM_ERR_ARG;
+  }
+  if (!w_out || !e_uncond || !e_conds || !scales) { set_error("perpneg words: NULL pointer"); return DPM_ERR_ARG; }
+  for (int k = 0; k < n_cond; ++k)
+    if (!e_conds[k]) { set_error("perpneg words: NULL e_conds[%d]", k); return DPM_ERR_ARG; }
+  if (!valid_dtype(model_dtype)) { set_error("perpneg words: bad dtype"); return DPM_ERR_ARG; }
+  if (n == 0) return DPM_OK;
+  if (per_sample == 0 || n % per_sample) { set_error("perpneg words: per_sample must divide n"); return DPM_ERR_ARG; }
+  return finish(launch_perpneg_words(w_out, e_uncond, e_conds, scales, n_cond, model_dtype, per_sample, n, workspace,
+                                     workspace_bytes, static_cast<cudaStream_t>(stream)));
+}
+
 int dpm_fdg_supported(uint64_t H, uint64_t W, int levels, int model_dtype) {
   return fdg_supported(H, W, levels, model_dtype);
 }

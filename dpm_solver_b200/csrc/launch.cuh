@@ -144,6 +144,10 @@ int launch_cfgzero_scale(float* s_out, const void* ec, const void* eu, int model
 size_t tcfg_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
 int launch_tcfg_words(float* w_out, const void* ec, const void* eu, int model_dtype, uint64_t per_sample, uint64_t n,
                       void* ws, size_t ws_bytes, cudaStream_t stream);
+size_t perpneg_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
+int launch_perpneg_words(float* w_out, const void* eu, const void* const* ec, const float* scales, int n_cond,
+                         int model_dtype, uint64_t per_sample, uint64_t n, void* ws, size_t ws_bytes,
+                         cudaStream_t stream);
 int fdg_supported(uint64_t H, uint64_t W, int levels, int model_dtype);
 int launch_fdg_guided(void* g, const void* ec, const void* eu, int model_dtype, uint64_t planes, uint64_t H, uint64_t W,
                       int64_t sample_stride, int64_t plane_stride, int64_t h_stride, int64_t w_stride, int levels,

@@ -403,6 +403,33 @@ class CudaBackend:
                      C.c_uint64(n), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
         return w
 
+    def perpneg_words(self, e_uncond: torch.Tensor, e_conds, scales) -> torch.Tensor:
+        """Perp-Neg's per-sample weight of the first condition, w_1 = fl32(s_1 - sum_{k>=2} s_k*<d_k, d_1>/||d_1||^2)
+        with d_k = e_k - u, as fp32 [B] on the device (dpm_perpneg_words): fp64 sums in storage order, merged per chunk
+        in order, then the header's left-to-right fp64 fold. `scales`: the K python-float scales (fp32-rounded). All
+        K+1 blocks keep a shared dense layout (a sample is one contiguous block in row-major and channels_last storage
+        alike)."""
+        K = len(e_conds)
+        if not 2 <= K <= _lib.MAX_CONDITIONS or len(scales) != K:
+            raise ValueError("dpm_solver_b200: Perp-Neg words take 2..{} conditional outputs and one scale each".format(
+                _lib.MAX_CONDITIONS))
+        n, dev = e_uncond.numel(), e_uncond.device
+        layout = self._layout(e_uncond)
+        if layout is None or any(self._layout(e) != layout for e in e_conds):
+            layout = "c"
+        eu = self._check(e_uncond, "e_uncond", dev, n, layout=layout)
+        ecs = [self._check(e, "e_conds[%d]" % k, dev, n, e_uncond.dtype, layout) for k, e in enumerate(e_conds)]
+        nb = e_uncond.shape[0]
+        per_sample = n // nb
+        w = torch.empty(nb, dtype=torch.float32, device=dev)
+        ws_bytes = int(self._lib.dpm_perpneg_workspace(nb, per_sample))
+        ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev)
+        ecp, sc = (C.c_void_p * K)(*[e.data_ptr() for e in ecs]), (C.c_float * K)(*scales)
+        self._launch(dev, self._lib.dpm_perpneg_words, C.c_void_p(w.data_ptr()), C.c_void_p(eu.data_ptr()), ecp, sc,
+                     C.c_int(K), C.c_int(_DTYPE_CODE[e_uncond.dtype]), C.c_uint64(per_sample), C.c_uint64(n),
+                     C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
+        return w
+
     def fdg_guided(self, e_cond: torch.Tensor, e_uncond: torch.Tensor, scales, levels: int) -> torch.Tensor:
         """Frequency-decoupled guidance (dpm_fdg_guided, one launch): g over the planes of the last two dims, in the
         outputs' dtype and dense layout. `scales`: `levels` python floats shared by the batch, or an fp32 [B, levels]

@@ -62,6 +62,7 @@ class RawOutput:
     # frequency-decoupled guidance (model_wrapper's fdg_scales): (scales, levels), the scales `levels` python floats or
     # an fp32 [B, levels] tensor on the outputs' device; the solver turns the pair into one output g (dpm_fdg_guided)
     fdg: Optional[tuple] = None
+    perp: bool = False              # Perp-Neg: conditions 2..K projected off condition 1's (model_wrapper's perp_neg)
 
 
 def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale, masked=False):
@@ -166,10 +167,33 @@ def _guidance_args(a: StepArgs, ratio: Optional[torch.Tensor], raw: RawOutput, r
         a.scales = raw.scales
         if raw.masks is not None:
             d = raw.e_cond.dim()
-            a.masks = raw.masks if rows is None else tuple(m if m is None else m.rows(rows, d) for m in raw.masks)
+            a.masks = raw.masks if rows is None else tuple(m if m is None else _map_rows(m, rows, d) for m in raw.masks)
     if a.ratio is not None or a.guidance_b is not None or a.masks is not None:
         a.per_sample = a.e_cond.numel() // a.e_cond.shape[0]
     return a
+
+
+def _map_rows(m, rows, x_dims: int):
+    """The weight map of the batch rows `rows`: a _CondMask's own rows, or those of a (w, period, sample_stride) triple
+    (a map shared by the batch, sample_stride 0, is kept)."""
+    if isinstance(m, _CondMask):
+        return m.rows(rows, x_dims)
+    w, period, stride = m
+    return m if stride == 0 else (w.reshape(-1, period)[rows].reshape(-1), period, stride)
+
+
+def _perp_output(be, raw: RawOutput) -> RawOutput:
+    """A Perp-Neg evaluation as an ordinary regional-guidance one: the words pass over the K+1 outputs (2 launches)
+    gives condition 1's per-sample weight w_1, which becomes its period-1 weight map under the scales (1, s_2, ..., s_K);
+    everything downstream is the masked multi-condition path."""
+    fn = getattr(be, "perpneg_words", None)
+    if fn is None:
+        raise RuntimeError("perp_neg needs an executor with perpneg_words; {} has none".format(
+            getattr(be, "name", type(be).__name__)))
+    w = fn(raw.e_uncond, raw.e_conds, raw.scales)
+    K = len(raw.scales)
+    return dataclasses.replace(raw, scales=(1.0,) + tuple(raw.scales[1:]), masks=((w, 1, 1),) + (None,) * (K - 1),
+                               perp=False)
 
 
 def _apg_args(be, raw: RawOutput, xe, marg, sdtype, x0: bool, ns, coef_dev=None, r_prev=None, r_out=None) -> StepArgs:
@@ -256,10 +280,11 @@ class WrappedModel:
     def __init__(self, model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                  unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale=0.,
                  apg_eta=None, apg_norm_threshold=0., apg_momentum=0., cfg_zero_star=False, cfg_zero_init_steps=0,
-                 cfg_pp=False, guidance_mask=None, tcfg=False, fdg_scales=None):
+                 cfg_pp=False, guidance_mask=None, tcfg=False, fdg_scales=None, perp_neg=False):
         self.model = model
         self.cfg_pp = cfg_pp
         self.tcfg = tcfg
+        self.perp_neg = perp_neg
         # frequency-decoupled guidance: its number of levels (0: off), shared scales or the per-sample tensor
         self.fdg_levels, self._fdg_shared, self._fdg_vec = (0, None, None) if fdg_scales is None else \
             _fdg_scales(fdg_scales)
@@ -432,7 +457,7 @@ class WrappedModel:
             t_in = None if t_input is not None else torch.cat([t_continuous] * n)
             outs = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(n)   # uncond first
             return RawOutput(outs[1], outs[0], param, 1.0, e_conds=tuple(outs[1:]), scales=self.cond_scales,
-                             masks=self.cond_masks)
+                             masks=self.cond_masks, perp=self.perp_neg)
         if self.guidance_type == "classifier-free":
             gb = self._scales(x) if self._scale_vec is not None else None     # (checked before the network runs)
             fdg = self.fdg_args(x) if self.fdg_levels else None               # likewise
@@ -497,6 +522,8 @@ class WrappedModel:
         r = self.raw(x, t_continuous, plain=True)
         if r.fdg is not None:
             r = _fdg_output(be, r)        # g, then converted as one network output
+        if r.perp:
+            r = _perp_output(be, r)       # over the whole batch: each sample's word reads its own values only
         if r.e_uncond is None and r.param == PARAM_NOISE:
             return r.e_cond
         if r.apg is not None and r.e_uncond is not None:
@@ -539,7 +566,7 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
                   condition=None, unconditional_condition=None, guidance_scale=1., classifier_fn=None,
                   classifier_kwargs={}, guidance_rescale=0., apg_eta=None, apg_norm_threshold=0., apg_momentum=0.,
                   cfg_zero_star=False, cfg_zero_init_steps=0, cfg_pp=False, guidance_mask=None, tcfg=False,
-                  fdg_scales=None):
+                  fdg_scales=None, perp_neg=False):
     """Wrap a network into `model_fn(x, t_continuous) -> noise`; same contract as the reference
     (:170-334): model_type in {noise, x_start, v, score}, guidance_type in {uncond, classifier,
     classifier-free}.
@@ -710,6 +737,39 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     unconditional_condition, several conditions, guidance_mask, guidance_rescale != 0, apg_eta, cfg_zero_star, cfg_pp
     and DPM_Solver(reference_rounding=True).
 
+    perp_neg=True (classifier-free guidance with condition=[c_1, ..., c_K], 2 <= K <= 4; not in the reference; default
+    False; anything other than a bool is a ValueError): perpendicular negative prompts (Perp-Neg; Armandpour,
+    Sadeghian, Zheng, Sadeghian and Zhou, arXiv:2304.04968; ComfyUI's PerpNeg / PerpNegGuider). c_1 is the positive
+    prompt; every later condition loses, per sample, its component along c_1's direction before it is weighted, so a
+    negative prompt no longer removes part of what the positive one asks for. Negatives take negative scales, as they
+    do with several conditions; ComfyUI's cond_scale s and neg_scale n are guidance_scale=[s, -s*n] with the empty
+    prompt as unconditional_condition. With d_k = e_k - e_u the raw network outputs' differences, in exact arithmetic:
+        eps = e_u + s_1*d_1 + sum_{k>=2} s_k*(d_k - (<d_k, d_1>/||d_1||^2)*d_1)
+    The projection coefficient is taken in the network's raw output space, as cfg_zero_star and tcfg take theirs; every
+    parameterisation converts the blocks of a sample by one affine map with a shared x term, so the ratio is the same
+    in the converted space up to rounding. Exact arithmetic, per sample b, all values in storage order:
+        N = sum d_1*d_1,  P_k = sum d_k*d_1 (k >= 2)     (fp64: each output widened, d_k = e_k - e_u in fp64, the sums
+                                                         in the chunking and merge order of the CFG-Zero* pass)
+        c_k = P_k / N, or 0 when N == 0 (condition 1 equals the unconditional output: the plain multi-condition combine)
+        w_1 = fl32(s_1 - s_2*c_2 - ... - s_K*c_K)      (fp64 left to right, each op rounded, s_k = the fp32 scale)
+    and a non-finite N or P_k gives a NaN w_1. The evaluation is then the regional-guidance one with the scales
+    (1, s_2, ..., s_K) and w_1 as condition 1's one-weight-per-sample mask: eps = eps_u + w_1*(eps_1 - eps_u) +
+    s_2*(eps_2 - eps_u) + ..., each block converted by the parameterisation first, every op rounded to fp32. The sums
+    run per sample, not over the whole batch: rows stay independent and batch sharding needs no collective. ComfyUI
+    normalises over the whole batch; for B = 1 the two agree. Consequences: negatives that differ from e_u only where
+    c_1 does not give P_k = +0 and w_1 == s_1, the run without perp_neg bit for bit; a negative exactly parallel to
+    the positive cancels its own effect to rounding; a condition-blind network gives the unguided run. Cost per guided
+    evaluation: the words pass (2 launches, reading the K+1 outputs once, no host sync, so capture() replays it) and
+    the masked fused step.
+    Accepted: everything several conditions accept -- every model type and schedule, both algorithms, singlestep,
+    multistep, singlestep_fixed, adaptive (host or device controller), dynamic thresholding, correcting_x0_fn /
+    correcting_xt_fn, denoise_to_zero, inverse(), return_intermediate, capture() and batch sharding; a direct call of
+    this callable returns the converted Perp-Neg value. Not available (ValueError before any launch and any network
+    call): other guidance types, no unconditional_condition, fewer than two conditions, guidance_mask, and everything
+    several conditions refuse (guidance_rescale, per-sample scales, apg_eta, cfg_zero_star, cfg_pp, tcfg, fdg_scales,
+    UniPC and DPM_Solver(reference_rounding=True)). Not offered: per-sample Perp-Neg scales, Gram-Schmidt among the
+    negatives (each is projected against the positive only), the paper's view-dependent weights for text-to-3D.
+
     fdg_scales=[w_0, ..., w_{N-1}] (classifier-free guidance only; not in the reference; default None: off):
     frequency-decoupled guidance (Sadat, Vontobel, Salehi and Weber, "Guidance in the Frequency Domain Enables
     High-Fidelity Sampling at Low CFG Scales", 2025; diffusers' FrequencyDecoupledGuidance guider). c - u is split into
@@ -853,6 +913,16 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
             raise ValueError("fdg_scales replaces guidance_scale, which must stay at its default 1.0, got {!r}".format(
                 guidance_scale))
         _fdg_scales(fdg_scales)                       # (the form and the number of levels)
+    if not isinstance(perp_neg, bool):
+        raise ValueError("perp_neg must be a bool, got {!r}".format(perp_neg))
+    if perp_neg:
+        if guidance_type != "classifier-free" or unconditional_condition is None:
+            raise ValueError("perp_neg needs guidance_type='classifier-free' and an unconditional_condition")
+        if not isinstance(condition, (list, tuple)) or len(condition) < 2:
+            raise ValueError("perp_neg needs a list of at least two conditions: the positive prompt first, then the "
+                             "negatives")
+        if guidance_mask is not None:
+            raise ValueError("perp_neg is not available with guidance_mask")
     if guidance_mask is not None:
         condition, guidance_scale, guidance_mask = _masked_arguments(
             guidance_type, condition, unconditional_condition, guidance_scale, guidance_mask, guidance_rescale,
@@ -869,7 +939,7 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
     return WrappedModel(model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                         unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale,
                         apg_eta, apg_norm_threshold, apg_momentum, cfg_zero_star, cfg_zero_init_steps, cfg_pp,
-                        guidance_mask, tcfg, fdg_scales)
+                        guidance_mask, tcfg, fdg_scales, perp_neg)
 
 
 def _masked_arguments(guidance_type, condition, unconditional_condition, guidance_scale, guidance_mask,
@@ -1259,6 +1329,11 @@ class DPM_Solver:
             # dtype, handed on as one network output of the same parameterisation; everything below is the one-output
             # path (the fused step with out / out2, the quantile, UniPC, device coefficients)
             raw = _fdg_output(be, raw)
+        if raw.perp:
+            # Perp-Neg: the words pass over the K+1 raw outputs (+2 launches) gives condition 1's per-sample weight;
+            # from here on the evaluation is a regional-guidance one (the masked fused step with its replicas, the fp32
+            # materialisation for the quantile, the correcting_x0_fn split, device coefficients)
+            raw = _perp_output(be, raw)
         pkey = None
         if slot is not None and self._prep_on:
             # (phi is part of the key: a rescaled evaluation is never served by a launch frozen without the rescale)

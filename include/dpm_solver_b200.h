@@ -30,7 +30,8 @@ extern "C" {
 
 #define DPM_B200_VERSION 108 /* 0.1.8: CFG++ (dpm_step_cfgpp); regional guidance (dpm_step_multi_masked), TCFG
                                 (dpm_tcfg_words, dpm_step_tcfg) and frequency-decoupled guidance (dpm_fdg_supported,
-                                dpm_fdg_guided) are additions to this ABI: test for their symbols */
+                                dpm_fdg_guided) and Perp-Neg (dpm_perpneg_workspace, dpm_perpneg_words) are additions
+                                to this ABI: test for their symbols */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -496,6 +497,34 @@ typedef struct dpm_cond_map {
 } dpm_cond_map;
 DPM_API int dpm_step_multi_masked(const dpm_step_desc* desc, const void* const* e_conds, const float* scales,
                                   const dpm_cond_map* maps, int n_cond, void* const* replicas, dpm_stream_t stream);
+
+/* ---- Perp-Neg: perpendicular negative prompts (Armandpour, Sadeghian, Zheng, Sadeghian and Zhou, "Re-imagine the
+ * Negative Prompt Algorithm: Transform 2D Diffusion into 3D, alleviate Janus problem and Beyond", arXiv:2304.04968) --
+ * Multi-condition guidance in which every condition after the first loses, per sample, its component along the first
+ * condition's direction before it is weighted. With u = e_uncond, e_k = e_conds[k-1] (raw network outputs, all K
+ * blocks flattened per sample in storage order), in exact arithmetic:
+ *   eps = u + s_1*d_1 + sum_{k>=2} s_k*(d_k - (<d_k, d_1>/||d_1||^2)*d_1),   d_k = e_k - u
+ * which is u + w_1*d_1 + sum_{k>=2} s_k*d_k with one per-sample weight w_1. Every parameterisation maps the blocks of
+ * a sample by one affine map whose x term is shared, so the ratio is the same in raw and converted space.
+ * dpm_perpneg_words: w_1 of each sample b -> w_out[b], b < n/per_sample, fp32 device memory. Per sample, each value
+ *   widened to fp64 and d_k = e_k - u formed in fp64, the fp64 sums N = sum d_1*d_1 and P_k = sum d_k*d_1 (k = 2..K)
+ *   run in the chunking, thread ownership and merge order of dpm_cfgzero_scale, so the word of sample b depends on
+ *   sample b's values only. Then c_k = P_k / N (c_k = 0 when N == 0: condition 1 equals u, nothing to project out)
+ *   and, in fp64 left to right with each op rounded, sigma_k = fl32(s_k) = scales[k-1] widened:
+ *     w_1 = fl32(sigma_1 - sigma_2*c_2 - ... - sigma_K*c_K)
+ *   A non-finite N or P_k gives the NaN 0x7fffffff. scales: HOST array of n_cond floats, passed by value (capturable).
+ *   Reads the K+1 blocks once ((K+1)*s_model bytes per element). workspace: dpm_perpneg_workspace(n/per_sample,
+ *   per_sample) bytes of 8-byte aligned device memory (contents irrelevant). Two launches; does not synchronise or
+ *   allocate. Returns DPM_ERR_ARG before any launch for n_cond outside 2..DPM_MAX_CONDITIONS, a NULL pointer (w_out,
+ *   e_uncond, e_conds, an entry of it, scales), a bad model_dtype, or per_sample not dividing n. 16-byte aligned blocks
+ *   (32-byte for fp32) with per_sample % 8 == 0 take 128-bit loads; anything else gives the same bits element-wise.
+ * The step is then dpm_step_multi_masked with scales (1, s_2, .., s_K), maps[0] = {w_out, 1, 1} and no other map:
+ *   eps_u + w_1*(eps_1 - eps_u) + s_2*(eps_2 - eps_u) + ..., each block converted by the parameterisation first (1*w_1
+ *   is w_1 exactly). Both entry points were added within version 108: test for their symbols. */
+DPM_API size_t dpm_perpneg_workspace(uint64_t n_samples, uint64_t per_sample);
+DPM_API int dpm_perpneg_words(float* w_out, const void* e_uncond, const void* const* e_conds, const float* scales,
+                              int n_cond, int model_dtype, uint64_t per_sample, uint64_t n, void* workspace,
+                              size_t workspace_bytes, dpm_stream_t stream);
 
 /* ---- UniPC multistep (Zhao et al. 2023, "UniPC: A Unified Predictor-Corrector Framework", arXiv:2302.04867) ------
  * One launch per network evaluation i: the corrector of step i and the predictor of step i+1 (dpm_solver_b200/unipc.py
