@@ -47,6 +47,15 @@ class UniDesc(C.Structure):
     ]
 
 
+class SdeDesc(C.Structure):
+    """struct dpm_sde_desc"""
+    _fields_ = [
+        ("z", C.c_void_p), ("guidance", C.c_void_p), ("ratio", C.c_void_p), ("s_star", C.c_void_p),
+        ("tcfg_words", C.c_void_p), ("seed", C.c_uint64), ("offset", C.c_uint64), ("cz", C.c_float), ("phi", C.c_float),
+        ("one_minus_phi", C.c_float),
+    ]
+
+
 class AdaptiveCtl(C.Structure):
     """struct dpm_adaptive_ctl"""
     _fields_ = [
@@ -113,6 +122,7 @@ PROTOTYPES = {
     "dpm_cfgzero_scale": (C.c_int, [_vp, _vp, _vp, _i, _u64, _u64, _vp, C.c_size_t, _vp]),
     "dpm_step_cfgzero": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _vp]),
     "dpm_step_cfgpp": (C.c_int, [C.POINTER(StepDesc), _f, _vp, _vp]),
+    "dpm_step_sde": (C.c_int, [C.POINTER(StepDesc), C.POINTER(SdeDesc), _vp]),
     "dpm_tcfg_workspace": (C.c_size_t, [_u64, _u64]),
     "dpm_tcfg_words": (C.c_int, [_vp, _vp, _vp, _i, _u64, _u64, _vp, C.c_size_t, _vp]),
     "dpm_step_tcfg": (C.c_int, [C.POINTER(StepDesc), _vp, _vp, _vp]),

@@ -506,6 +506,35 @@ static int step_cfgpp_impl(const dpm_step_desc* desc, float g, const float* guid
   return finish(rc);
 }
 
+static int step_sde_impl(const dpm_step_desc* desc, const dpm_sde_desc* s, cudaStream_t stream) {
+  if (desc == nullptr || s == nullptr) { set_error("sde step: desc or sde is NULL"); return DPM_ERR_ARG; }
+  if ((desc->form != DPM_FORM_LIN1 && desc->form != DPM_FORM_DIFF2 && desc->form != DPM_FORM_MS3) || desc->c0_on_old ||
+      desc->raw_round != 0 || desc->dev_coef != nullptr || s->offset % 4 != 0) {
+    set_error("sde step: needs form LIN1, DIFF2 or MS3 with c0_on_old == 0, raw_round == 0, dev_coef == NULL and a "
+              "philox offset divisible by 4");
+    return DPM_ERR_ARG;
+  }
+  const bool words = s->guidance != nullptr || s->ratio != nullptr || s->s_star != nullptr || s->tcfg_words != nullptr;
+  if (words && (desc->n_model != 2 || desc->per_sample == 0 || desc->n % desc->per_sample)) {
+    set_error("sde step: per-sample words need n_model == 2 and per_sample dividing n");
+    return DPM_ERR_ARG;
+  }
+  if ((s->s_star != nullptr && s->tcfg_words != nullptr) ||
+      ((s->s_star != nullptr || s->tcfg_words != nullptr) && s->ratio != nullptr)) {
+    set_error("sde step: s_star, tcfg_words and ratio exclude each other");
+    return DPM_ERR_ARG;
+  }
+  if (desc->n == 0) return DPM_OK;
+  KParams p;
+  Needs nd;
+  int rc = build_params(desc, &p, &nd, false);
+  if (rc != DPM_OK) return rc;
+  p.ratio = s->ratio; p.phi = s->phi; p.psi = s->one_minus_phi;
+  p.gscale = s->guidance; p.zs = s->s_star; p.td = s->tcfg_words;
+  const bool al = all_aligned(p, nd) && (s->z == nullptr || aligned(s->z, DPM_F32));
+  return finish(launch_step_sde(p, s->z, s->cz, s->seed, s->offset, al, stream));
+}
+
 }  // namespace dpm
 
 using namespace dpm;
@@ -710,6 +739,10 @@ int dpm_fdg_guided(void* g_out, const void* e_cond, const void* e_uncond, int mo
 
 int dpm_step_cfgpp(const dpm_step_desc* desc, float g, const float* guidance, dpm_stream_t stream) {
   return step_cfgpp_impl(desc, g, guidance, static_cast<cudaStream_t>(stream));
+}
+
+int dpm_step_sde(const dpm_step_desc* desc, const dpm_sde_desc* sde, dpm_stream_t stream) {
+  return step_sde_impl(desc, sde, static_cast<cudaStream_t>(stream));
 }
 
 static dpm_step_desc base_desc(void* out, const void* x, uint64_t n, int dtype, int form) {

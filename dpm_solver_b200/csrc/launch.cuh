@@ -124,6 +124,9 @@ int launch_step_unipc(const UniParams& up, const Tuning& t, cudaStream_t stream)
 int launch_step_unipc_scalar(const UniParams& up, cudaStream_t stream);
 int launch_step_cfgpp(const CfgppParams& q, const Tuning& t, cudaStream_t stream);
 int launch_step_cfgpp_scalar(const CfgppParams& q, cudaStream_t stream);
+// one SDE-DPM-Solver++ update (step_sde.cu): p as dpm_step builds it plus the per-sample words; z NULL = drawn in-kernel
+int launch_step_sde(const KParams& p, const float* z, float cz, uint64_t seed, uint64_t offset, bool aligned_all,
+                    cudaStream_t stream);
 int launch_replicate(void* dst, const void* src, uint64_t bytes, int copies, cudaStream_t stream);
 int launch_quantile(float* s_out, const KParams& p, uint64_t n_samples, float q, float max_val,
                     void* workspace, size_t workspace_bytes, cudaStream_t stream);

@@ -27,11 +27,10 @@
 
 #include "common.cuh"
 #include "launch.cuh"
+#include "philox.cuh"
 
 namespace dpm {
 
-constexpr int kPhiloxBlock = 256;   // ATen: block_size_bound
-constexpr int kPhiloxUnroll = 4;    // curand_normal4 -> float4
 constexpr int kMaxTimes = 16;
 
 struct NoiseParams {
@@ -81,7 +80,7 @@ __global__ void __launch_bounds__(kPhiloxBlock, 4) k_noise_philox(const __grid_c
 }
 
 // ATen's calc_execution_policy for one launch over `numel` elements on the current device
-static void launch_policy(uint64_t numel, uint32_t* grid, uint64_t* counter_offset) {
+void launch_policy(uint64_t numel, uint32_t* grid, uint64_t* counter_offset) {
   int dev = 0, max_thr = 2048;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&max_thr, cudaDevAttrMaxThreadsPerMultiProcessor, dev);
@@ -96,12 +95,6 @@ static void launch_policy(uint64_t numel, uint32_t* grid, uint64_t* counter_offs
 static bool fits_32bit_indexing(uint64_t len) {
   return len <= (uint64_t)INT32_MAX && 1 + (len - 1) * sizeof(float) <= (uint64_t)INT32_MAX;
 }
-
-struct NoiseSegment {
-  uint64_t base, len;   // elements [base, base + len) of the noise tensor
-  uint64_t offset;      // philox offset of this launch, relative to the generator's offset before the draw
-  uint32_t grid;
-};
 
 // SplitUntil32Bit on the coalesced 1-D iterator: TensorIteratorBase::split gives the first len/2 elements to the
 // piece it returns, which is drawn (and split further) before the rest. Each piece takes its counter offset from
@@ -121,7 +114,7 @@ static void split_segments(uint64_t base, uint64_t len, uint64_t* offset, std::v
 
 // The launches ATen's distribution_nullary_kernel makes for a contiguous fp32 noise tensor of `numel` elements
 // (appended to *segs when it is not NULL) and the total amount they advance the generator's philox offset by
-static uint64_t noise_segments(uint64_t numel, std::vector<NoiseSegment>* segs) {
+uint64_t noise_segments(uint64_t numel, std::vector<NoiseSegment>* segs) {
   if (numel == 0) return 0;
   uint32_t grid = 0;
   uint64_t offset = 0;

@@ -100,6 +100,8 @@ class StepArgs:
     # of G - U; None is off. m_out then receives U, the x0 of e_uncond alone; `guidance_b`, when set, gives the
     # per-sample scales (else `guidance`, always combined)
     cfgpp_g: Optional[float] = None
+    # SDE-DPM-Solver++ (dpm_step_sde; form LIN1, DIFF2 or MS3): the update's Gaussian noise, None is off
+    sde: Optional["SdeNoise"] = None
 
     def state_tensors(self):
         return [t for t in (self.x, self.xe, self.m0, self.m1, self.m2) if t is not None]
@@ -112,6 +114,15 @@ class StepArgs:
             if t is not None:
                 return t
         raise ValueError("StepArgs without tensors")
+
+
+@dataclass
+class SdeNoise:
+    """The noise of one SDE-DPM-Solver++ update: out = <the update> + cz*z, z = torch.empty_like(x,
+    dtype=torch.float32).normal_(generator=generator) drawn at the launch (generator None: the default generator of x's
+    device), in x's storage order."""
+    cz: float
+    generator: Optional[torch.Generator] = None
 
 
 _raw_stream = getattr(torch._C, "_cuda_getCurrentRawStream", None)
@@ -132,6 +143,16 @@ def fdg_check(shape, levels: int, dtype=torch.float32) -> None:
     if lib.dpm_fdg_supported(int(shape[-2]), int(shape[-1]), int(levels), _DTYPE_CODE[dtype]) != 0:
         raise ValueError("frequency-decoupled guidance with x of shape {}: {}".format(
             tuple(shape), lib.dpm_last_error().decode("utf-8", "replace")))
+
+
+def same_device(a: torch.device, b: torch.device) -> bool:
+    """One device, a CUDA device without an index meaning the current one (torch.Generator("cuda") reports none)."""
+    if a.type != b.type:
+        return False
+    if a.type != "cuda":
+        return True
+    cur = torch.cuda.current_device() if (a.index is None or b.index is None) else None
+    return (cur if a.index is None else a.index) == (cur if b.index is None else b.index)
 
 
 def _dense(t: torch.Tensor) -> bool:
@@ -281,7 +302,9 @@ class CudaBackend:
                     raise ValueError("dpm_solver_b200: out2 must be dense and laid out like out")   # doubled CFG batch is)
                 d.out2 = a.out2.data_ptr()
         self._check_per_sample(a, ref)
-        if a.unipc is not None:
+        if a.sde is not None:
+            self._step_sde(a, d, ref, layout, keep)
+        elif a.unipc is not None:
             self._step_unipc(a, d, ref, sdt, layout, keep)
         elif a.e_conds is not None:
             self._step_multi(a, d, ref, sdt, layout, keep)
@@ -514,6 +537,34 @@ class CudaBackend:
             keep.append(w)
             maps[k].w, maps[k].period, maps[k].sample_stride = w.data_ptr(), period, stride
         return maps
+
+    def _step_sde(self, a: StepArgs, d, ref, layout, keep) -> None:
+        """dpm_step_sde: the update of `a` plus a.sde.cz times its noise (d already filled). The noise is drawn inside the
+        launch from the generator's (seed, offset), the generator advanced as normal_ would advance it; under CUDA-graph
+        capture, or when the launch's layout is not x's own, it is drawn by torch instead (graph-safe) and read."""
+        if a.form not in (FORM_LIN1, FORM_DIFF2, FORM_MS3) or a.c0_on_old or a.raw_round or a.coef_dev is not None \
+                or a.e_conds is not None or a.apg_words is not None or a.cfgpp_g is not None:
+            raise ValueError("dpm_solver_b200: an SDE step is a multistep LIN1 / DIFF2 / MS3 update with one scalar or "
+                             "per-sample scale, rescale, CFG-Zero* or TCFG words")
+        gen = a.sde.generator
+        if gen is not None and not same_device(gen.device, ref.device):
+            raise ValueError("dpm_solver_b200: the generator is on {}, x on {}".format(gen.device, ref.device))
+        s = _lib.SdeDesc()
+        s.cz = a.sde.cz
+        if torch.cuda.is_current_stream_capturing() or self._layout(a.x) != layout:
+            z = torch.empty_like(a.x, dtype=torch.float32).normal_(generator=gen)
+            z = self._check(z, "z", ref.device, ref.numel(), torch.float32, layout)
+            keep.append(z)
+            s.z = z.data_ptr()
+        else:
+            with torch.cuda.device(ref.device):
+                s.seed, s.offset = self._philox_state(ref.device, ref.numel(), self._lib, gen)
+        for name, v in (("guidance", a.guidance_b), ("ratio", a.ratio), ("s_star", a.cfgzero_s),
+                        ("tcfg_words", a.tcfg_w)):
+            if v is not None:
+                setattr(s, name, v.data_ptr())
+        s.phi, s.one_minus_phi = a.phi, 1.0 - a.phi
+        self._launch(ref.device, self._lib.dpm_step_sde, C.byref(d), C.byref(s))
 
     def _step_unipc(self, a: StepArgs, d, ref, sdt, layout, keep) -> None:
         """dpm_step_unipc: the UniPC words, m_{i-3} and the corrected-state output of a launch (d already filled)."""
@@ -812,7 +863,7 @@ class PreparedStep:
         if a.thr is not None or a.raw_round or a.ratio is not None or a.guidance_b is not None \
                 or a.e_conds is not None or a.coef_dev is not None or a.unipc is not None \
                 or a.apg_words is not None or a.cfgzero_s is not None or a.cfgpp_g is not None \
-                or a.tcfg_w is not None or a.out is not None and a.out2 is None:
+                or a.tcfg_w is not None or a.sde is not None or a.out is not None and a.out2 is None:
             # (a rescaled step reads a fresh ratio tensor every evaluation, an APG one fresh words, a CFG-Zero* one fresh
             # scales s*, a TCFG one fresh words (wu, wc), a CFG++ one goes through its own entry point, a guided one a
             # scales tensor the descriptor does not carry, a multi-condition one K outputs and scales it does not
@@ -920,5 +971,5 @@ def cfg_combine(eps_uncond, eps_cond, scale):
 
 
 __all__ = ["StepArgs", "CudaBackend", "backend", "set_backend", "lincomb", "cfg_combine",
-           "SUPPORTED_DTYPES", "FORM_NONE", "FORM_LIN1", "FORM_LIN2", "FORM_LIN3", "FORM_DIFF2",
+           "SdeNoise", "SUPPORTED_DTYPES", "FORM_NONE", "FORM_LIN1", "FORM_LIN2", "FORM_LIN3", "FORM_DIFF2",
            "FORM_MS3", "FORM_SS3T"]

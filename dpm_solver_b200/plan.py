@@ -43,6 +43,7 @@ class Coeffs:
     r_tensor: int = 0   # SS3T: bit 0 / 1 = r1 / r2 came as tensors (matters to reference_rounding only)
     dev: Optional[torch.Tensor] = None   # scalars live in this device block instead (on-device adaptive controller)
     g: float = 0.0      # CFG++ (dpm_step_cfgpp): alpha_t of the update's end time, the weight of G - U; 0 when not asked
+    cz: float = 0.0     # SDE-DPM-Solver++ (dpm_step_sde): sigma_t*sqrt(-expm1(-2*eta*h)), the weight of the update's noise
 
 
 def _cpu(t: torch.Tensor) -> torch.Tensor:
@@ -96,11 +97,22 @@ def first_update(ns, algorithm_type: str, s: torch.Tensor, t: torch.Tensor):
     return _first(algorithm_type, Marginals(ns, s), Marginals(ns, t))
 
 
-def _first(algorithm_type: str, ms: Marginals, mt: Marginals):
+def _sde(eta: float, h, mt: Marginals):
+    """SDE-DPM-Solver++ (eta > 0): (h_eta = (1 + eta)*h, the decay exp(-eta*h) that multiplies a, and the noise weight
+    cz = sigma_t*sqrt(-expm1(-2*eta*h))). eta == 0 gives (h, None, None): the ODE coefficients, op for op."""
+    if not eta:
+        return h, None, None
+    return (1. + eta) * h, torch.exp(-eta * h), mt.sigma * torch.sqrt(-torch.expm1(-2. * eta * h))
+
+
+def _first(algorithm_type: str, ms: Marginals, mt: Marginals, eta: float = 0.0):
     h = mt.lam - ms.lam
     if algorithm_type == "dpmsolver++":
+        h, decay, _ = _sde(eta, h, mt)
         phi_1 = torch.expm1(-h)
         a = mt.sigma / ms.sigma
+        if decay is not None:
+            a = a * decay
         c0 = -(mt.alpha * phi_1)
     else:
         phi_1 = torch.expm1(h)
@@ -121,14 +133,17 @@ def multistep_second(ns, algorithm_type, solver_type, t_prev_1, t_prev_0, t):
     return _ms2(algorithm_type, solver_type, Marginals(ns, t_prev_1), Marginals(ns, t_prev_0), Marginals(ns, t))
 
 
-def _ms2(algorithm_type, solver_type, m1: Marginals, m0: Marginals, mt: Marginals):
+def _ms2(algorithm_type, solver_type, m1: Marginals, m0: Marginals, mt: Marginals, eta: float = 0.0):
     h_0 = m0.lam - m1.lam
     h = mt.lam - m0.lam
     r0 = h_0 / h
     inv_r0 = 1. / r0
     if algorithm_type == "dpmsolver++":
+        h, decay, _ = _sde(eta, h, mt)
         phi_1 = torch.expm1(-h)
         a = mt.sigma / m0.sigma
+        if decay is not None:
+            a = a * decay
         b = mt.alpha * phi_1
         c1 = -(0.5 * b) if solver_type == "dpmsolver" else mt.alpha * (phi_1 / h + 1.)
     else:
@@ -144,7 +159,7 @@ def multistep_third(ns, algorithm_type, t_prev_2, t_prev_1, t_prev_0, t):
     return _ms3(algorithm_type, *(Marginals(ns, v) for v in (t_prev_2, t_prev_1, t_prev_0, t)))
 
 
-def _ms3(algorithm_type, m2: Marginals, m1: Marginals, m0: Marginals, mt: Marginals):
+def _ms3(algorithm_type, m2: Marginals, m1: Marginals, m0: Marginals, mt: Marginals, eta: float = 0.0):
     h_1 = m1.lam - m2.lam
     h_0 = m0.lam - m1.lam
     h = mt.lam - m0.lam
@@ -153,10 +168,13 @@ def _ms3(algorithm_type, m2: Marginals, m1: Marginals, m0: Marginals, mt: Margin
     w2 = r0 / (r0 + r1)
     w3 = 1. / (r0 + r1)
     if algorithm_type == "dpmsolver++":
+        h, decay, _ = _sde(eta, h, mt)
         phi_1 = torch.expm1(-h)
         phi_2 = phi_1 / h + 1.
         phi_3 = phi_2 / h - 0.5
         a = mt.sigma / m0.sigma
+        if decay is not None:
+            a = a * decay
         c0, c1, c2 = -(mt.alpha * phi_1), mt.alpha * phi_2, -(mt.alpha * phi_3)
     else:
         phi_1 = torch.expm1(h)
@@ -197,11 +215,14 @@ def multistep_orders(steps: int, order: int, lower_order_final: bool) -> List[in
 
 
 def multistep_plan(ns, algorithm_type, solver_type, timesteps: torch.Tensor, order: int,
-                   lower_order_final: bool, marginals: Optional[Marginals] = None, cfg_pp: bool = False) -> List[Coeffs]:
+                   lower_order_final: bool, marginals: Optional[Marginals] = None, cfg_pp: bool = False,
+                   eta: float = 0.0) -> List[Coeffs]:
     """Coefficients of every update of a multistep run; plan[i] moves timesteps[i] -> [i+1].
     One vectorised evaluation of the schedule over the grid, then one vector op set per order.
     cfg_pp=True (dpmsolver++, orders 1 and 2): each update also carries g = alpha_t of its end time, the fp32 alpha its
-    c0 = -(alpha_t*phi_1) is formed from."""
+    c0 = -(alpha_t*phi_1) is formed from.
+    eta > 0 (dpmsolver++ only): SDE-DPM-Solver++ -- h_eta = (1 + eta)*h in every phi, a multiplied by exp(-eta*h), and
+    each update carries cz = sigma_t*sqrt(-expm1(-2*eta*h)), the weight of its Gaussian noise."""
     ts = _cpu(timesteps)
     steps = ts.numel() - 1
     M = marginals if marginals is not None else Marginals(ns, ts)
@@ -210,12 +231,12 @@ def multistep_plan(ns, algorithm_type, solver_type, timesteps: torch.Tensor, ord
     idx = {p: [i for i, o in enumerate(orders) if o == p] for p in (1, 2, 3)}
     if idx[1]:
         i = torch.tensor(idx[1])
-        a, c0 = (v.reshape(-1).tolist() for v in _first(algorithm_type, M[i], M[i + 1]))
+        a, c0 = (v.reshape(-1).tolist() for v in _first(algorithm_type, M[i], M[i + 1], eta))
         for k, j in enumerate(idx[1]):
             plan[j] = Coeffs(FORM_LIN1, a[k], c0[k], order=1)
     if idx[2]:
         i = torch.tensor(idx[2])
-        a, c0, c1, w0 = (v.reshape(-1).tolist() for v in _ms2(algorithm_type, solver_type, M[i - 1], M[i], M[i + 1]))
+        a, c0, c1, w0 = (v.reshape(-1).tolist() for v in _ms2(algorithm_type, solver_type, M[i - 1], M[i], M[i + 1], eta))
         for k, j in enumerate(idx[2]):
             plan[j] = Coeffs(FORM_DIFF2, a[k], c0[k], c1[k], w0=w0[k], order=2)
     if cfg_pp:
@@ -224,10 +245,15 @@ def multistep_plan(ns, algorithm_type, solver_type, timesteps: torch.Tensor, ord
             plan[j].g = g[j + 1]
     if idx[3]:
         i = torch.tensor(idx[3])
-        v = [u.reshape(-1).tolist() for u in _ms3(algorithm_type, M[i - 2], M[i - 1], M[i], M[i + 1])]
+        v = [u.reshape(-1).tolist() for u in _ms3(algorithm_type, M[i - 2], M[i - 1], M[i], M[i + 1], eta)]
         for k, j in enumerate(idx[3]):
             plan[j] = Coeffs(FORM_MS3, v[0][k], v[1][k], v[2][k], v[3][k], w0=v[4][k], w1=v[5][k], w2=v[6][k],
                              w3=v[7][k], order=3)
+    if eta:
+        j = torch.arange(steps)
+        cz = _sde(eta, M.lam[j + 1] - M.lam[j], M[j + 1])[2].reshape(-1).tolist()
+        for k in range(steps):
+            plan[k].cz = cz[k]
     return plan  # type: ignore[return-value]
 
 

@@ -1020,8 +1020,10 @@ class DPM_Solver:
             # the reference would promote x and every update to that dtype; there are no fp64 kernels
             raise TypeError("dpm_solver_b200 computes in fp32: NoiseScheduleVP(dtype={}) is not supported "
                             "by DPM_Solver".format(tables.dtype))
-        assert algorithm_type in ["dpmsolver", "dpmsolver++"]
+        assert algorithm_type in ["dpmsolver", "dpmsolver++", "sde-dpmsolver++"]
         self.algorithm_type = algorithm_type
+        if algorithm_type == "sde-dpmsolver++":
+            self._check_sde_model(model_fn, reference_rounding)
         if correcting_x0_fn == "dynamic_thresholding":
             self.correcting_x0_fn = self.dynamic_thresholding_fn
             self._dynamic_thresholding = True
@@ -1067,6 +1069,23 @@ class DPM_Solver:
         self._prep_on = False
 
     @staticmethod
+    def _check_sde_model(model_fn, reference_rounding) -> None:
+        """The guidance forms and options SDE-DPM-Solver++ does not take: ValueError before any launch."""
+        if reference_rounding:
+            raise ValueError("reference_rounding=True reproduces the reference, which has no SDE solver")
+        for attr, what in (("perp_neg", "perp_neg"), ("cond_masks", "guidance_mask"), ("apg", "apg_eta"),
+                           ("cfg_pp", "cfg_pp")):
+            if getattr(model_fn, attr, None) not in (None, False):
+                raise ValueError("{} is not available with algorithm_type='sde-dpmsolver++'".format(what))
+        if getattr(model_fn, "n_cond", 0) >= 2:
+            raise ValueError("several conditions are not available with algorithm_type='sde-dpmsolver++'")
+
+    def _no_sde(self, what: str) -> None:
+        if self.algorithm_type == "sde-dpmsolver++":
+            raise ValueError("{} is not available with algorithm_type='sde-dpmsolver++': the SDE solver runs inside "
+                             "sample() with method='multistep'".format(what))
+
+    @staticmethod
     def _x0_hook(fn):
         """`correcting_x0_fn(x0, t)` (:379-380). The older vendored copy calls it with x0 only
         (examples/stable-diffusion/.../dpm_solver.py:447-448); a one-argument callable keeps working."""
@@ -1103,7 +1122,7 @@ class DPM_Solver:
     # -- small helpers ------------------------------------------------------------------------
     @property
     def _pp(self) -> bool:
-        return self.algorithm_type == "dpmsolver++"
+        return self.algorithm_type in ("dpmsolver++", "sde-dpmsolver++")   # data prediction
 
     def _sdtype(self, x) -> torch.dtype:
         if self.state_dtype is not None:
@@ -1501,6 +1520,7 @@ class DPM_Solver:
             x_next = self._pure_update(co, x, m_new, m1, m2, rr=rr & 4 and rr) if co is not None else None
             return m_new, x_next
         self._fill_update(a, co, x, m1, m2)
+        a.sde = self.__dict__.get("_sde_noise")
         a.want_m_out = want_m
         a.raw_round = rr
         dup = self._dup_target(x) if dup_out else None
@@ -1619,6 +1639,7 @@ class DPM_Solver:
         a = StepArgs(n_model=0, m0=self._state_like(m0, x.dtype), state_dtype=x.dtype, raw_round=rr)
         self._fill_update(a, co, x, None if m1 is None else self._state_like(m1, x.dtype),
                           None if m2 is None else self._state_like(m2, x.dtype))
+        a.sde = self.__dict__.get("_sde_noise")
         out = ops.backend().step(a)[1]
         if pkey is not None and not rr:
             self._remember(pkey, a)
@@ -1704,6 +1725,7 @@ class DPM_Solver:
     # -- reference API: single updates (direct-call path; scalars computed per call) -------------
     def dpm_solver_first_update(self, x, s, t, model_s=None, return_intermediate=False):
         """DPM-Solver-1 / DDIM step s -> t (:547-592)."""
+        self._no_sde("dpm_solver_first_update()")
         self._no_cfgpp("dpm_solver_first_update")
         x = self._state(x)
         co = P.first_update_coeffs(self.noise_schedule, self.algorithm_type, s, t)
@@ -1722,6 +1744,7 @@ class DPM_Solver:
     def singlestep_dpm_solver_second_update(self, x, s, t, r1=0.5, model_s=None, return_intermediate=False,
                                             solver_type='dpmsolver'):
         """Singlestep DPM-Solver-2 s -> t (:594-673)."""
+        self._no_sde("singlestep_dpm_solver_second_update()")
         self._no_cfgpp("singlestep_dpm_solver_second_update")
         if solver_type not in ['dpmsolver', 'taylor']:
             raise ValueError("'solver_type' must be either 'dpmsolver' or 'taylor', got {}".format(solver_type))
@@ -1734,6 +1757,7 @@ class DPM_Solver:
     def singlestep_dpm_solver_third_update(self, x, s, t, r1=1. / 3., r2=2. / 3., model_s=None, model_s1=None,
                                            return_intermediate=False, solver_type='dpmsolver'):
         """Singlestep DPM-Solver-3 s -> t (:675-794)."""
+        self._no_sde("singlestep_dpm_solver_third_update()")
         self._no_cfgpp("singlestep_dpm_solver_third_update")
         if solver_type not in ['dpmsolver', 'taylor']:
             raise ValueError("'solver_type' must be either 'dpmsolver' or 'taylor', got {}".format(solver_type))
@@ -1789,6 +1813,7 @@ class DPM_Solver:
 
     def multistep_dpm_solver_second_update(self, x, model_prev_list, t_prev_list, t, solver_type="dpmsolver"):
         """Multistep DPM-Solver-2 (:796-852)."""
+        self._no_sde("multistep_dpm_solver_second_update()")
         self._no_cfgpp("multistep_dpm_solver_second_update")
         if solver_type not in ['dpmsolver', 'taylor']:
             raise ValueError("'solver_type' must be either 'dpmsolver' or 'taylor', got {}".format(solver_type))
@@ -1797,6 +1822,7 @@ class DPM_Solver:
 
     def multistep_dpm_solver_third_update(self, x, model_prev_list, t_prev_list, t, solver_type='dpmsolver'):
         """Multistep DPM-Solver-3 (:854-904); needs exactly three buffered values."""
+        self._no_sde("multistep_dpm_solver_third_update()")
         self._no_cfgpp("multistep_dpm_solver_third_update")
         model_prev_2, model_prev_1, model_prev_0 = model_prev_list
         t_prev_2, t_prev_1, t_prev_0 = t_prev_list
@@ -1807,6 +1833,7 @@ class DPM_Solver:
     def singlestep_dpm_solver_update(self, x, s, t, order, return_intermediate=False, solver_type='dpmsolver',
                                      r1=None, r2=None):
         """Order dispatch (:906-930)."""
+        self._no_sde("singlestep_dpm_solver_update()")
         self._no_cfgpp("singlestep_dpm_solver_update")
         if order == 1:
             return self.dpm_solver_first_update(x, s, t, return_intermediate=return_intermediate)
@@ -1821,6 +1848,7 @@ class DPM_Solver:
 
     def multistep_dpm_solver_update(self, x, model_prev_list, t_prev_list, t, order, solver_type='dpmsolver'):
         """Order dispatch (:932-954)."""
+        self._no_sde("multistep_dpm_solver_update()")
         self._no_cfgpp("multistep_dpm_solver_update")
         if order == 1:
             return self.dpm_solver_first_update(x, t_prev_list[-1], t, model_s=model_prev_list[-1])
@@ -1836,6 +1864,7 @@ class DPM_Solver:
                             t_err=1e-5, solver_type='dpmsolver'):
         """Adaptive step size DPM-Solver-12 / -23 (:956-1010). Updates and the error estimate run on
         the fused kernels; the step-size controller is the reference's host logic."""
+        self._no_sde("the adaptive method")
         self._no_cfgpp("method='adaptive'")
         ns = self.noise_schedule
         x = self._state(x)
@@ -1996,6 +2025,7 @@ class DPM_Solver:
                 method='multistep', lower_order_final=True, denoise_to_zero=False, solver_type='dpmsolver',
                 atol=0.0078, rtol=0.05, return_intermediate=False):
         """Invert `x` from t_start (default 1/N) to t_end (default T) (:1032-1045)."""
+        self._no_sde("inverse()")
         t_0 = 1. / self.noise_schedule.total_N if t_start is None else t_start
         t_T = self.noise_schedule.T if t_end is None else t_end
         assert t_0 > 0 and t_T > 0, "Time range needs to be greater than 0. For discrete-time DPMs, it needs to be in [1 / N, 1], where N is the length of betas array"
@@ -2004,6 +2034,25 @@ class DPM_Solver:
                            solver_type=solver_type, atol=atol, rtol=rtol, return_intermediate=return_intermediate)
 
     # -- whole-loop CUDA graph (SURVEY 8f-1; no counterpart in the reference) -----------------------
+    def _sde_args(self, x, method, eta, generator) -> float:
+        """Validate sample()'s eta and generator: the run's eta for the SDE solver (0: the ODE run, nothing drawn), else
+        0. ValueError before any launch or network call."""
+        if self.algorithm_type != "sde-dpmsolver++":
+            if eta is not None or generator is not None:
+                raise ValueError("eta and generator are arguments of algorithm_type='sde-dpmsolver++', not {!r}".format(
+                    self.algorithm_type))
+            return 0.0
+        if method != "multistep":
+            self._no_sde("method={!r}".format(method))
+        eta = 1.0 if eta is None else eta
+        if isinstance(eta, bool) or not isinstance(eta, (int, float)) or not math.isfinite(eta) or eta < 0:
+            raise ValueError("eta must be a finite number >= 0, got {!r}".format(eta))
+        if generator is not None:
+            if not isinstance(generator, torch.Generator) or not ops.same_device(generator.device, x.device):
+                raise ValueError("the generator must be a torch.Generator on x's device {}, got {!r}".format(
+                    x.device, getattr(generator, "device", generator)))
+        return float(eta)
+
     def capture(self, x_example, **sample_kwargs):
         """Capture `sample(x, **sample_kwargs)` -- the network calls included -- in ONE CUDA graph.
 
@@ -2020,6 +2069,9 @@ class DPM_Solver:
         x_static = self._state(x_example).clone()
         self.sample(x_static, **sample_kwargs)                       # builds and caches plan + tables
         graph = torch.cuda.CUDAGraph()
+        gen = sample_kwargs.get("generator")
+        if gen is not None and hasattr(graph, "register_generator_state"):
+            graph.register_generator_state(gen)       # SDE noise from a user generator: replays advance it
         side = torch.cuda.Stream(device=x_static.device)
         side.wait_stream(torch.cuda.current_stream(x_static.device))
         with torch.cuda.stream(side):
@@ -2039,8 +2091,37 @@ class DPM_Solver:
     # -- sample (:1047-1245) ---------------------------------------------------------------------
     def sample(self, x, steps=20, t_start=None, t_end=None, order=2, skip_type='time_uniform',
                method='multistep', lower_order_final=True, denoise_to_zero=False, solver_type='dpmsolver',
-               atol=0.0078, rtol=0.05, return_intermediate=False):
-        """Integrate the diffusion ODE from t_start to t_end; arguments as in the reference."""
+               atol=0.0078, rtol=0.05, return_intermediate=False, eta=None, generator=None):
+        """Integrate the diffusion ODE from t_start to t_end; arguments as in the reference.
+
+        With algorithm_type="sde-dpmsolver++" the run integrates the diffusion SDE instead (SDE-DPM-Solver++, Lu et al.
+        2022, arXiv:2211.01095), method='multistep' only. `eta` (finite, >= 0, default 1.0) scales the noise and
+        `generator` (a torch.Generator on x's device, default: that device's default generator) draws it; passing
+        either with another algorithm_type is a ValueError. Take one update s -> t with h = lambda_t - lambda_s and
+        h_eta = (1 + eta)*h. The host forms every scalar in fp32 through torch CPU ops, as for "dpmsolver++", with h
+        replaced by h_eta in every phi and a multiplied by exp(-eta*h):
+          order 1 (LIN1):  a = (sigma_t/sigma_s)*exp(-eta*h), c0 = -(alpha_t*phi_1), phi_1 = expm1(-h_eta)
+          order 2 (DIFF2): a, c0 as order 1; c1 = -(0.5*(alpha_t*phi_1)) for solver_type="dpmsolver" (midpoint),
+                           alpha_t*(phi_1/h_eta + 1) for "taylor" (Heun); w0 = 1/r0 as for the ODE
+          order 3 (MS3):   a, c0 as order 1; phi_2 = phi_1/h_eta + 1, phi_3 = phi_2/h_eta - 0.5, c1 = alpha_t*phi_2,
+                           c2 = -(alpha_t*phi_3); w0..w3 as for the ODE
+        and the noise weight cz = sigma_t*sqrt(-expm1(-2*eta*h)). Per element, in fp32 with each op rounded and no
+        contraction, x_t = <the ODE form's expression> + cz*z, stored in the state dtype, where update i (1..steps)
+        draws z_i = torch.empty_like(x_i, dtype=torch.float32).normal_(generator=g) at that update (row-major: the
+        values of torch.randn(x.shape, generator=g); channels_last: filled in storage order). The values are
+        torch's bit for bit, drawn inside the fused update launch, and the generator ends where those calls would
+        leave it, in program order with every other consumer of it (a correcting_xt_fn, say). Under CUDA-graph
+        capture z is drawn by torch (graph-safe) and read. denoise_to_zero returns the x0 of its final evaluation and
+        draws nothing. eta=0 is the "dpmsolver++" run bit for bit and draws nothing.
+        Equivalences (in the VE coordinates x/alpha, sigma/alpha): k-diffusion's sample_dpmpp_2m_sde(eta,
+        solver_type) is order=2, lower_order_final=False with midpoint -> "dpmsolver" and heun -> "taylor";
+        sample_dpmpp_3m_sde(eta) is order=3, solver_type="taylor", lower_order_final=False (its order-2 warm-up step
+        uses the Heun phi_2); diffusers' DPMSolverMultistepScheduler(algorithm_type="sde-dpmsolver++") is eta=1.
+        Thresholding, correcting_x0_fn, correcting_xt_fn, return_intermediate, every skip_type, schedule and model type,
+        and the guidance forms uncond, classifier, classifier-free (scalar or per-sample scale, guidance_rescale,
+        cfg_zero_star, tcfg, fdg_scales) are accepted; singlestep / adaptive methods, inverse(), the direct update
+        methods, several conditions, guidance_mask, perp_neg, apg_eta, cfg_pp and reference_rounding are not."""
+        sde_eta = self._sde_args(x, method, eta, generator)
         if getattr(self._wrapped, "cfg_pp", False) and (method != "multistep" or order not in (1, 2)):
             self._no_cfgpp("method='{}' and order {}".format(method, order))
         t_0 = 1. / self.noise_schedule.total_N if t_end is None else t_end
@@ -2063,7 +2144,7 @@ class DPM_Solver:
         self._xin_pair = None
         self._rr_run = 0
         # prepared launches: the CUDA executor, no python-side x0 hook, no 16-bit reference-rounding mode
-        self._prep_on = (hasattr(ops.backend(), "prepare") and not self.reference_rounding
+        self._prep_on = (hasattr(ops.backend(), "prepare") and not self.reference_rounding and not sde_eta
                          and (self.correcting_x0_fn is None or self._dynamic_thresholding))
         with torch.no_grad(), self._apg_scope():
             x = self._state(x)
@@ -2082,13 +2163,15 @@ class DPM_Solver:
                 cfgpp = getattr(self._wrapped, "cfg_pp", False)
                 if cfgpp:
                     key = key + ("cfg_pp",)     # (the plan carries g)
+                if self.algorithm_type == "sde-dpmsolver++":
+                    key = key + ("eta", sde_eta)    # (the plan carries h_eta's coefficients and cz)
 
                 def build():
                     ts = self.get_time_steps(skip_type=skip_type, t_T=t_T, t_0=t_0, N=steps, device='cpu')
                     assert ts.shape[0] - 1 == steps
                     marg = P.Marginals(ns, ts)
-                    plan = P.multistep_plan(ns, self.algorithm_type, solver_type, ts, order, lower_order_final,
-                                            marginals=marg, cfg_pp=cfgpp)
+                    plan = P.multistep_plan(ns, "dpmsolver++" if self._pp else self.algorithm_type, solver_type, ts,
+                                            order, lower_order_final, marginals=marg, cfg_pp=cfgpp, eta=sde_eta)
                     # (alpha_t, sigma_t) per grid point: scalars of the eps->x0 / parameterisation step
                     return ts, plan, list(zip(marg.alpha_e.tolist(), marg.sigma.tolist()))
 
@@ -2111,9 +2194,15 @@ class DPM_Solver:
                     m1 = older[-1] if co.order >= 2 else None
                     m2 = older[-2] if co.order >= 3 else None
                     want = order >= 2 and step < steps
-                    m_new, x_new = self._post_model(raw, xe, ts_dev[step - 1], alsig[step - 1], co, x,
-                                                    m1, m2, want_m=want, dup_out=step < steps,
-                                                    slot=(pid, step))
+                    if sde_eta:
+                        # the update launch of this step adds cz*z, its noise drawn at that launch
+                        self._sde_noise = ops.SdeNoise(co.cz, generator)
+                    try:
+                        m_new, x_new = self._post_model(raw, xe, ts_dev[step - 1], alsig[step - 1], co, x,
+                                                        m1, m2, want_m=want, dup_out=step < steps,
+                                                        slot=(pid, step))
+                    finally:
+                        self._sde_noise = None
                     x = x_new
                     t = ts_dev[step]
                     if self.correcting_xt_fn is not None:

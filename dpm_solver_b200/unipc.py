@@ -104,6 +104,8 @@ class UniPC(DPM_Solver):
         as in DPM_Solver."""
         if variant not in ("bh1", "bh2"):
             raise ValueError("variant must be 'bh1' or 'bh2', got {!r}".format(variant))
+        if algorithm_type == "sde-dpmsolver++":
+            raise ValueError("UniPC has no SDE variant: algorithm_type='sde-dpmsolver++' is a DPM_Solver sampler")
         super().__init__(model_fn, noise_schedule, algorithm_type=algorithm_type, correcting_x0_fn=correcting_x0_fn,
                          correcting_xt_fn=correcting_xt_fn, thresholding_max_val=thresholding_max_val,
                          dynamic_thresholding_ratio=dynamic_thresholding_ratio, state_dtype=state_dtype)

@@ -30,8 +30,8 @@ extern "C" {
 
 #define DPM_B200_VERSION 108 /* 0.1.8: CFG++ (dpm_step_cfgpp); regional guidance (dpm_step_multi_masked), TCFG
                                 (dpm_tcfg_words, dpm_step_tcfg) and frequency-decoupled guidance (dpm_fdg_supported,
-                                dpm_fdg_guided) and Perp-Neg (dpm_perpneg_workspace, dpm_perpneg_words) are additions
-                                to this ABI: test for their symbols */
+                                dpm_fdg_guided), Perp-Neg (dpm_perpneg_workspace, dpm_perpneg_words) and
+                                SDE-DPM-Solver++ (dpm_step_sde) are additions to this ABI: test for their symbols */
 
 #if defined(__GNUC__)
 #define DPM_API __attribute__((visibility("default")))
@@ -456,6 +456,34 @@ DPM_API int dpm_fdg_guided(void* g_out, const void* e_cond, const void* e_uncond
  * per-sample scales over samples that do not hold whole 8-element packets by the generic kernel); never by the TMA
  * variant. */
 DPM_API int dpm_step_cfgpp(const dpm_step_desc* desc, float g, const float* guidance, dpm_stream_t stream);
+
+/* ---- SDE-DPM-Solver++ (Lu et al. 2022, arXiv:2211.01095; k-diffusion's DPM++ 2M / 3M SDE) -----------------------------
+ * dpm_step with Gaussian noise added to the update, the noise drawn inside the launch:
+ *   out = <the LIN1 / DIFF2 / MS3 expression of dpm_step> + cz*z          (fp32, each op rounded, stored as S)
+ * z is torch.randn's value for the element: element i (storage order) of `torch.empty(n).normal_(generator=g)` where g
+ * holds (seed, offset) -- the normal of ATen's grid-stride Philox4_32_10 kernel (curand_init(seed, idx, offset), one
+ * curand_normal4 per 4*G elements, G = 256*grid), split beyond 2^29 elements as ATen splits it (dpm_philox_policy gives
+ * the offset the draw consumes, to advance the generator by). With sde->z set, z is read from there instead (fp32 [n],
+ * storage order: a draw materialised by torch under CUDA-graph capture) and seed, offset are ignored.
+ * The model stage is dpm_step's, with the optional per-sample words of dpm_step_guided (guidance, ratio, phi,
+ * one_minus_phi), dpm_step_cfgzero (s_star) and dpm_step_tcfg (tcfg_words), which mean what they mean there (s_star and
+ * tcfg_words exclude each other and the ratio; any of them needs n_model == 2 and desc->per_sample dividing n).
+ * Needs desc->form LIN1, DIFF2 or MS3 with c0_on_old == 0, raw_round == 0, dev_coef == NULL and sde->offset % 4 == 0
+ * (DPM_ERR_ARG before any launch). Reads and writes the bytes dpm_step reads and writes (x, the network outputs or m0,
+ * the older buffers; out, out2, m_out) and no noise bytes: one CUDA thread draws 8 Philox blocks, the 32 normals of four
+ * 8-element packets. Packets over a tail or a segment boundary, unaligned views and per-sample words over samples that
+ * do not hold whole packets take the element path of the same launch. */
+typedef struct dpm_sde_desc {
+  const float* z;           /* NULL: draw in the launch from (seed, offset) */
+  const float* guidance;    /* per-sample scales [n/per_sample] or NULL */
+  const float* ratio;       /* guidance rescale ratio [n/per_sample] or NULL */
+  const float* s_star;      /* CFG-Zero* scales [n/per_sample] or NULL */
+  const float* tcfg_words;  /* TCFG words [n/per_sample][2] or NULL */
+  uint64_t seed, offset;
+  float cz;
+  float phi, one_minus_phi; /* rescale weights (with ratio) */
+} dpm_sde_desc;
+DPM_API int dpm_step_sde(const dpm_step_desc* desc, const dpm_sde_desc* sde, dpm_stream_t stream);
 
 /* ---- multi-condition classifier-free guidance (composable prompts, Liu et al. 2022) ----------------------------
  * The network runs once on cat([x] * (n_cond + 1)) with the conditions cat([uc, c_1, ..., c_n]) and returns
