@@ -22,7 +22,7 @@ import dataclasses
 import inspect
 import math
 from dataclasses import dataclass
-from typing import List, Optional
+from typing import List, NamedTuple, Optional
 
 import torch
 import torch.distributed as dist
@@ -40,6 +40,53 @@ _DEV = object()     # marker: the scalars of this evaluation live in device memo
 # model_wrapper
 # =================================================================================================
 
+class _Option(NamedTuple):
+    name: str           # as messages name it
+    combine: bool       # a guidance form of the combine: it runs with no other form but those _JOINED with it
+    per_sample: bool    # takes per-sample guidance scales
+    needs_uc: bool      # needs guidance_type='classifier-free' and an unconditional_condition
+    refuses: str        # the solver contexts (_CONTEXTS) it does not run in
+
+
+# The guidance options and what each runs with. A refused pair names the later option first, so this order decides
+# which of several refusals a call reports. "sde" is DPM_Solver's algorithm_type, which refuses contexts as they do.
+_OPTIONS = {
+    "several": _Option("several conditions", True, False, False, "rr sde unipc"),
+    "mask": _Option("guidance_mask", True, False, True, "rr sde unipc"),
+    "perp": _Option("perp_neg", True, False, True, "rr sde unipc"),
+    "rescale": _Option("guidance_rescale", True, True, False, "rr unipc"),
+    "apg": _Option("adaptive projected guidance (apg_eta)", True, True, True, "rr sde"),
+    "cfgzero": _Option("cfg_zero_star", True, True, True, "rr"),
+    "cfgpp": _Option("cfg_pp", True, True, True, "rr sde unipc eps x0_fn adaptive singlestep order direct"),
+    "tcfg": _Option("tcfg", True, True, True, "rr"),
+    "fdg": _Option("fdg_scales", True, False, True, "rr"),
+    "per_sample": _Option("a per-sample guidance_scale", False, True, False, "rr unipc"),
+    "zero_init": _Option("cfg_zero_init_steps > 0", False, True, False, "adaptive"),
+    "momentum": _Option("apg_momentum != 0", False, True, False, "adaptive"),
+    "sde": _Option("algorithm_type='sde-dpmsolver++'", False, True, False, "rr adaptive singlestep direct inverse"),
+}
+_JOINED = ({"several", "mask"}, {"several", "perp"})     # the forms of the multi-condition combine
+_CONTEXTS = {"rr": "reference_rounding=True", "sde": "algorithm_type='sde-dpmsolver++'", "unipc": "UniPC",
+             "eps": "algorithm_type='dpmsolver'", "x0_fn": "dynamic thresholding or a correcting_x0_fn",
+             "adaptive": "method='adaptive'", "inverse": "inverse()"}
+
+
+def _check_options(options, contexts=(), what=None) -> None:
+    """ValueError unless the guidance options `options` (keys of _OPTIONS) run together and in every solver context of
+    `contexts`; `what` names the context in the message when _CONTEXTS does not."""
+    active = [k for k in _OPTIONS if k in options]
+    for i, k in enumerate(active):
+        o = _OPTIONS[k]
+        for j in active[:i]:
+            p = _OPTIONS[j]
+            if ((o.combine and p.combine and {j, k} not in _JOINED) or (k == "per_sample" and not p.per_sample)
+                    or (j == "per_sample" and not o.per_sample)):
+                raise ValueError("{} is not available with {}".format(o.name, p.name))
+        for c in contexts:
+            if c in o.refuses.split():
+                raise ValueError("{} is not available with {}".format(o.name, what or _CONTEXTS[c]))
+
+
 @dataclass
 class RawOutput:
     """Network output(s) before parameterisation / guidance have been applied."""
@@ -47,7 +94,6 @@ class RawOutput:
     e_uncond: Optional[torch.Tensor]
     param: int
     guidance: float
-    phi: float = 0.0        # guidance rescale of the combine (model_wrapper's guidance_rescale); 0 = off
     guidance_b: Optional[torch.Tensor] = None   # per-sample scales, fp32 [B] (then `guidance` is not read)
     # multi-condition guidance (K >= 2 conditions): the K conditional outputs in condition order (`e_cond` is the first)
     # and their fp32-rounded scales; `guidance` is then not read
@@ -55,17 +101,16 @@ class RawOutput:
     scales: Optional[tuple] = None
     masks: Optional[tuple] = None   # regional guidance: one _CondMask or None (all ones) per condition, with e_conds
     is_x0: bool = False     # `e_cond` is a materialised x0 (a guided flow or EDM prediction): it is only clamped, not converted
-    apg: Optional[tuple] = None     # adaptive projected guidance of the combine: (eta, norm_threshold, momentum)
-    cfgzero: bool = False           # CFG-Zero*: the combine against s*-scaled `e_uncond` (model_wrapper's cfg_zero_star)
-    cfgpp: bool = False             # CFG++: an update buffers U (e_uncond alone) and adds g*(G - U) (model_wrapper's cfg_pp)
-    tcfg: bool = False              # TCFG: the combine against the damped `e_uncond` (model_wrapper's tcfg)
-    # frequency-decoupled guidance (model_wrapper's fdg_scales): (scales, levels), the scales `levels` python floats or
-    # an fp32 [B, levels] tensor on the outputs' device; the solver turns the pair into one output g (dpm_fdg_guided)
+    # the guidance form of the combine, a key of _OPTIONS ("" for plain guidance), and its host constants: (phi,) for
+    # "rescale", (eta, norm_threshold, momentum) for "apg"
+    form: str = ""
+    consts: tuple = ()
+    # frequency-decoupled guidance (form "fdg"): (scales, levels), the scales `levels` python floats or an fp32
+    # [B, levels] tensor on the outputs' device; the solver turns the pair into one output g (dpm_fdg_guided)
     fdg: Optional[tuple] = None
-    perp: bool = False              # Perp-Neg: conditions 2..K projected off condition 1's (model_wrapper's perp_neg)
 
 
-def _multi_condition(condition, unconditional_condition, guidance_scale, guidance_rescale, masked=False):
+def _multi_condition(condition, unconditional_condition, guidance_scale, masked=False):
     """model_wrapper's list or tuple of conditions -> (condition, guidance_scale, per-condition scales or None).
     One condition is the tensor form (its scale as one python float); K >= 2 conditions, or any K with guidance masks,
     keep their K scales, each read on the host once and rounded to fp32 once."""
@@ -87,8 +132,6 @@ def _multi_condition(condition, unconditional_condition, guidance_scale, guidanc
         return condition[0], scales[0], None
     if unconditional_condition is None:
         raise ValueError("classifier-free guidance with {} conditions needs an unconditional_condition".format(K))
-    if guidance_rescale != 0:
-        raise ValueError("guidance_rescale is not available with several conditions")
     return tuple(condition), scales, scales
 
 
@@ -145,21 +188,33 @@ class _CondMask:
         return _CondMask(m[rows])
 
 
-def _cfg_ratio(be, raw: RawOutput) -> Optional[torch.Tensor]:
-    """Per-sample ratio std(out_c)/std(g) of a rescaled CFG evaluation (device fp32 [B]); None without rescale."""
-    if raw.phi == 0 or raw.e_uncond is None:
-        return None
-    fn = getattr(be, "cfg_rescale_ratio", None)
-    if fn is None:
-        raise RuntimeError("guidance_rescale needs an executor with cfg_rescale_ratio; {} has none".format(
-            getattr(be, "name", type(be).__name__)))
-    return fn(raw.e_cond, raw.e_uncond, raw.guidance if raw.guidance_b is None else raw.guidance_b)
+def _words(be, raw: RawOutput) -> Optional[torch.Tensor]:
+    """The per-sample words pass of a guided evaluation over both raw halves (2 launches; each sample's words read its
+    own values only): the rescale ratio std(out_c)/std(g), CFG-Zero*'s s* or TCFG's (wu, wc). None for other forms."""
+    if raw.form == "rescale":
+        fn = getattr(be, "cfg_rescale_ratio", None)
+        if fn is None:
+            raise RuntimeError("guidance_rescale needs an executor with cfg_rescale_ratio; {} has none".format(
+                getattr(be, "name", type(be).__name__)))
+        return fn(raw.e_cond, raw.e_uncond, raw.guidance if raw.guidance_b is None else raw.guidance_b)
+    if raw.form == "cfgzero":
+        return be.cfgzero_scale(raw.e_cond, raw.e_uncond)
+    if raw.form == "tcfg":
+        return be.tcfg_words(raw.e_cond, raw.e_uncond)
+    return None
 
 
-def _guidance_args(a: StepArgs, ratio: Optional[torch.Tensor], raw: RawOutput, rows=None) -> StepArgs:
-    """The rescale ratio and the per-sample scales (rows `rows` of them) of `raw` on a CFG step."""
-    if ratio is not None:
-        a.ratio, a.phi = ratio, raw.phi
+def _guidance_args(a: StepArgs, words: Optional[torch.Tensor], raw: RawOutput, rows=None) -> StepArgs:
+    """The guidance of `raw` on a step (rows `rows` of its per-sample fields): its per-sample words (`_words`), its
+    per-sample scales, and the outputs, scales and masks of several conditions."""
+    if words is not None:
+        w = words if rows is None else words[rows]
+        if raw.form == "rescale":
+            a.ratio, a.phi = w, raw.consts[0]
+        elif raw.form == "cfgzero":
+            a.cfgzero_s = w
+        else:
+            a.tcfg_w = w
     if raw.guidance_b is not None and a.n_model == 2:
         a.guidance_b = raw.guidance_b if rows is None else raw.guidance_b[rows]
     if raw.e_conds is not None and a.n_model == 2:
@@ -168,7 +223,7 @@ def _guidance_args(a: StepArgs, ratio: Optional[torch.Tensor], raw: RawOutput, r
         if raw.masks is not None:
             d = raw.e_cond.dim()
             a.masks = raw.masks if rows is None else tuple(m if m is None else _map_rows(m, rows, d) for m in raw.masks)
-    if a.ratio is not None or a.guidance_b is not None or a.masks is not None:
+    if words is not None or a.guidance_b is not None or a.masks is not None:
         a.per_sample = a.e_cond.numel() // a.e_cond.shape[0]
     return a
 
@@ -193,7 +248,7 @@ def _perp_output(be, raw: RawOutput) -> RawOutput:
     w = fn(raw.e_uncond, raw.e_conds, raw.scales)
     K = len(raw.scales)
     return dataclasses.replace(raw, scales=(1.0,) + tuple(raw.scales[1:]), masks=((w, 1, 1),) + (None,) * (K - 1),
-                               perp=False)
+                               form="")
 
 
 def _apg_args(be, raw: RawOutput, xe, marg, sdtype, x0: bool, ns, coef_dev=None, r_prev=None, r_out=None) -> StepArgs:
@@ -201,7 +256,7 @@ def _apg_args(be, raw: RawOutput, xe, marg, sdtype, x0: bool, ns, coef_dev=None,
     both halves converted to x0 with the marginals `marg` = (alpha_t, sigma_t) (EDM: its x0 words), or with those of the
     device block `coef_dev` when `marg` is None; the guided x0 buffered when `x0`, else converted to eps with the same
     marginals. r_prev / r_out: the momentum buffer (read / written), or None."""
-    eta, norm_threshold, momentum = raw.apg
+    eta, norm_threshold, momentum = raw.consts
     al, sg = marg if marg is not None else (1.0, 0.0)
     a = StepArgs(n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=raw.param, guidance=raw.guidance,
                  predict_x0=x0, xe=xe, alpha_e=al, sigma_e=sg, alpha_t=al, sigma_t=sg, state_dtype=sdtype,
@@ -304,7 +359,7 @@ class WrappedModel:
             None if m is None else _CondMask(m) for m in guidance_mask)
         if guidance_type == "classifier-free" and isinstance(condition, (list, tuple)):
             condition, guidance_scale, self.cond_scales = _multi_condition(
-                condition, unconditional_condition, guidance_scale, guidance_rescale, self.cond_masks is not None)
+                condition, unconditional_condition, guidance_scale, self.cond_masks is not None)
         self.condition = condition
         self.unconditional_condition = unconditional_condition
         if isinstance(guidance_scale, (list, tuple)) and self.cond_scales is None:
@@ -342,6 +397,32 @@ class WrappedModel:
     def n_cond(self) -> int:
         """Number of conditions of a multi-condition run (K >= 2, or K >= 1 with guidance masks), else 0."""
         return 0 if self.cond_scales is None else len(self.cond_scales)
+
+    def guidance_options(self) -> frozenset:
+        """The guidance options (keys of _OPTIONS) the wrapper's attributes select now."""
+        if self.guidance_type != "classifier-free":
+            return frozenset()
+        return frozenset(k for k, on in (
+            ("several", self.n_cond >= 2), ("mask", self.cond_masks is not None), ("perp", self.perp_neg),
+            ("rescale", self.guidance_rescale != 0), ("apg", self.apg is not None), ("cfgzero", self.cfg_zero_star),
+            ("cfgpp", self.cfg_pp), ("tcfg", self.tcfg), ("fdg", self.fdg_levels > 0),
+            ("per_sample", self._scale_vec is not None), ("zero_init", self.cfg_zero_init_steps > 0),
+            ("momentum", self.apg is not None and self.apg[2] != 0)) if on)
+
+    def _form(self, plain: bool) -> tuple:
+        """(form, host constants) of a guided evaluation of the two halves, as the wrapper's attributes select it now
+        (`plain`: the plain guided noise of a direct call, never CFG++)."""
+        if self.apg is not None:
+            return "apg", self.apg
+        if self.cfg_zero_star:
+            return "cfgzero", ()
+        if self.cfg_pp and not plain:
+            return "cfgpp", ()
+        if self.tcfg:
+            return "tcfg", ()
+        if self.guidance_rescale != 0:
+            return "rescale", (self.guidance_rescale,)
+        return "", ()
 
     def _one_scale(self):
         """The single guidance scale as the host reads it. A 0-dim or one-element tensor is read once per (tensor,
@@ -457,24 +538,21 @@ class WrappedModel:
             t_in = None if t_input is not None else torch.cat([t_continuous] * n)
             outs = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(n)   # uncond first
             return RawOutput(outs[1], outs[0], param, 1.0, e_conds=tuple(outs[1:]), scales=self.cond_scales,
-                             masks=self.cond_masks, perp=self.perp_neg)
+                             masks=self.cond_masks, form="perp" if self.perp_neg else "")
         if self.guidance_type == "classifier-free":
             gb = self._scales(x) if self._scale_vec is not None else None     # (checked before the network runs)
             fdg = self.fdg_args(x) if self.fdg_levels else None               # likewise
             if not ((self._combines() or self.fdg_levels > 0) if plain else self.uses_cfg):
                 return RawOutput(self._call_model(x, t_continuous, cond=self.condition, t_input=t_input), None, param, 1.0)
-            cfgpp = self.cfg_pp and not plain
             if x_in is None:
                 x_in = ops.backend().duplicate(x)              # cat([x] * 2) :326 (the solver hands over a prebuilt one)
             t_in = None if t_input is not None else torch.cat([t_continuous] * 2)
             out_u, out_c = self._call_model(x_in, t_in, cond=self._cond_in(), t_input=t_input).chunk(2)  # uncond first
             if fdg is not None:
-                return RawOutput(out_c, out_u, param, 1.0, fdg=fdg)
-            if gb is not None:
-                return RawOutput(out_c, out_u, param, 1.0, self.guidance_rescale, gb, apg=self.apg,
-                                 cfgzero=self.cfg_zero_star, cfgpp=cfgpp, tcfg=self.tcfg)
-            return RawOutput(out_c, out_u, param, float(self._one_scale()), self.guidance_rescale, apg=self.apg,
-                             cfgzero=self.cfg_zero_star, cfgpp=cfgpp, tcfg=self.tcfg)
+                return RawOutput(out_c, out_u, param, 1.0, form="fdg", fdg=fdg)
+            form, consts = self._form(plain)
+            return RawOutput(out_c, out_u, param, 1.0 if gb is not None else float(self._one_scale()), gb, form=form,
+                             consts=consts)
         raise RuntimeError("raw() is not available with classifier guidance")
 
     def _alpha_sigma(self, t_continuous):
@@ -520,13 +598,13 @@ class WrappedModel:
                 return ops.lincomb(o, [grad[rows]], 1.0, [-gs])
             return self._per_sample(pairs, x.shape[0], guided)
         r = self.raw(x, t_continuous, plain=True)
-        if r.fdg is not None:
+        if r.form == "fdg":
             r = _fdg_output(be, r)        # g, then converted as one network output
-        if r.perp:
+        if r.form == "perp":
             r = _perp_output(be, r)       # over the whole batch: each sample's word reads its own values only
         if r.e_uncond is None and r.param == PARAM_NOISE:
             return r.e_cond
-        if r.apg is not None and r.e_uncond is not None:
+        if r.form == "apg":
             # adaptive projected guidance: the words pass, then the guided x0 converted to noise (a direct call is the
             # first evaluation of its own: no momentum)
             xo = x.to(r.e_cond.dtype)
@@ -543,19 +621,13 @@ class WrappedModel:
             pairs = [self.noise_schedule.conversion_words(al, sg, False) for al, sg in pairs]   # eps words
         needs_x = r.param in (PARAM_BY_NAME["x_start"], PARAM_BY_NAME["v"], PARAM_FLOW, PARAM_EDM)
         xo = x.to(r.e_cond.dtype) if needs_x else None
-        ratio = _cfg_ratio(be, r)      # over the whole batch: each sample's ratio reads its own values only
-        zs = be.cfgzero_scale(r.e_cond, r.e_uncond) if r.cfgzero and r.e_uncond is not None else None   # likewise
-        tw = be.tcfg_words(r.e_cond, r.e_uncond) if r.tcfg and r.e_uncond is not None else None         # likewise
+        words = _words(be, r)          # over the whole batch: each sample's words read its own values only
 
         def convert(rows, alpha, sigma):
             a = StepArgs(form=FORM_NONE, n_model=2 if r.e_uncond is not None else 1, e_cond=r.e_cond[rows],
                          e_uncond=None if r.e_uncond is None else r.e_uncond[rows], param=r.param,
                          guidance=r.guidance, alpha_e=alpha, sigma_e=sigma, state_dtype=r.e_cond.dtype)
-            _guidance_args(a, None if ratio is None else ratio[rows], r, rows)
-            if zs is not None:
-                a.cfgzero_s, a.per_sample = zs[rows], a.e_cond.numel() // a.e_cond.shape[0]
-            if tw is not None:
-                a.tcfg_w, a.per_sample = tw[rows], a.e_cond.numel() // a.e_cond.shape[0]
+            _guidance_args(a, words, r, rows)
             if needs_x:
                 a.xe = xo[rows]
             return be.step(a)[0]
@@ -845,13 +917,6 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
             raise ValueError("apg_norm_threshold and apg_momentum need apg_eta")
     else:
         apg_eta = float(apg_eta)
-        if guidance_type != "classifier-free" or unconditional_condition is None:
-            raise ValueError("adaptive projected guidance needs guidance_type='classifier-free' and an "
-                             "unconditional_condition")
-        if isinstance(condition, (list, tuple)) and len(condition) >= 2:
-            raise ValueError("adaptive projected guidance is not available with several conditions")
-        if guidance_rescale != 0:
-            raise ValueError("adaptive projected guidance is not available with guidance_rescale")
         if not (math.isfinite(apg_eta) and math.isfinite(apg_momentum)):
             raise ValueError("apg_eta and apg_momentum must be finite, got {} and {}".format(apg_eta, apg_momentum))
         if not (math.isfinite(apg_norm_threshold) and apg_norm_threshold >= 0):
@@ -860,93 +925,49 @@ def model_wrapper(model, noise_schedule, model_type="noise", model_kwargs={}, gu
         raise ValueError("cfg_zero_init_steps must be an int >= 0, got {!r}".format(cfg_zero_init_steps))
     if cfg_zero_init_steps and not cfg_zero_star:
         raise ValueError("cfg_zero_init_steps needs cfg_zero_star=True")
-    if not isinstance(cfg_pp, bool):
-        raise ValueError("cfg_pp must be a bool, got {!r}".format(cfg_pp))
-    if cfg_pp:
-        if guidance_type != "classifier-free" or unconditional_condition is None:
-            raise ValueError("cfg_pp needs guidance_type='classifier-free' and an unconditional_condition")
-        if isinstance(condition, (list, tuple)) and len(condition) >= 2:
-            raise ValueError("cfg_pp is not available with several conditions")
-        if guidance_rescale != 0:
-            raise ValueError("cfg_pp is not available with guidance_rescale")
-        if apg_eta is not None:
-            raise ValueError("cfg_pp is not available with adaptive projected guidance (apg_eta)")
-        if cfg_zero_star:
-            raise ValueError("cfg_pp is not available with cfg_zero_star")
-    if not isinstance(tcfg, bool):
-        raise ValueError("tcfg must be a bool, got {!r}".format(tcfg))
-    if tcfg:
-        if guidance_type != "classifier-free" or unconditional_condition is None:
-            raise ValueError("tcfg needs guidance_type='classifier-free' and an unconditional_condition")
-        if isinstance(condition, (list, tuple)) and len(condition) >= 2:
-            raise ValueError("tcfg is not available with several conditions")
-        if guidance_mask is not None:
-            raise ValueError("tcfg is not available with guidance_mask")
-        if guidance_rescale != 0:
-            raise ValueError("tcfg is not available with guidance_rescale")
-        if apg_eta is not None:
-            raise ValueError("tcfg is not available with adaptive projected guidance (apg_eta)")
-        if cfg_zero_star:
-            raise ValueError("tcfg is not available with cfg_zero_star")
-        if cfg_pp:
-            raise ValueError("tcfg is not available with cfg_pp")
+    for name, v in (("cfg_pp", cfg_pp), ("tcfg", tcfg), ("perp_neg", perp_neg)):
+        if not isinstance(v, bool):
+            raise ValueError("{} must be a bool, got {!r}".format(name, v))
+    cf, many = guidance_type == "classifier-free", isinstance(condition, (list, tuple))
+    options = {k for k, on in (
+        ("several", cf and many and len(condition) >= 2), ("mask", guidance_mask is not None), ("perp", perp_neg),
+        ("rescale", guidance_rescale != 0), ("apg", apg_eta is not None), ("cfgzero", cfg_zero_star),
+        ("cfgpp", cfg_pp), ("tcfg", tcfg), ("fdg", fdg_scales is not None),
+        ("per_sample", cf and _per_sample_scales(condition, guidance_scale)),
+        ("zero_init", cfg_zero_init_steps > 0), ("momentum", apg_momentum != 0)) if on}
+    for k in options:
+        if _OPTIONS[k].needs_uc and (not cf or unconditional_condition is None):
+            raise ValueError("{} needs guidance_type='classifier-free' and an unconditional_condition".format(
+                _OPTIONS[k].name))
+    if perp_neg and (not many or len(condition) < 2):
+        raise ValueError("perp_neg needs a list of at least two conditions: the positive prompt first, then the "
+                         "negatives")
+    _check_options(options)
     if fdg_scales is not None:
-        if guidance_type != "classifier-free" or unconditional_condition is None:
-            raise ValueError("fdg_scales needs guidance_type='classifier-free' and an unconditional_condition")
-        if isinstance(condition, (list, tuple)) and len(condition) >= 2:
-            raise ValueError("fdg_scales is not available with several conditions")
-        if guidance_mask is not None:
-            raise ValueError("fdg_scales is not available with guidance_mask")
-        if guidance_rescale != 0:
-            raise ValueError("fdg_scales is not available with guidance_rescale")
-        if apg_eta is not None:
-            raise ValueError("fdg_scales is not available with adaptive projected guidance (apg_eta)")
-        if cfg_zero_star:
-            raise ValueError("fdg_scales is not available with cfg_zero_star")
-        if cfg_pp:
-            raise ValueError("fdg_scales is not available with cfg_pp")
-        if tcfg:
-            raise ValueError("fdg_scales is not available with tcfg")
-        if torch.is_tensor(guidance_scale) and guidance_scale.numel() != 1:
-            raise ValueError("fdg_scales replaces guidance_scale: give per-sample scales as a [B, N] fdg_scales tensor")
         if torch.is_tensor(guidance_scale) or guidance_scale != 1.:
             raise ValueError("fdg_scales replaces guidance_scale, which must stay at its default 1.0, got {!r}".format(
                 guidance_scale))
         _fdg_scales(fdg_scales)                       # (the form and the number of levels)
-    if not isinstance(perp_neg, bool):
-        raise ValueError("perp_neg must be a bool, got {!r}".format(perp_neg))
-    if perp_neg:
-        if guidance_type != "classifier-free" or unconditional_condition is None:
-            raise ValueError("perp_neg needs guidance_type='classifier-free' and an unconditional_condition")
-        if not isinstance(condition, (list, tuple)) or len(condition) < 2:
-            raise ValueError("perp_neg needs a list of at least two conditions: the positive prompt first, then the "
-                             "negatives")
-        if guidance_mask is not None:
-            raise ValueError("perp_neg is not available with guidance_mask")
     if guidance_mask is not None:
-        condition, guidance_scale, guidance_mask = _masked_arguments(
-            guidance_type, condition, unconditional_condition, guidance_scale, guidance_mask, guidance_rescale,
-            apg_eta, cfg_zero_star, cfg_pp)
-    if cfg_zero_star:
-        if guidance_type != "classifier-free" or unconditional_condition is None:
-            raise ValueError("cfg_zero_star needs guidance_type='classifier-free' and an unconditional_condition")
-        if isinstance(condition, (list, tuple)) and len(condition) >= 2:
-            raise ValueError("cfg_zero_star is not available with several conditions")
-        if guidance_rescale != 0:
-            raise ValueError("cfg_zero_star is not available with guidance_rescale")
-        if apg_eta is not None:
-            raise ValueError("cfg_zero_star is not available with adaptive projected guidance (apg_eta)")
+        condition, guidance_scale, guidance_mask = _masked_arguments(condition, guidance_scale, guidance_mask)
     return WrappedModel(model, noise_schedule, model_type, model_kwargs, guidance_type, condition,
                         unconditional_condition, guidance_scale, classifier_fn, classifier_kwargs, guidance_rescale,
                         apg_eta, apg_norm_threshold, apg_momentum, cfg_zero_star, cfg_zero_init_steps, cfg_pp,
                         guidance_mask, tcfg, fdg_scales, perp_neg)
 
 
-def _masked_arguments(guidance_type, condition, unconditional_condition, guidance_scale, guidance_mask,
-                      guidance_rescale, apg_eta, cfg_zero_star, cfg_pp):
+def _per_sample_scales(condition, s) -> bool:
+    """Whether model_wrapper's guidance_scale holds one scale per sample: a tensor of several values for one condition,
+    or a 2-D tensor or entries of several values for a list of conditions."""
+    many = isinstance(condition, (list, tuple))
+    if torch.is_tensor(s):
+        return s.dim() >= 2 if many else s.numel() != 1
+    return isinstance(s, (list, tuple)) and ((not many and len(s) != 1) or
+                                             any(torch.is_tensor(v) and v.numel() != 1 for v in s))
+
+
+def _masked_arguments(condition, guidance_scale, guidance_mask):
     """model_wrapper's arguments of a run with guidance masks, validated: (K conditions, their scales, K masks)."""
-    if guidance_type != "classifier-free" or unconditional_condition is None:
-        raise ValueError("guidance_mask needs guidance_type='classifier-free' and an unconditional_condition")
     many = isinstance(condition, (list, tuple))
     conds = list(condition) if many else [condition]
     masks = list(guidance_mask) if isinstance(guidance_mask, (list, tuple)) else [guidance_mask]
@@ -955,18 +976,6 @@ def _masked_arguments(guidance_type, condition, unconditional_condition, guidanc
     if any(m is not None and not torch.is_tensor(m) for m in masks):
         raise ValueError("each guidance_mask entry must be a tensor or None")
     s = guidance_scale
-    per_sample = (torch.is_tensor(s) and (s.dim() >= 2 or (not many and s.numel() != 1))) or \
-        (isinstance(s, (list, tuple)) and any(torch.is_tensor(v) and v.numel() != 1 for v in s))
-    if per_sample:
-        raise ValueError("a per-sample guidance_scale is not available with guidance_mask; use a [B, 1, 1, 1] mask")
-    if guidance_rescale != 0:
-        raise ValueError("guidance_rescale is not available with guidance_mask")
-    if apg_eta is not None:
-        raise ValueError("adaptive projected guidance (apg_eta) is not available with guidance_mask")
-    if cfg_zero_star:
-        raise ValueError("cfg_zero_star is not available with guidance_mask")
-    if cfg_pp:
-        raise ValueError("cfg_pp is not available with guidance_mask")
     if not many:
         s = [float(s)] if torch.is_tensor(s) else [s]
     elif isinstance(s, (list, tuple)):
@@ -1022,8 +1031,9 @@ class DPM_Solver:
                             "by DPM_Solver".format(tables.dtype))
         assert algorithm_type in ["dpmsolver", "dpmsolver++", "sde-dpmsolver++"]
         self.algorithm_type = algorithm_type
-        if algorithm_type == "sde-dpmsolver++":
-            self._check_sde_model(model_fn, reference_rounding)
+        self._refuse(*(c for c, on in (("rr", reference_rounding), ("sde", algorithm_type == "sde-dpmsolver++"),
+                                       ("eps", algorithm_type == "dpmsolver"), ("x0_fn", correcting_x0_fn is not None))
+                       if on))
         if correcting_x0_fn == "dynamic_thresholding":
             self.correcting_x0_fn = self.dynamic_thresholding_fn
             self._dynamic_thresholding = True
@@ -1041,49 +1051,19 @@ class DPM_Solver:
         if self.reference_rounding and getattr(noise_schedule, "schedule", None) in ("flow", "edm"):
             raise ValueError("reference_rounding=True reproduces the reference, which has no {} schedule".format(
                 noise_schedule.schedule))
-        if self.reference_rounding and getattr(model_fn, "guidance_rescale", 0) != 0:
-            raise ValueError("guidance_rescale is not available with reference_rounding=True")
-        if self.reference_rounding and getattr(model_fn, "per_sample_guidance", False):
-            raise ValueError("a per-sample guidance_scale is not available with reference_rounding=True")
-        if self.reference_rounding and getattr(model_fn, "n_cond", 0) >= 2:
-            raise ValueError("several conditions are not available with reference_rounding=True")
-        if self.reference_rounding and getattr(model_fn, "cond_masks", None) is not None:
-            raise ValueError("guidance_mask is not available with reference_rounding=True")
-        if self.reference_rounding and getattr(model_fn, "apg", None) is not None:
-            raise ValueError("adaptive projected guidance is not available with reference_rounding=True")
-        if self.reference_rounding and getattr(model_fn, "cfg_zero_star", False):
-            raise ValueError("cfg_zero_star is not available with reference_rounding=True")
-        if self.reference_rounding and getattr(model_fn, "tcfg", False):
-            raise ValueError("tcfg is not available with reference_rounding=True")
-        if self.reference_rounding and getattr(model_fn, "fdg_levels", 0):
-            raise ValueError("fdg_scales is not available with reference_rounding=True")
-        if getattr(model_fn, "cfg_pp", False):
-            if algorithm_type != "dpmsolver++":
-                raise ValueError("cfg_pp needs algorithm_type='dpmsolver++' (CFG++ re-noises a data prediction)")
-            if correcting_x0_fn is not None:
-                raise ValueError("cfg_pp is not available with dynamic thresholding or a correcting_x0_fn")
-            if self.reference_rounding:
-                raise ValueError("cfg_pp is not available with reference_rounding=True")
         self._rr_run = 0     # raw_round of the buffered values of the run in flight (reference_rounding)
         self._prep_cache = {}   # frozen launch descriptors of cached plan steps (ops.PreparedStep)
         self._prep_on = False
 
-    @staticmethod
-    def _check_sde_model(model_fn, reference_rounding) -> None:
-        """The guidance forms and options SDE-DPM-Solver++ does not take: ValueError before any launch."""
-        if reference_rounding:
-            raise ValueError("reference_rounding=True reproduces the reference, which has no SDE solver")
-        for attr, what in (("perp_neg", "perp_neg"), ("cond_masks", "guidance_mask"), ("apg", "apg_eta"),
-                           ("cfg_pp", "cfg_pp")):
-            if getattr(model_fn, attr, None) not in (None, False):
-                raise ValueError("{} is not available with algorithm_type='sde-dpmsolver++'".format(what))
-        if getattr(model_fn, "n_cond", 0) >= 2:
-            raise ValueError("several conditions are not available with algorithm_type='sde-dpmsolver++'")
+    def _options(self) -> frozenset:
+        """The guidance options of the model function (none for a plain callable), and "sde" for the SDE solver."""
+        w = self._wrapped
+        options = w.guidance_options() if isinstance(w, WrappedModel) else frozenset()
+        return options | {"sde"} if self.algorithm_type == "sde-dpmsolver++" else options
 
-    def _no_sde(self, what: str) -> None:
-        if self.algorithm_type == "sde-dpmsolver++":
-            raise ValueError("{} is not available with algorithm_type='sde-dpmsolver++': the SDE solver runs inside "
-                             "sample() with method='multistep'".format(what))
+    def _refuse(self, *contexts, what=None) -> None:
+        """ValueError unless the options run in the solver contexts `contexts` (_check_options)."""
+        _check_options(self._options(), contexts, what)
 
     @staticmethod
     def _x0_hook(fn):
@@ -1342,27 +1322,27 @@ class DPM_Solver:
         `slot` names a step of a CACHED coefficient plan (sample() loops): its launch descriptor is frozen after
         the first run (ops.PreparedStep) and later runs only patch tensor pointers -- the steady-state host path."""
         be = ops.backend()
-        fdg = raw.fdg is not None
-        if fdg:
+        guided = (raw.form, raw.consts)
+        if raw.form == "fdg":
             # frequency-decoupled guidance: the pyramid pass over both raw halves (+1 launch) gives g in the network's
             # dtype, handed on as one network output of the same parameterisation; everything below is the one-output
             # path (the fused step with out / out2, the quantile, UniPC, device coefficients)
             raw = _fdg_output(be, raw)
-        if raw.perp:
+        if raw.form == "perp":
             # Perp-Neg: the words pass over the K+1 raw outputs (+2 launches) gives condition 1's per-sample weight;
             # from here on the evaluation is a regional-guidance one (the masked fused step with its replicas, the fp32
             # materialisation for the quantile, the correcting_x0_fn split, device coefficients)
             raw = _perp_output(be, raw)
         pkey = None
         if slot is not None and self._prep_on:
-            # (phi is part of the key: a rescaled evaluation is never served by a launch frozen without the rescale)
+            # (the guidance form and its constants are part of the key: a launch frozen for one form never serves
+            # another)
             # (and so is a per-sample scale: a guided evaluation never meets a launch frozen with one scale)
             # (and so are the scales of several conditions: such a step is never frozen, and a key with them cannot
             # meet a launch frozen for one condition)
             # (and so is dynamic thresholding: a launch frozen without the clamp never serves a solver switched to it)
-            pkey = (slot, raw.param, raw.guidance, raw.phi, raw.guidance_b is None, raw.e_uncond is None,
-                    raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, raw.scales, self._dynamic_thresholding,
-                    raw.apg, raw.cfgzero, raw.cfgpp, raw.tcfg, fdg)
+            pkey = (slot, raw.param, raw.guidance, raw.scales, raw.guidance_b is None, raw.e_uncond is None,
+                    raw.e_cond.dtype, xe.dtype, xe.shape, want_m, dup_out, self._dynamic_thresholding, guided)
             prep = self._prep_cache.get(pkey)
             if prep is not None:
                 r = prep.launch((x, xe, raw.e_cond, m1, m2, raw.e_cond, raw.e_uncond))
@@ -1373,17 +1353,18 @@ class DPM_Solver:
                     if m_new is None and prep.d.n_model == 0:
                         m_new = raw.e_cond                  # pure update on the raw noise: it IS the buffered value
                     return m_new, x_next
-        if raw.cfgpp and co is not None:
+        if raw.form == "cfgpp" and co is not None:
             return self._cfgpp_step(raw, xe, alsig, co, x, m1, want_m, dup_out)
         x0 = self._pp if x0 is None else x0          # buffered value: x0 (dpmsolver++ / data_prediction_fn) or eps
         sd = xe.dtype if xe is not None else (x.dtype if x is not None else raw.e_cond.dtype)
         custom_fix = x0 and self.correcting_x0_fn is not None and not self._dynamic_thresholding
+        thresholded = x0 and self._dynamic_thresholding
         code = self._rr_code(raw)
         rr = 0
         q_raw = None        # what the quantile reads, when not `raw` itself
         apg_a = None        # the step arguments of an adaptive-projected-guidance evaluation
         split = False       # the buffered value and the update in two launches
-        if raw.apg is not None and raw.e_uncond is not None:
+        if raw.form == "apg":
             # the words pass (+2 launches), then the fused step. With dynamic thresholding (the quantile takes one
             # plain combine) the guided x0 is materialised once in fp32 (+1 launch) and handed on as one network output.
             # Under UniPC, whose launch converts at its own state and takes one network output, a FORM_NONE launch
@@ -1394,7 +1375,6 @@ class DPM_Solver:
                 marg, cdev = None, co.dev
             else:
                 marg, cdev = (alsig if isinstance(alsig, tuple) else self._alpha_sigma(alsig)), None
-            thresholded = x0 and self._dynamic_thresholding
             r_prev, r_out = self._apg_buffers(raw, xe)
             xa = xe.float() if thresholded and xe.dtype != torch.float32 else xe
             a = _apg_args(be, raw, xa, marg, torch.float32 if thresholded else sd, x0, self._wrapped.noise_schedule,
@@ -1421,32 +1401,7 @@ class DPM_Solver:
                 return m_new, x_next
             else:
                 apg_a = a
-        cfz = None          # CFG-Zero*'s per-sample s* of a fused evaluation
-        if raw.cfgzero and raw.e_uncond is not None:
-            # the s* pass over both raw halves (+2 launches), then the fused step. With dynamic thresholding (the
-            # quantile takes one plain combine), and under UniPC (its launch takes one network output and converts at its
-            # own state), g is materialised once in fp32 (+1 launch) and handed on as one network output of the same
-            # parameterisation: the combine runs in raw space, so no x0 detour is needed.
-            cfz = be.cfgzero_scale(raw.e_cond, raw.e_uncond)
-            if (x0 and self._dynamic_thresholding) or self._apg_materialise:
-                a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
-                             guidance=raw.guidance, state_dtype=torch.float32, guidance_b=raw.guidance_b,
-                             per_sample=raw.e_cond.numel() // raw.e_cond.shape[0], cfgzero_s=cfz)
-                raw = RawOutput(be.step(a)[0], None, raw.param, 1.0)
-                cfz = None
-        tcw = None          # TCFG's per-sample words (wu, wc) of a fused evaluation
-        if raw.tcfg and raw.e_uncond is not None:
-            # the words pass over both raw halves (+2 launches), then the fused step; with dynamic thresholding, and
-            # under UniPC, g is materialised once in fp32 (+1 launch) and handed on as one network output, as for
-            # CFG-Zero*
-            tcw = be.tcfg_words(raw.e_cond, raw.e_uncond)
-            if (x0 and self._dynamic_thresholding) or self._apg_materialise:
-                a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
-                             guidance=raw.guidance, state_dtype=torch.float32, guidance_b=raw.guidance_b,
-                             per_sample=raw.e_cond.numel() // raw.e_cond.shape[0], tcfg_w=tcw)
-                raw = RawOutput(be.step(a)[0], None, raw.param, 1.0)
-                tcw = None
-        ratio = _cfg_ratio(be, raw)     # guidance rescale: one streaming pass over both halves (+2 launches)
+        words = _words(be, raw)     # guidance rescale, CFG-Zero*, TCFG: the per-sample words pass (+2 launches)
         if code:
             # reference-rounding mode (raw 16-bit NOISE outputs, fp32 state): bits 0-1 make the fused kernel take the
             # CFG combine in the network's type, three rounded ops (:329-330); for the eps-solver the buffered values
@@ -1454,15 +1409,20 @@ class DPM_Solver:
             rr = code
             if not x0:
                 rr = self._rr_run = code | 4
-        if raw.e_uncond is not None and x0 and self._dynamic_thresholding and (
-                code or ratio is not None or raw.guidance_b is not None or raw.e_conds is not None):
-            # the quantile kernels take the plain fp32 combine with one scale: give them (and the step) the reference's
-            # rounded noise, or the rescaled network output, materialised once in fp32 and then treated as one network
-            # output (the parameterisation, which the quantile and the step apply, still converts it) -- or, with
-            # per-sample scales and no rescale, the guided noise: each half parameterised, then combined with its
-            # sample's scale, as the reference orders it (+1 launch) -- or, with several conditions, their combined
-            # noise, each block parameterised first (+1 launch)
-            if ratio is None and (raw.guidance_b is not None or raw.e_conds is not None):
+        if raw.e_uncond is not None and (thresholded or (self._apg_materialise and raw.form in ("cfgzero", "tcfg"))):
+            # one fp32 output for the quantile kernels, which take the plain fp32 combine with one scale, and for UniPC,
+            # whose launch takes one network output and converts at its own state (+1 launch)
+            if words is not None or code:
+                # the reference's rounded noise, or the rescaled, CFG-Zero* or TCFG combine of the raw outputs, then
+                # treated as one network output (the parameterisation, which the quantile and the step apply, still
+                # converts it)
+                a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
+                             guidance=raw.guidance, state_dtype=torch.float32, raw_round=code)
+                raw = RawOutput(be.step(_guidance_args(a, words, raw))[0], None, raw.param, 1.0)
+                words, rr = None, 0
+            elif raw.guidance_b is not None or raw.e_conds is not None:
+                # per-sample scales: the guided noise, each half parameterised, then combined with its sample's scale,
+                # as the reference orders it; several conditions: their combined noise, each block parameterised first.
                 # (a flow or EDM network's outputs are converted to x0 directly and combined as x0: no eps -> x0
                 # follows)
                 flow = raw.param in (PARAM_FLOW, PARAM_EDM)
@@ -1480,13 +1440,6 @@ class DPM_Solver:
                     q_raw = RawOutput(e, None, PARAM_NOISE, 1.0, is_x0=flow)
                 else:
                     raw = RawOutput(e, None, PARAM_NOISE, 1.0, is_x0=flow)
-            else:
-                a = StepArgs(form=FORM_NONE, n_model=2, e_cond=raw.e_cond, e_uncond=raw.e_uncond, param=PARAM_NOISE,
-                             guidance=raw.guidance, state_dtype=torch.float32, raw_round=code)
-                e = be.step(_guidance_args(a, ratio, raw))[0]
-                raw = RawOutput(e, None, raw.param, 1.0)
-            rr = 0
-            ratio = None
         if (rr & 4) and co is not None:
             co = self._rr_coeffs(co, code)
         if not self._needs_conversion(raw, sd, x0):
@@ -1494,11 +1447,7 @@ class DPM_Solver:
             x_next = self._pure_update(co, x, m_new, m1, m2, rr=rr & 4 and rr, pkey=pkey if m_new is raw.e_cond else None) \
                 if co is not None else None
             return m_new, x_next
-        a = apg_a if apg_a is not None else _guidance_args(self._conv_args(raw, xe, alsig, sd, x0), ratio, raw)
-        if cfz is not None:
-            a.cfgzero_s, a.per_sample = cfz, raw.e_cond.numel() // raw.e_cond.shape[0]
-        if tcw is not None:
-            a.tcfg_w, a.per_sample = tcw, raw.e_cond.numel() // raw.e_cond.shape[0]
+        a = apg_a if apg_a is not None else _guidance_args(self._conv_args(raw, xe, alsig, sd, x0), words, raw)
         if alsig is _DEV:
             if co is None or co.dev is None:
                 raise RuntimeError("device-side scalars need the coefficient block of the consuming launch")
@@ -1561,16 +1510,11 @@ class DPM_Solver:
             self._xin_pair = (x_next, dup[0])
         return m_new, x_next
 
-    def _no_cfgpp(self, what: str) -> None:
-        if getattr(self._wrapped, "cfg_pp", False):
-            raise ValueError("cfg_pp is not available with {}: CFG++ runs inside sample() / inverse() with "
-                             "method='multistep' and order 1 or 2".format(what))
-
     def _apg_buffers(self, raw: RawOutput, xe):
         """(r_prev, r_out) of an APG evaluation. Without momentum, or outside a sample() / inverse() run: (None, None).
         The first evaluation of a run allocates the run's fp32 buffer and writes it without reading it (so a captured
         graph needs no reset launch); later ones update it in place."""
-        if raw.apg[2] == 0 or not self.__dict__.get("_apg_run"):
+        if raw.consts[2] == 0 or not self.__dict__.get("_apg_run"):
             return None, None
         r = self.__dict__.get("_apg_r")
         if r is None:
@@ -1583,7 +1527,8 @@ class DPM_Solver:
         """One sample() / inverse() run: the APG momentum buffer lives for its duration, and so do CFG-Zero*'s count of
         zero-init evaluations left and its zero outputs."""
         self._apg_run, self._apg_r = True, None
-        self._cfz_left, self._cfz_zero = getattr(self._wrapped, "cfg_zero_init_steps", 0), {}
+        self._cfz_left = self._wrapped.cfg_zero_init_steps if "zero_init" in self._options() else 0
+        self._cfz_zero = {}
         try:
             yield
         finally:
@@ -1598,10 +1543,6 @@ class DPM_Solver:
         if z is None:
             z = self._cfz_zero[key] = torch.zeros_like(x)
         return z
-
-    def _apg_momentum(self) -> float:
-        apg = getattr(self._wrapped, "apg", None)
-        return 0. if apg is None else apg[2]
 
     def _remember(self, pkey, a: StepArgs, dup=None) -> None:
         """Freeze the launch that just ran as the prepared form of its plan step."""
@@ -1725,8 +1666,7 @@ class DPM_Solver:
     # -- reference API: single updates (direct-call path; scalars computed per call) -------------
     def dpm_solver_first_update(self, x, s, t, model_s=None, return_intermediate=False):
         """DPM-Solver-1 / DDIM step s -> t (:547-592)."""
-        self._no_sde("dpm_solver_first_update()")
-        self._no_cfgpp("dpm_solver_first_update")
+        self._refuse("direct", what="dpm_solver_first_update()")
         x = self._state(x)
         co = P.first_update_coeffs(self.noise_schedule, self.algorithm_type, s, t)
         if model_s is None:
@@ -1744,8 +1684,7 @@ class DPM_Solver:
     def singlestep_dpm_solver_second_update(self, x, s, t, r1=0.5, model_s=None, return_intermediate=False,
                                             solver_type='dpmsolver'):
         """Singlestep DPM-Solver-2 s -> t (:594-673)."""
-        self._no_sde("singlestep_dpm_solver_second_update()")
-        self._no_cfgpp("singlestep_dpm_solver_second_update")
+        self._refuse("direct", what="singlestep_dpm_solver_second_update()")
         if solver_type not in ['dpmsolver', 'taylor']:
             raise ValueError("'solver_type' must be either 'dpmsolver' or 'taylor', got {}".format(solver_type))
         sp = P.singlestep_second(self.noise_schedule, self.algorithm_type, solver_type, s, t, r1)
@@ -1757,8 +1696,7 @@ class DPM_Solver:
     def singlestep_dpm_solver_third_update(self, x, s, t, r1=1. / 3., r2=2. / 3., model_s=None, model_s1=None,
                                            return_intermediate=False, solver_type='dpmsolver'):
         """Singlestep DPM-Solver-3 s -> t (:675-794)."""
-        self._no_sde("singlestep_dpm_solver_third_update()")
-        self._no_cfgpp("singlestep_dpm_solver_third_update")
+        self._refuse("direct", what="singlestep_dpm_solver_third_update()")
         if solver_type not in ['dpmsolver', 'taylor']:
             raise ValueError("'solver_type' must be either 'dpmsolver' or 'taylor', got {}".format(solver_type))
         sp = P.singlestep_third(self.noise_schedule, self.algorithm_type, solver_type, s, t, r1, r2)
@@ -1813,8 +1751,7 @@ class DPM_Solver:
 
     def multistep_dpm_solver_second_update(self, x, model_prev_list, t_prev_list, t, solver_type="dpmsolver"):
         """Multistep DPM-Solver-2 (:796-852)."""
-        self._no_sde("multistep_dpm_solver_second_update()")
-        self._no_cfgpp("multistep_dpm_solver_second_update")
+        self._refuse("direct", what="multistep_dpm_solver_second_update()")
         if solver_type not in ['dpmsolver', 'taylor']:
             raise ValueError("'solver_type' must be either 'dpmsolver' or 'taylor', got {}".format(solver_type))
         co = P.multistep_coeffs(self.noise_schedule, self.algorithm_type, solver_type, 2, t_prev_list, t)
@@ -1822,8 +1759,7 @@ class DPM_Solver:
 
     def multistep_dpm_solver_third_update(self, x, model_prev_list, t_prev_list, t, solver_type='dpmsolver'):
         """Multistep DPM-Solver-3 (:854-904); needs exactly three buffered values."""
-        self._no_sde("multistep_dpm_solver_third_update()")
-        self._no_cfgpp("multistep_dpm_solver_third_update")
+        self._refuse("direct", what="multistep_dpm_solver_third_update()")
         model_prev_2, model_prev_1, model_prev_0 = model_prev_list
         t_prev_2, t_prev_1, t_prev_0 = t_prev_list
         co = P.multistep_coeffs(self.noise_schedule, self.algorithm_type, solver_type, 3,
@@ -1833,8 +1769,7 @@ class DPM_Solver:
     def singlestep_dpm_solver_update(self, x, s, t, order, return_intermediate=False, solver_type='dpmsolver',
                                      r1=None, r2=None):
         """Order dispatch (:906-930)."""
-        self._no_sde("singlestep_dpm_solver_update()")
-        self._no_cfgpp("singlestep_dpm_solver_update")
+        self._refuse("direct", what="singlestep_dpm_solver_update()")
         if order == 1:
             return self.dpm_solver_first_update(x, s, t, return_intermediate=return_intermediate)
         elif order == 2:
@@ -1848,8 +1783,7 @@ class DPM_Solver:
 
     def multistep_dpm_solver_update(self, x, model_prev_list, t_prev_list, t, order, solver_type='dpmsolver'):
         """Order dispatch (:932-954)."""
-        self._no_sde("multistep_dpm_solver_update()")
-        self._no_cfgpp("multistep_dpm_solver_update")
+        self._refuse("direct", what="multistep_dpm_solver_update()")
         if order == 1:
             return self.dpm_solver_first_update(x, t_prev_list[-1], t, model_s=model_prev_list[-1])
         elif order == 2:
@@ -1864,8 +1798,7 @@ class DPM_Solver:
                             t_err=1e-5, solver_type='dpmsolver'):
         """Adaptive step size DPM-Solver-12 / -23 (:956-1010). Updates and the error estimate run on
         the fused kernels; the step-size controller is the reference's host logic."""
-        self._no_sde("the adaptive method")
-        self._no_cfgpp("method='adaptive'")
+        self._refuse("direct", what="dpm_solver_adaptive()")
         ns = self.noise_schedule
         x = self._state(x)
         device = x.device
@@ -2025,7 +1958,7 @@ class DPM_Solver:
                 method='multistep', lower_order_final=True, denoise_to_zero=False, solver_type='dpmsolver',
                 atol=0.0078, rtol=0.05, return_intermediate=False):
         """Invert `x` from t_start (default 1/N) to t_end (default T) (:1032-1045)."""
-        self._no_sde("inverse()")
+        self._refuse("inverse")
         t_0 = 1. / self.noise_schedule.total_N if t_start is None else t_start
         t_T = self.noise_schedule.T if t_end is None else t_end
         assert t_0 > 0 and t_T > 0, "Time range needs to be greater than 0. For discrete-time DPMs, it needs to be in [1 / N, 1], where N is the length of betas array"
@@ -2034,7 +1967,7 @@ class DPM_Solver:
                            solver_type=solver_type, atol=atol, rtol=rtol, return_intermediate=return_intermediate)
 
     # -- whole-loop CUDA graph (SURVEY 8f-1; no counterpart in the reference) -----------------------
-    def _sde_args(self, x, method, eta, generator) -> float:
+    def _sde_args(self, x, eta, generator) -> float:
         """Validate sample()'s eta and generator: the run's eta for the SDE solver (0: the ODE run, nothing drawn), else
         0. ValueError before any launch or network call."""
         if self.algorithm_type != "sde-dpmsolver++":
@@ -2042,8 +1975,6 @@ class DPM_Solver:
                 raise ValueError("eta and generator are arguments of algorithm_type='sde-dpmsolver++', not {!r}".format(
                     self.algorithm_type))
             return 0.0
-        if method != "multistep":
-            self._no_sde("method={!r}".format(method))
         eta = 1.0 if eta is None else eta
         if isinstance(eta, bool) or not isinstance(eta, (int, float)) or not math.isfinite(eta) or eta < 0:
             raise ValueError("eta must be a finite number >= 0, got {!r}".format(eta))
@@ -2121,9 +2052,12 @@ class DPM_Solver:
         and the guidance forms uncond, classifier, classifier-free (scalar or per-sample scale, guidance_rescale,
         cfg_zero_star, tcfg, fdg_scales) are accepted; singlestep / adaptive methods, inverse(), the direct update
         methods, several conditions, guidance_mask, perp_neg, apg_eta, cfg_pp and reference_rounding are not."""
-        sde_eta = self._sde_args(x, method, eta, generator)
-        if getattr(self._wrapped, "cfg_pp", False) and (method != "multistep" or order not in (1, 2)):
-            self._no_cfgpp("method='{}' and order {}".format(method, order))
+        options = self._options()
+        if method != "multistep":
+            _check_options(options, ("adaptive" if method == "adaptive" else "singlestep",), "method={!r}".format(method))
+        elif order not in (1, 2):
+            _check_options(options, ("order",), "order {}".format(order))
+        sde_eta = self._sde_args(x, eta, generator)
         t_0 = 1. / self.noise_schedule.total_N if t_end is None else t_end
         t_T = self.noise_schedule.T if t_start is None else t_start
         assert t_0 > 0 and t_T > 0, "Time range needs to be greater than 0. For discrete-time DPMs, it needs to be in [1 / N, 1], where N is the length of betas array"
@@ -2131,12 +2065,6 @@ class DPM_Solver:
             assert method in ['multistep', 'singlestep', 'singlestep_fixed'], "Cannot use adaptive solver when saving intermediate values"
         if self.correcting_xt_fn is not None:
             assert method in ['multistep', 'singlestep', 'singlestep_fixed'], "Cannot use adaptive solver when correcting_xt_fn is not None"
-        if method == 'adaptive' and getattr(self._wrapped, "cfg_zero_init_steps", 0) > 0:
-            raise ValueError("cfg_zero_init_steps > 0 is not available with method='adaptive': its rejected steps leave "
-                             "'the first K evaluations' undefined")
-        if method == 'adaptive' and self._apg_momentum() != 0:
-            raise ValueError("apg_momentum != 0 is not available with method='adaptive': its evaluations, the device "
-                             "controller's surplus iterations included, define no momentum sequence")
         self._check_fdg(x)
         device = x.device
         intermediates = []
@@ -2160,7 +2088,7 @@ class DPM_Solver:
                 if order not in (1, 2, 3):
                     raise ValueError("Solver order must be 1 or 2 or 3, got {}".format(order))
                 key = ("multistep", steps, order, skip_type, t_T, t_0, solver_type, lower_order_final)
-                cfgpp = getattr(self._wrapped, "cfg_pp", False)
+                cfgpp = "cfgpp" in options
                 if cfgpp:
                     key = key + ("cfg_pp",)     # (the plan carries g)
                 if self.algorithm_type == "sde-dpmsolver++":

@@ -80,7 +80,7 @@ from typing import Optional
 import torch
 
 from . import plan as P
-from .solver import DPM_Solver, WrappedModel
+from .solver import DPM_Solver
 
 __all__ = ["UniPC"]
 
@@ -127,18 +127,7 @@ class UniPC(DPM_Solver):
             raise ValueError("reference_rounding=True is not available with UniPC")
         if self.plan_broadcast:
             raise ValueError("plan_broadcast=True is not available with UniPC")
-        w = self._wrapped
-        if isinstance(w, WrappedModel):
-            if w.per_sample_guidance:
-                raise ValueError("a per-sample guidance_scale is not available with UniPC")
-            if w.n_cond >= 2:
-                raise ValueError("several conditions are not available with UniPC")
-            if w.cond_masks is not None:
-                raise ValueError("guidance_mask is not available with UniPC")
-            if w.guidance_type == "classifier-free" and w.guidance_rescale != 0:
-                raise ValueError("guidance_rescale is not available with UniPC")
-            if w.cfg_pp:
-                raise ValueError("cfg_pp is not available with UniPC (CFG++ is a DPM-Solver++ multistep update)")
+        self._refuse("unipc")
 
     def inverse(self, x, steps=20, t_start=None, t_end=None, order=2, skip_type='time_uniform', lower_order_final=True,
                 denoise_to_zero=False, use_corrector=True, return_intermediate=False):
