@@ -25,7 +25,7 @@ OUT_DIR = PKG / "lib"
 BUILD_DIR = PKG / "build"
 LIB_NAME = "libdpmsolver_b200.so"
 
-SOURCES = ["capi.cu", "step_direct.cu", "step_multi.cu", "step_unipc.cu", "step_tma.cu","quantile.cu", "adaptive.cu", "adaptive_ctl.cu", "philox.cu", "apg.cu", "step_cfgpp.cu", "fdg.cu", "step_sde.cu"]
+SOURCES = ["capi.cu", "step_direct.cu", "step_multi.cu", "step_unipc.cu", "step_tma.cu","quantile.cu", "adaptive.cu", "adaptive_ctl.cu", "philox.cu", "words.cu", "step_cfgpp.cu", "fdg.cu", "step_sde.cu"]
 # philox.cu embeds curand's Box-Muller, which must round exactly like the copy inside torch's randn kernel: it is
 # compiled with nvcc's default fma contraction and spells the reference's unfused chain with __fmul_rn/__fadd_rn
 FMAD_DEFAULT = {"philox.cu"}

@@ -582,32 +582,43 @@ int dpm_step_guided(const dpm_step_desc* desc, const float* guidance, const floa
   return step_impl(desc, static_cast<cudaStream_t>(stream), &rs, guidance);
 }
 
+// The argument checks of the pair passes (the rescale ratio, CFG-Zero*, TCFG), after their `n == 0: nothing to do`:
+// a NULL tensor (`tensors` false), then the dtype and per_sample dividing n.
+static int pair_check(const char* what, bool tensors, int model_dtype, uint64_t per_sample, uint64_t n) {
+  if (!tensors) { set_error("%s: NULL tensor", what); return DPM_ERR_ARG; }
+  if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) {
+    set_error("%s: bad dtype or sizes", what);
+    return DPM_ERR_ARG;
+  }
+  return DPM_OK;
+}
+
 size_t dpm_cfg_rescale_workspace(uint64_t n_samples, uint64_t per_sample) {
-  return cfg_rescale_workspace_bytes(n_samples, per_sample);
+  return words_workspace_bytes(n_samples, per_sample, 4);
 }
 
 int dpm_cfg_rescale_ratio(float* ratio_out, const void* e_cond, const void* e_uncond, float guidance,
                           uint64_t per_sample, uint64_t n, int model_dtype, void* workspace, size_t workspace_bytes,
                           dpm_stream_t stream) {
   if (n == 0) return DPM_OK;
-  if (!ratio_out || !e_cond || !e_uncond) { set_error("cfg rescale: NULL tensor"); return DPM_ERR_ARG; }
-  if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) { set_error("cfg rescale: bad dtype or sizes"); return DPM_ERR_ARG; }
-  return finish(launch_cfg_rescale_ratio(ratio_out, e_cond, e_uncond, guidance, per_sample, n, model_dtype, workspace,
-                                         workspace_bytes, static_cast<cudaStream_t>(stream)));
+  const int rc = pair_check("cfg rescale", ratio_out && e_cond && e_uncond, model_dtype, per_sample, n);
+  return rc != DPM_OK ? rc : finish(launch_cfg_rescale_ratio(ratio_out, e_cond, e_uncond, guidance, per_sample, n,
+                                                             model_dtype, workspace, workspace_bytes,
+                                                             static_cast<cudaStream_t>(stream)));
 }
 
 int dpm_cfg_rescale_ratio_guided(float* ratio_out, const void* e_cond, const void* e_uncond, const float* guidance,
                                  uint64_t per_sample, uint64_t n, int model_dtype, void* workspace,
                                  size_t workspace_bytes, dpm_stream_t stream) {
   if (n == 0) return DPM_OK;
-  if (!ratio_out || !e_cond || !e_uncond || !guidance) { set_error("cfg rescale: NULL tensor"); return DPM_ERR_ARG; }
-  if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) { set_error("cfg rescale: bad dtype or sizes"); return DPM_ERR_ARG; }
-  return finish(launch_cfg_rescale_ratio(ratio_out, e_cond, e_uncond, 0.f, per_sample, n, model_dtype, workspace,
-                                         workspace_bytes, static_cast<cudaStream_t>(stream), guidance));
+  const int rc = pair_check("cfg rescale", ratio_out && e_cond && e_uncond && guidance, model_dtype, per_sample, n);
+  return rc != DPM_OK ? rc : finish(launch_cfg_rescale_ratio(ratio_out, e_cond, e_uncond, 0.f, per_sample, n,
+                                                             model_dtype, workspace, workspace_bytes,
+                                                             static_cast<cudaStream_t>(stream), guidance));
 }
 
 size_t dpm_apg_workspace(uint64_t n_samples, uint64_t per_sample) {
-  return apg_workspace_bytes(n_samples, per_sample);
+  return words_workspace_bytes(n_samples, per_sample, 3);
 }
 
 // the checks both APG entries share: a CFG pair of whole samples, no reference rounding, no EDM words from dev_coef
@@ -652,19 +663,15 @@ int dpm_step_apg(const dpm_step_desc* desc, const float* words, const float* gui
 }
 
 size_t dpm_cfgzero_workspace(uint64_t n_samples, uint64_t per_sample) {
-  return cfgzero_workspace_bytes(n_samples, per_sample);
+  return words_workspace_bytes(n_samples, per_sample, 2);
 }
 
 int dpm_cfgzero_scale(float* s_out, const void* e_cond, const void* e_uncond, int model_dtype, uint64_t per_sample,
                       uint64_t n, void* workspace, size_t workspace_bytes, dpm_stream_t stream) {
   if (n == 0) return DPM_OK;
-  if (!s_out || !e_cond || !e_uncond) { set_error("cfg-zero* scale: NULL tensor"); return DPM_ERR_ARG; }
-  if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) {
-    set_error("cfg-zero* scale: bad dtype or sizes");
-    return DPM_ERR_ARG;
-  }
-  return finish(launch_cfgzero_scale(s_out, e_cond, e_uncond, model_dtype, per_sample, n, workspace, workspace_bytes,
-                                     static_cast<cudaStream_t>(stream)));
+  const int rc = pair_check("cfg-zero* scale", s_out && e_cond && e_uncond, model_dtype, per_sample, n);
+  return rc != DPM_OK ? rc : finish(launch_cfgzero_scale(s_out, e_cond, e_uncond, model_dtype, per_sample, n, workspace,
+                                                         workspace_bytes, static_cast<cudaStream_t>(stream)));
 }
 
 int dpm_step_cfgzero(const dpm_step_desc* desc, const float* s_star, const float* guidance, dpm_stream_t stream) {
@@ -678,19 +685,15 @@ int dpm_step_cfgzero(const dpm_step_desc* desc, const float* s_star, const float
 }
 
 size_t dpm_tcfg_workspace(uint64_t n_samples, uint64_t per_sample) {
-  return tcfg_workspace_bytes(n_samples, per_sample);
+  return words_workspace_bytes(n_samples, per_sample, 3);
 }
 
 int dpm_tcfg_words(float* w_out, const void* e_cond, const void* e_uncond, int model_dtype, uint64_t per_sample,
                    uint64_t n, void* workspace, size_t workspace_bytes, dpm_stream_t stream) {
   if (n == 0) return DPM_OK;
-  if (!w_out || !e_cond || !e_uncond) { set_error("tcfg words: NULL tensor"); return DPM_ERR_ARG; }
-  if (!valid_dtype(model_dtype) || per_sample == 0 || n % per_sample) {
-    set_error("tcfg words: bad dtype or sizes");
-    return DPM_ERR_ARG;
-  }
-  return finish(launch_tcfg_words(w_out, e_cond, e_uncond, model_dtype, per_sample, n, workspace, workspace_bytes,
-                                  static_cast<cudaStream_t>(stream)));
+  const int rc = pair_check("tcfg words", w_out && e_cond && e_uncond, model_dtype, per_sample, n);
+  return rc != DPM_OK ? rc : finish(launch_tcfg_words(w_out, e_cond, e_uncond, model_dtype, per_sample, n, workspace,
+                                                      workspace_bytes, static_cast<cudaStream_t>(stream)));
 }
 
 int dpm_step_tcfg(const dpm_step_desc* desc, const float* words, const float* guidance, dpm_stream_t stream) {
@@ -704,7 +707,7 @@ int dpm_step_tcfg(const dpm_step_desc* desc, const float* words, const float* gu
 }
 
 size_t dpm_perpneg_workspace(uint64_t n_samples, uint64_t per_sample) {
-  return perpneg_workspace_bytes(n_samples, per_sample);
+  return words_workspace_bytes(n_samples, per_sample, DPM_MAX_CONDITIONS);   // whatever n_cond is
 }
 
 int dpm_perpneg_words(float* w_out, const void* e_uncond, const void* const* e_conds, const float* scales, int n_cond,

@@ -134,20 +134,17 @@ size_t quantile_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
 size_t adaptive_workspace_bytes(uint64_t n, uint64_t per_sample);
 int launch_adaptive_error(float* out, const void* xh, const void* xl, const void* xp, float atol, float rtol,
                           uint64_t per_sample, uint64_t n, int dtype, void* ws, size_t ws_bytes, cudaStream_t stream);
-size_t cfg_rescale_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
+// the per-sample guidance words passes (words.cu): the workspace of `sums` fp64 partials per chunk of a sample
+size_t words_workspace_bytes(uint64_t n_samples, uint64_t per_sample, int sums);
 int launch_cfg_rescale_ratio(float* ratio, const void* ec, const void* eu, float guidance, uint64_t per_sample,
                              uint64_t n, int dtype, void* ws, size_t ws_bytes, cudaStream_t stream,
                              const float* gscale = nullptr);
-size_t apg_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
 int launch_apg_words(float* words, const KParams& kp, const float* gscale, float eta, float norm_threshold,
                      float momentum, const float* r_prev, float* r_out, void* ws, size_t ws_bytes, cudaStream_t stream);
-size_t cfgzero_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
 int launch_cfgzero_scale(float* s_out, const void* ec, const void* eu, int model_dtype, uint64_t per_sample,
                          uint64_t n, void* ws, size_t ws_bytes, cudaStream_t stream);
-size_t tcfg_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
 int launch_tcfg_words(float* w_out, const void* ec, const void* eu, int model_dtype, uint64_t per_sample, uint64_t n,
                       void* ws, size_t ws_bytes, cudaStream_t stream);
-size_t perpneg_workspace_bytes(uint64_t n_samples, uint64_t per_sample);
 int launch_perpneg_words(float* w_out, const void* eu, const void* const* ec, const float* scales, int n_cond,
                          int model_dtype, uint64_t per_sample, uint64_t n, void* ws, size_t ws_bytes,
                          cudaStream_t stream);

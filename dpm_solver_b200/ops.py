@@ -377,8 +377,7 @@ class CudaBackend:
                 raise ValueError("dpm_solver_b200: r_out must be dense and laid out like the inputs")
             ro = r_out
         words = torch.empty(2, nb, dtype=torch.float32, device=ref.device)
-        ws_bytes = int(self._lib.dpm_apg_workspace(nb, a.per_sample))
-        ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=ref.device)
+        ws, ws_bytes = self._workspace(self._lib.dpm_apg_workspace, nb, a.per_sample, ref.device)
         self._launch(ref.device, self._lib.dpm_apg_words, C.c_void_p(words.data_ptr()), C.byref(d),
                      C.c_void_p(None if a.guidance_b is None else a.guidance_b.data_ptr()), C.c_float(eta),
                      C.c_float(norm_threshold), C.c_float(momentum), C.c_void_p(None if rp is None else rp.data_ptr()),
@@ -389,42 +388,16 @@ class CudaBackend:
         """CFG-Zero*'s per-sample s*_b = <c_b, u_b> / (||u_b||^2 + 1e-8) of the two raw halves, as fp32 [B] on the
         device (dpm_cfgzero_scale): fp64 sums in storage order, merged per chunk in order. Both halves keep a shared
         dense layout (a sample is one contiguous block in row-major and channels_last storage alike)."""
-        n, dev = e_cond.numel(), e_cond.device
-        layout = self._layout(e_cond)
-        if layout is None or self._layout(e_uncond) != layout:
-            layout = "c"
-        ec = self._check(e_cond, "e_cond", dev, n, layout=layout)
-        eu = self._check(e_uncond, "e_uncond", dev, n, e_cond.dtype, layout)
-        nb = e_cond.shape[0]
-        per_sample = n // nb
-        s = torch.empty(nb, dtype=torch.float32, device=dev)
-        ws_bytes = int(self._lib.dpm_cfgzero_workspace(nb, per_sample))
-        ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev)
-        self._launch(dev, self._lib.dpm_cfgzero_scale, C.c_void_p(s.data_ptr()), C.c_void_p(ec.data_ptr()),
-                     C.c_void_p(eu.data_ptr()), C.c_int(_DTYPE_CODE[e_cond.dtype]), C.c_uint64(per_sample),
-                     C.c_uint64(n), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
-        return s
+        return self._words(self._lib.dpm_cfgzero_scale, self._lib.dpm_cfgzero_workspace, (),
+                           [("e_cond", e_cond), ("e_uncond", e_uncond)], lambda p, ps, n, dt: (*p, dt, ps, n))
 
     def tcfg_words(self, e_cond: torch.Tensor, e_uncond: torch.Tensor) -> torch.Tensor:
         """TCFG's per-sample words (wu_b, wc_b), u' = wu_b*u + wc_b*c the projection of the unconditional output on the
         first right singular vector of [u_b; c_b], as fp32 [B, 2] on the device (dpm_tcfg_words): fp64 sums ||u||^2,
         <u, c>, ||c||^2 in storage order, merged per chunk in order, then the closed form of the header. Both halves
         keep a shared dense layout (a sample is one contiguous block in row-major and channels_last storage alike)."""
-        n, dev = e_cond.numel(), e_cond.device
-        layout = self._layout(e_cond)
-        if layout is None or self._layout(e_uncond) != layout:
-            layout = "c"
-        ec = self._check(e_cond, "e_cond", dev, n, layout=layout)
-        eu = self._check(e_uncond, "e_uncond", dev, n, e_cond.dtype, layout)
-        nb = e_cond.shape[0]
-        per_sample = n // nb
-        w = torch.empty(nb, 2, dtype=torch.float32, device=dev)
-        ws_bytes = int(self._lib.dpm_tcfg_workspace(nb, per_sample))
-        ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev)
-        self._launch(dev, self._lib.dpm_tcfg_words, C.c_void_p(w.data_ptr()), C.c_void_p(ec.data_ptr()),
-                     C.c_void_p(eu.data_ptr()), C.c_int(_DTYPE_CODE[e_cond.dtype]), C.c_uint64(per_sample),
-                     C.c_uint64(n), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
-        return w
+        return self._words(self._lib.dpm_tcfg_words, self._lib.dpm_tcfg_workspace, (2,),
+                           [("e_cond", e_cond), ("e_uncond", e_uncond)], lambda p, ps, n, dt: (*p, dt, ps, n))
 
     def perpneg_words(self, e_uncond: torch.Tensor, e_conds, scales) -> torch.Tensor:
         """Perp-Neg's per-sample weight of the first condition, w_1 = fl32(s_1 - sum_{k>=2} s_k*<d_k, d_1>/||d_1||^2)
@@ -436,22 +409,37 @@ class CudaBackend:
         if not 2 <= K <= _lib.MAX_CONDITIONS or len(scales) != K:
             raise ValueError("dpm_solver_b200: Perp-Neg words take 2..{} conditional outputs and one scale each".format(
                 _lib.MAX_CONDITIONS))
-        n, dev = e_uncond.numel(), e_uncond.device
-        layout = self._layout(e_uncond)
-        if layout is None or any(self._layout(e) != layout for e in e_conds):
+        blocks = [("e_uncond", e_uncond)] + [("e_conds[%d]" % k, e) for k, e in enumerate(e_conds)]
+        return self._words(self._lib.dpm_perpneg_words, self._lib.dpm_perpneg_workspace, (), blocks,
+                           lambda p, ps, n, dt: (p[0], (C.c_void_p * K)(*p[1:]), (C.c_float * K)(*scales), C.c_int(K),
+                                                 dt, ps, n))
+
+    def _words(self, fn, workspace, shape, blocks, args):
+        """Launch the words pass fn(out, *args(pointers, per_sample, n, dtype), ws, ws_bytes) over the [B, ...] network
+        output blocks, given as (name, tensor), and return its fp32 words [B, *shape]. The blocks keep a shared dense
+        layout (a sample is one contiguous block in row-major and channels_last storage alike), else all go row-major;
+        all take the first block's device and dtype. `args` gets the ctypes values of the blocks' data pointers,
+        per_sample, n and the dtype code."""
+        ref = blocks[0][1]
+        n, dev = ref.numel(), ref.device
+        layout = self._layout(ref)
+        if layout is None or any(self._layout(t) != layout for _, t in blocks):
             layout = "c"
-        eu = self._check(e_uncond, "e_uncond", dev, n, layout=layout)
-        ecs = [self._check(e, "e_conds[%d]" % k, dev, n, e_uncond.dtype, layout) for k, e in enumerate(e_conds)]
-        nb = e_uncond.shape[0]
+        ts = [self._check(t, what, dev, n, None if k == 0 else ref.dtype, layout) for k, (what, t) in enumerate(blocks)]
+        nb = ref.shape[0]
         per_sample = n // nb
-        w = torch.empty(nb, dtype=torch.float32, device=dev)
-        ws_bytes = int(self._lib.dpm_perpneg_workspace(nb, per_sample))
-        ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev)
-        ecp, sc = (C.c_void_p * K)(*[e.data_ptr() for e in ecs]), (C.c_float * K)(*scales)
-        self._launch(dev, self._lib.dpm_perpneg_words, C.c_void_p(w.data_ptr()), C.c_void_p(eu.data_ptr()), ecp, sc,
-                     C.c_int(K), C.c_int(_DTYPE_CODE[e_uncond.dtype]), C.c_uint64(per_sample), C.c_uint64(n),
-                     C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
-        return w
+        out = torch.empty(nb, *shape, dtype=torch.float32, device=dev)
+        ws, ws_bytes = self._workspace(workspace, nb, per_sample, dev)
+        middle = args([C.c_void_p(t.data_ptr()) for t in ts], C.c_uint64(per_sample), C.c_uint64(n),
+                      C.c_int(_DTYPE_CODE[ref.dtype]))
+        self._launch(dev, fn, C.c_void_p(out.data_ptr()), *middle, C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
+        return out
+
+    @staticmethod
+    def _workspace(workspace, n_samples, per_sample, dev):
+        """The device workspace of a words pass (at least 8 bytes, so that it has an address) and its size."""
+        ws_bytes = int(workspace(n_samples, per_sample))
+        return torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev), ws_bytes
 
     def fdg_guided(self, e_cond: torch.Tensor, e_uncond: torch.Tensor, scales, levels: int) -> torch.Tensor:
         """Frequency-decoupled guidance (dpm_fdg_guided, one launch): g over the planes of the last two dims, in the
@@ -612,31 +600,20 @@ class CudaBackend:
         device (dpm_cfg_rescale_ratio). Both halves keep a shared dense layout: a sample is one contiguous block
         in row-major and in channels_last storage alike. `guidance` may be a contiguous fp32 device tensor of B
         per-sample scales (dpm_cfg_rescale_ratio_guided)."""
-        n, dev = e_cond.numel(), e_cond.device
-        layout = self._layout(e_cond)
-        if layout is None or self._layout(e_uncond) != layout:
-            layout = "c"
-        ec = self._check(e_cond, "e_cond", dev, n, layout=layout)
-        eu = self._check(e_uncond, "e_uncond", dev, n, e_cond.dtype, layout)
-        nb = e_cond.shape[0]
-        per_sample = n // nb
-        r = torch.empty(nb, dtype=torch.float32, device=dev)
-        ws_bytes = int(self._lib.dpm_cfg_rescale_workspace(nb, per_sample))
-        ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev)
-        if torch.is_tensor(guidance):
+        blocks = [("e_cond", e_cond), ("e_uncond", e_uncond)]
+        if not torch.is_tensor(guidance):
+            return self._words(self._lib.dpm_cfg_rescale_ratio, self._lib.dpm_cfg_rescale_workspace, (), blocks,
+                               lambda p, ps, n, dt: (*p, C.c_float(guidance), ps, n, dt))
+
+        def guided_args(p, ps, n, dt):
+            # (checked once _words has checked the halves, so that a bad half is reported first)
             if not guidance.is_cuda or guidance.dtype != torch.float32 or not guidance.is_contiguous() \
-                    or guidance.device != dev or guidance.numel() != nb:
+                    or guidance.device != e_cond.device or guidance.numel() != e_cond.shape[0]:
                 raise ValueError("dpm_solver_b200: per-sample guidance must be a contiguous fp32 [B] tensor on the "
                                  "tensors' device")
-            self._launch(dev, self._lib.dpm_cfg_rescale_ratio_guided, C.c_void_p(r.data_ptr()),
-                         C.c_void_p(ec.data_ptr()), C.c_void_p(eu.data_ptr()), C.c_void_p(guidance.data_ptr()),
-                         C.c_uint64(per_sample), C.c_uint64(n), C.c_int(_DTYPE_CODE[e_cond.dtype]),
-                         C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
-            return r
-        self._launch(dev, self._lib.dpm_cfg_rescale_ratio, C.c_void_p(r.data_ptr()), C.c_void_p(ec.data_ptr()),
-                     C.c_void_p(eu.data_ptr()), C.c_float(guidance), C.c_uint64(per_sample), C.c_uint64(n),
-                     C.c_int(_DTYPE_CODE[e_cond.dtype]), C.c_void_p(ws.data_ptr()), C.c_size_t(ws_bytes))
-        return r
+            return (*p, C.c_void_p(guidance.data_ptr()), ps, n, dt)
+        return self._words(self._lib.dpm_cfg_rescale_ratio_guided, self._lib.dpm_cfg_rescale_workspace, (), blocks,
+                           guided_args)
 
     def _launch(self, device, fn, *args):
         """Call a C-ABI entry on torch's current stream of `device` (device guard only if needed)."""

@@ -7,8 +7,8 @@
 * `x0_fp64`: each parameterisation's denoised prediction in float64.
 * `APGOracle`: the numpy executor (edm_oracle.EDMOracle: every parameterisation, guidance form and dpm_step_unipc) plus
   dpm_apg_words and dpm_step_apg as include/dpm_solver_b200.h states them, op for op in IEEE fp32, the sums in fp64
-  (numpy's pairwise order; `exact=True`: apg.cu's order, `apg_words_exact`, so that the words are bit-exact).
-* `apg_words_exact`: the words of apg.cu operation for operation -- its chunks, thread ownership, warp butterflies,
+  (numpy's pairwise order; `exact=True`: words.cu's order, `apg_words_exact`, so that the words are bit-exact).
+* `apg_words_exact`: the words of words.cu operation for operation -- its chunks, thread ownership, warp butterflies,
   warp order, chunk merge and k_apg_final's left-to-right fp64 formula.
 * `reference_solver`: the UNMODIFIED reference DPM_Solver driven by an fp64 APG data-prediction function, with the
   momentum kept in its closure.
@@ -71,43 +71,53 @@ def x0_fp64(param, out, x, alpha, sigma, sigma_data=None):
     raise ValueError(param)
 
 
-# ---- apg.cu's reduction, operation for operation -----------------------------------------------------------------------
+# ---- words.cu's reduction, operation for operation -------------------------------------------------------------------
 
 CHUNK, THREADS, WARP = 8192, 256, 32
 
 
-def apg_sums_exact(R, c):
-    """(||R||^2, <R, c>, ||c||^2) per sample as k_apg_partial + k_apg_final sum them, from fp32 [B, per_sample] arrays.
-    CTA (b, chunk) covers chunk elements [chunk*8192, min(+8192, per_sample)); thread tid owns the elements
-    (u*256 + tid)*8 + i, u = 0..3, i = 0..7, and adds their fp64 products in that order to sums that start at 0.0 (the
-    product of two fp32 values is exact in fp64). Each warp folds its 32 lanes by v += shfl_xor(v, o), o = 16 .. 1; then
-    s = 0.0 + warp 0 + ... + warp 7, and the chunks are merged from 0.0 in chunk order. Elements past the end of the
-    sample contribute the product +0.0, which leaves every such sum (never -0.0: it starts at +0.0) unchanged."""
-    R, c = np.asarray(R, f32), np.asarray(c, f32)
-    Bn, ps = R.shape
+def chunk_sums(v):
+    """The CTA sums [B, chunks] of fp64 terms v [B, per_sample] as the words passes form them: CTA (b, chunk) covers
+    chunk elements [chunk*8192, min(+8192, per_sample)); thread tid owns the elements (u*256 + tid)*8 + i, u = 0..3,
+    i = 0..7, and adds their terms in that order to a sum that starts at 0.0. Each warp folds its 32 lanes by
+    v += shfl_xor(v, o), o = 16 .. 1; then s = 0.0 + warp 0 + ... + warp 7. Elements past the end of the sample are
+    skipped; here they add +0.0, which leaves every such sum (never -0.0: it starts at +0.0) unchanged."""
+    Bn, ps = v.shape
     chunks = -(-ps // CHUNK)
     pad = chunks * CHUNK - ps
-    out = []
     with np.errstate(all="ignore"):
-        for a, b in ((R, R), (R, c), (c, c)):
-            prod = a.astype(np.float64) * b.astype(np.float64)
-            prod = np.concatenate([prod, np.zeros((Bn, pad))], axis=1) if pad else prod
-            # [B, chunk, u, tid, i] -> [B, chunk, tid, (u, i)]: each thread's 32 products in the order it adds them
-            per_thread = prod.reshape(Bn, chunks, 4, THREADS, 8).transpose(0, 1, 3, 2, 4).reshape(Bn, chunks, THREADS, 32)
-            v = np.zeros((Bn, chunks, THREADS))
-            for k in range(32):
-                v = v + per_thread[..., k]
-            lanes = v.reshape(Bn, chunks, THREADS // WARP, WARP)
-            for o in (16, 8, 4, 2, 1):
-                lanes = lanes + lanes[..., np.arange(WARP) ^ o]
-            s = np.zeros((Bn, chunks))
-            for w in range(THREADS // WARP):
-                s = s + lanes[:, :, w, 0]
-            t = np.zeros(Bn)
-            for ch in range(chunks):
-                t = t + s[:, ch]
-            out.append(t)
-    return tuple(out)
+        v = np.concatenate([v, np.zeros((Bn, pad))], axis=1) if pad else v
+        # [B, chunk, u, tid, i] -> [B, chunk, tid, (u, i)]: each thread's 32 terms in the order it adds them
+        per_thread = v.reshape(Bn, chunks, 4, THREADS, 8).transpose(0, 1, 3, 2, 4).reshape(Bn, chunks, THREADS, 32)
+        t = np.zeros((Bn, chunks, THREADS))
+        for k in range(32):
+            t = t + per_thread[..., k]
+        lanes = t.reshape(Bn, chunks, THREADS // WARP, WARP)
+        for o in (16, 8, 4, 2, 1):
+            lanes = lanes + lanes[..., np.arange(WARP) ^ o]
+        s = np.zeros((Bn, chunks))
+        for w in range(THREADS // WARP):
+            s = s + lanes[:, :, w, 0]
+    return s
+
+
+def device_sum(v):
+    """The per-sample fp64 sum [B] of the terms v [B, per_sample] in the words passes' order: chunk_sums, merged from
+    0.0 in chunk order."""
+    s = chunk_sums(v)
+    t = np.zeros(s.shape[0])
+    with np.errstate(all="ignore"):
+        for ch in range(s.shape[1]):
+            t = t + s[:, ch]
+    return t
+
+
+def apg_sums_exact(R, c):
+    """(||R||^2, <R, c>, ||c||^2) per sample as the APG words pass (ApgPass) + k_apg_final sum them, from fp32
+    [B, per_sample] arrays: the device_sum of the fp64 products (the product of two fp32 values is exact in fp64)."""
+    R, c = np.asarray(R, f32).astype(np.float64), np.asarray(c, f32).astype(np.float64)
+    with np.errstate(all="ignore"):
+        return device_sum(R * R), device_sum(R * c), device_sum(c * c)
 
 
 def apg_final(srr, src, scc, w, eta, norm_threshold):
@@ -134,7 +144,7 @@ def apg_words_exact(R, c, w, eta, norm_threshold):
 # ---- the executor ----------------------------------------------------------------------------------------------------
 
 class APGOracle(EDMOracle):
-    """The numpy executor with dpm_apg_words and dpm_step_apg. `exact`: the words summed in apg.cu's order
+    """The numpy executor with dpm_apg_words and dpm_step_apg. `exact`: the words summed in words.cu's order
     (apg_words_exact), bit-exact with the device; otherwise in numpy's pairwise order (within an ulp of it)."""
 
     def __init__(self, exact=False):

@@ -3,7 +3,7 @@
 * `s_star_fsum`: the optimised scale of each sample from exactly rounded sums (math.fsum), the division in fp64 and
   one rounding to fp32: the formula of Fan, Zheng, Yeh and Liu, "CFG-Zero*: Improved Classifier-Free Guidance for Flow
   Matching Models" (2025, arXiv:2503.18886), with diffusers' 1e-8 in the denominator.
-* `s_star_exact`: the same scale as dpm_cfgzero_scale sums it, operation for operation: apg.cu's chunks, thread
+* `s_star_exact`: the same scale as dpm_cfgzero_scale sums it, operation for operation: words.cu's chunks, thread
   ownership, warp butterflies, warp order and chunk merge (apg_oracle.apg_sums_exact), so that it is bit-exact with
   the device.
 * `cfgzero_combine`: g = us + w*(c - us), us = u*s*, in torch fp32 ops in that order (a per-sample scale of 1: c).
@@ -46,7 +46,8 @@ def s_star_fsum(c, u):
 
 
 def s_star_exact(c, u):
-    """fp32 [B] as k_cfgzero_partial + k_cfgzero_final compute it, from [B, per_sample] rows in storage order."""
+    """fp32 [B] as the CFG-Zero* words pass (PairPass<2>) + k_cfgzero_final compute it, from [B, per_sample] rows
+    in storage order."""
     uu, uc, _ = apg_sums_exact(np.asarray(u, f32), np.asarray(c, f32))   # (the fp64 product c*u == u*c, exactly)
     with np.errstate(all="ignore"):
         return (uc / (uu + EPS)).astype(f32)

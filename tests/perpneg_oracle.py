@@ -2,8 +2,8 @@
 
 * `perpneg_reference`: the method in float64, written from its formula: with d_k = e_k - u per sample,
   eps = u + s_1*d_1 + sum_{k>=2} s_k*(d_k - (<d_k, d_1>/||d_1||^2)*d_1).
-* `sums_exact`: the fp64 sums N = sum d_1*d_1 and P_k = sum d_k*d_1 as k_perpneg_partial + k_perpneg_final form them:
-  the chunks, thread ownership, warp butterflies, warp order and chunk merge of the CFG-Zero* pass.
+* `sums_exact`: the fp64 sums N = sum d_1*d_1 and P_k = sum d_k*d_1 as the Perp-Neg words pass forms them
+  (apg_oracle.device_sum: the chunks, thread ownership, warp butterflies, warp order and chunk merge of words.cu).
 * `words_final`: k_perpneg_final's fold of the merged sums, fp64 left to right with each op rounded, rounded to fp32.
 * `words_exact`: both together, bit-exact with dpm_perpneg_words; `words_fsum`: the fold on exactly rounded sums.
 * `PerpNegOracle`: the numpy executor (cfg_mask_oracle.MaskOracle, which serves dpm_step_multi_masked) plus
@@ -16,12 +16,12 @@ import math
 import numpy as np
 import torch
 
+from apg_oracle import device_sum
 from cfg_mask_oracle import MaskOracle
 from cfgzero_oracle import _storage_rows
 
 f32 = np.float32
 NAN32 = np.array([0x7fffffff], np.uint32).view(np.float32)[0]    # the NaN k_perpneg_final writes
-CHUNK, THREADS, WARP = 8192, 256, 32
 
 
 def perpneg_reference(u, es, scales):
@@ -38,32 +38,6 @@ def perpneg_reference(u, es, scales):
     return out
 
 
-def _device_sum(prod):
-    """Sum the fp64 products [B, per_sample] per sample in the device's order: CTA (b, chunk) covers chunk elements
-    [chunk*8192, min(+8192, per_sample)); thread tid adds the products of its elements (u*256 + tid)*8 + i, u = 0..3,
-    i = 0..7, in that order to 0.0; each warp folds by v += shfl_xor(v, o), o = 16 .. 1; s = 0.0 + warp 0 + ... +
-    warp 7; the chunks are merged from 0.0 in chunk order. Missing elements add +0.0, which changes no such sum."""
-    Bn, ps = prod.shape
-    chunks = -(-ps // CHUNK)
-    pad = chunks * CHUNK - ps
-    with np.errstate(all="ignore"):
-        prod = np.concatenate([prod, np.zeros((Bn, pad))], axis=1) if pad else prod
-        per_thread = prod.reshape(Bn, chunks, 4, THREADS, 8).transpose(0, 1, 3, 2, 4).reshape(Bn, chunks, THREADS, 32)
-        v = np.zeros((Bn, chunks, THREADS))
-        for k in range(32):
-            v = v + per_thread[..., k]
-        lanes = v.reshape(Bn, chunks, THREADS // WARP, WARP)
-        for o in (16, 8, 4, 2, 1):
-            lanes = lanes + lanes[..., np.arange(WARP) ^ o]
-        s = np.zeros((Bn, chunks))
-        for w in range(THREADS // WARP):
-            s = s + lanes[:, :, w, 0]
-        t = np.zeros(Bn)
-        for ch in range(chunks):
-            t = t + s[:, ch]
-    return t
-
-
 def _diffs(u, es):
     """d_k = e_k - u in fp64 from fp32 [B, per_sample] rows."""
     u = np.asarray(u, f32).astype(np.float64)
@@ -75,7 +49,7 @@ def sums_exact(u, es):
     """(N, [P_2 .. P_K]) per sample, fp64 [B] each, as the device forms them from [B, per_sample] rows."""
     d = _diffs(u, es)
     with np.errstate(all="ignore"):
-        return _device_sum(d[0] * d[0]), [_device_sum(dk * d[0]) for dk in d[1:]]
+        return device_sum(d[0] * d[0]), [device_sum(dk * d[0]) for dk in d[1:]]
 
 
 def words_final(N, P, scales):

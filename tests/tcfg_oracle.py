@@ -6,7 +6,7 @@
 * `words_closed_form`: the closed form of the contract on given fp64 sums (A, B, C) = (||u||^2, <u, c>, ||c||^2),
   fp64 with each op rounded, each word rounded to fp32 once.
 * `words_fsum`: the closed form on exactly rounded sums (math.fsum).
-* `words_exact`: the words as dpm_tcfg_words computes them, operation for operation: the CFG-Zero* pass's chunks,
+* `words_exact`: the words as dpm_tcfg_words computes them, operation for operation: words.cu's chunks,
   thread ownership, warp butterflies, warp order and chunk merge (apg_oracle.apg_sums_exact), then the closed form.
 * `tcfg_combine`: g = us + w*(c - us), us = u*wu + c*wc, in torch fp32 ops in that order (a per-sample scale of 1: c).
 * `TCFGOracle`: the numpy executor (cfgzero_oracle.CFGZeroOracle) plus dpm_tcfg_words and dpm_step_tcfg as
@@ -74,8 +74,8 @@ def words_fsum(c, u):
 
 
 def words_exact(c, u):
-    """fp32 [B, 2] as k_cfgzero_partial<NS = 3> + k_tcfg_final compute them, from [B, per_sample] rows in storage
-    order. apg_sums_exact(R, c) sums R*R, R*c, c*c in the device's order: with R = u these are A, B, C."""
+    """fp32 [B, 2] as the TCFG words pass (PairPass<3>) + k_tcfg_final compute them, from [B, per_sample] rows in
+    storage order. apg_sums_exact(R, c) sums R*R, R*c, c*c in the device's order: with R = u these are A, B, C."""
     A, B, C = apg_sums_exact(np.asarray(u, f32), np.asarray(c, f32))
     return words_closed_form(A, B, C)
 

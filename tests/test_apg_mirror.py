@@ -1,7 +1,7 @@
-"""The exact mirror of apg.cu's words reduction (apg_oracle.apg_words_exact), on the CPU: it is still the paper's
+"""The exact mirror of words.cu's APG words reduction (apg_oracle.apg_words_exact), on the CPU: it is still the paper's
 formula -- within an ulp of the fp64 words summed in numpy's order over many shapes and over finite edge data, with the
 same non-finite results -- and its vectorised order is the kernel's, thread by thread, against a plain loop over the
-CTAs, threads and lanes of k_apg_partial."""
+CTAs, threads and lanes of the words pass."""
 import numpy as np
 import pytest
 
@@ -13,7 +13,7 @@ PER_SAMPLE = [1, 7, 8, 9, 104, 1000, 8191, 8192, 8193, 8192 * 3 - 8, 16384, 3 * 
 
 
 def loop_sums(R, c):
-    """k_apg_partial and k_apg_final's merge written as plain loops (one python add per device add)."""
+    """The APG words pass and k_apg_final's merge written as plain loops (one python add per device add)."""
     Bn, ps = R.shape
     chunks = -(-ps // CHUNK)
     out = []

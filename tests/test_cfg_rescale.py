@@ -26,6 +26,36 @@ def ratio64(c, g):
         return (np.std(c64, axis=1, ddof=1).astype(f32) / np.std(g64, axis=1, ddof=1).astype(f32)).astype(f32)
 
 
+def ratio_exact(c, g):
+    """ratio64 as dpm_cfg_rescale_ratio computes it, operation for operation, from fp32 [B, per_sample] rows: per chunk
+    the fp64 mean (the chunk's device-order sum over its cnt live elements, / cnt) and the sum of squared deviations
+    from it (dead elements add +0.0), then Chan et al.'s merge in chunk order as k_cfg_ratio_final writes it."""
+    from apg_oracle import CHUNK, chunk_sums     # (apg_oracle imports this module through the executors)
+    Bn, ps = c.shape
+    live = np.minimum(CHUNK, ps - CHUNK * np.arange(-(-ps // CHUNK))).astype(np.float64)   # cnt of each chunk
+    stats = []
+    with np.errstate(all="ignore"):
+        for v in (np.asarray(c, f32).astype(np.float64), np.asarray(g, f32).astype(np.float64)):
+            mean = chunk_sums(v) / live
+            d = v - np.repeat(mean, CHUNK, axis=1)[:, :ps]
+            stats.append((mean, chunk_sums(d * d)))
+        out = np.empty(Bn, f32)
+        for b in range(Bn):
+            n = 0.0
+            (mc, qc), (mg, qg) = [(m[b, 0], q[b, 0]) for m, q in stats]
+            for k in range(len(live)):
+                nb = live[k]
+                if k:
+                    nab = n + nb
+                    wb, wab = nb / nab, n * nb / nab
+                    dc, dg = stats[0][0][b, k] - mc, stats[1][0][b, k] - mg
+                    mc, qc = mc + dc * wb, (qc + stats[0][1][b, k]) + dc * dc * wab
+                    mg, qg = mg + dg * wb, (qg + stats[1][1][b, k]) + dg * dg * wab
+                n += nb
+            out[b] = f32(np.sqrt(qc / (n - 1.0))) / f32(np.sqrt(qg / (n - 1.0)))
+    return out
+
+
 class RescaleOracle(OracleBackend):
     """OracleBackend plus the rescale: r in fp64 numpy, g' = phi*(g*r) + psi*g in fp32 numpy."""
 

@@ -2,7 +2,7 @@
 guidance difference overflows, scattered (step_edges.scatter_edges) into one sample's x, conditional and unconditional
 outputs and momentum buffer, for every parameterisation and dtype pair, on the vector words path with the direct step
 kernel and on the element-wise words path with k_step_scalar_apg. The words, R and the step's outputs must equal the
-exact oracle bit for bit, and every other sample must come out as in a run where the edge sample is finite (apg.cu:
+exact oracle bit for bit, and every other sample must come out as in a run where the edge sample is finite (words.cu:
 the words of sample b depend on its values only). Built cases: c = 0 in one sample, out_c == out_u (R = 0 with a
 threshold), R beyond fp32, one NaN, an infinite R on a bypassed row (its output is c exactly) and the smallest positive
 threshold; where the fp64 formula (APG64) defines the result, the non-finite pattern is its pattern."""

@@ -1,4 +1,4 @@
-"""Adaptive projected guidance on the H100, bit for bit: the words of dpm_apg_words against the exact mirror of apg.cu
+"""Adaptive projected guidance on the H100, bit for bit: the words of dpm_apg_words against the exact mirror of words.cu
 (apg_oracle.apg_words_exact) on every dtype pair, on sample sizes that end inside a packet, at a chunk edge and past it,
 on the vector and the element-wise path, with and without momentum (R too), with per-sample scales and channels_last;
 the merge order of a sample's chunks; the coefficient block (dev_coef) of the adaptive controller feeding both the words

@@ -10,7 +10,7 @@ import torch
 import torch.multiprocessing as mp
 
 from cases import exact_net, make_betas, seeded
-from test_cfg_rescale import PHI, S, RescaleOracle, inner_net, ratio64, ref_rescaled_net, schedules
+from test_cfg_rescale import PHI, S, RescaleOracle, inner_net, ratio64, ratio_exact, ref_rescaled_net, schedules
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -83,6 +83,28 @@ def test_ratio_kernel_vs_fp64(cuda_backend, dt, ps):
             for b in range(B):      # a sample alone (aligned, fresh storage) gives the same bits as inside the batch
                 rb = cuda_backend.cfg_rescale_ratio(c[b:b + 1].clone(), u[b:b + 1].clone(), S)
                 assert rb.cpu().numpy().tobytes() == got[b:b + 1].tobytes(), (regime, offset, b)
+
+
+@pytest.mark.parametrize("dt", ["f32", "bf16", "f16"])
+@pytest.mark.parametrize("ps", SIZES)
+def test_ratio_kernel_bit_exact(cuda_backend, dt, ps):
+    """The ratio against its exact mirror (ratio_exact) bit for bit, with one scale and with per-sample scales. This
+    pins the algorithm -- each chunk's mean over its cnt live elements, dead elements adding +0 to the squared
+    deviations, the two reductions per chunk and Chan's merge -- not the order of the fp64 additions, which moves these
+    sums far less than an fp32 ulp of the rounded stds."""
+    gen = torch.Generator().manual_seed(ps + 1)
+    B = 5 if ps < 100000 else 3
+    scales = torch.tensor([S, 1.0, 0.0, 7.25, -2.5][:B], dtype=torch.float32)
+    for regime in ["random", "special"] + (["large_mean"] if dt != "f16" else []):
+        for offset in (0, 1):
+            c, u = halves(B, ps, DT[dt], gen, regime, offset)
+            cn, un = c.float().cpu().numpy(), u.float().cpu().numpy()
+            for s, w in ((S, np.float32(S)), (scales.cuda(), scales.numpy().reshape(B, 1))):
+                got = cuda_backend.cfg_rescale_ratio(c, u, s).cpu().numpy()
+                want = ratio_exact(cn, (un + w * (cn - un)).astype(np.float32))
+                nan = np.isnan(want)    # (numpy's 0/0 and the device's NaN differ in sign and payload)
+                assert np.array_equal(np.isnan(got), nan) and got[~nan].tobytes() == want[~nan].tobytes(), \
+                    (regime, offset, torch.is_tensor(s), got, want)
 
 
 def test_ratio_kernel_channels_last(cuda_backend):
