@@ -142,6 +142,18 @@ class Rig:
         self.scale = scale
         self.fn = mod.model_wrapper(net, self.ns, condition=cond, guidance_scale=scale, **kw)
 
+    @property
+    def calls(self):
+        return self.__dict__.get("_calls")
+
+    @calls.setter
+    def calls(self, v):
+        """A list set here is also kept as `trace_log` after sample() lets go of it, so that a call that raised can be
+        checked for network calls."""
+        self._calls = v
+        if v is not None:
+            self.trace_log = v
+
     def make_schedule(self):
         kind, betas = make_betas(self.c["schedule"])
         return self.mod.NoiseScheduleVP("linear") if kind == "linear" else \

@@ -1,5 +1,5 @@
-"""Random CFG-Zero*, CFG++, regional-guidance, TCFG and frequency-decoupled-guidance `sample()` configurations for the
-end-to-end tests on the device (tests/test_gpu_guidance_random_configs.py) and their CPU side
+"""Random CFG-Zero*, CFG++, regional-guidance, TCFG, frequency-decoupled-guidance and Perp-Neg `sample()` configurations
+for the end-to-end tests on the device (tests/test_gpu_guidance_random_configs.py) and their CPU side
 (tests/test_guidance_draws_vs_reference.py): the draw (apg_configs.draw_apg's base, one feature per configuration), a
 `GuidanceRig` and the CPU oracle.
 
@@ -20,16 +20,22 @@ state and model dtypes, inverse(), denoise_to_zero, t_start / t_end, skip types 
     refuses; the scales as N floats, N one-element tensors, a 1-D tensor, an fp32 [B, N] tensor read in place, a bf16
     or CPU [B, N] tensor (converted), or a [B + 1, N] tensor (refused); now and then equal scales, whose run must be
     the N == 1 run.
+  * perp: K = 2..4 conditions with scales from PERP_SCALES (negatives, 0 and 1), now and then a sample whose first
+    condition is the unconditional one (||d_1|| = 0: its word is s_1); DPM_Solver (every method); now and then a
+    configuration Perp-Neg refuses (PERP_REFUSALS: per-sample scales, a guidance_mask, UniPC, a single condition,
+    reference_rounding).
 
 The oracle of a configuration, on CPU tensors:
   * the product's host logic on the numpy executor -- `MaskOracle(exact=True)` (which is also the CFG++, CFG-Zero* and
-    APG executor), or for tcfg and fdg `FDGOracle()` (TCFG's words in the device's summation order): y, every
-    intermediate and the trace of network calls -- what the device must give bit for bit;
+    APG executor), for tcfg and fdg `FDGOracle()` (TCFG's words in the device's summation order), for perp
+    `PerpNegOracle(exact=True)` (the words in the device's summation order): y, every intermediate and the trace of
+    network calls -- what the device must give bit for bit;
   * where the unmodified reference can express the configuration, the executor against it with as many network calls:
     cfgzero, tcfg and fdg bit for bit through cfgzero_oracle / tcfg_oracle / fdg_oracle.guided_net behind a
     guidance_type="uncond" wrapper, cfgpp within CFGPP_TOL of cfgpp_oracle.cfgpp_fp64 (plus, for an x_start network,
     the rounding bound of its x0 conversion: _reference_cfgpp), mask bit for bit against
-    test_cfg_mask.reference_composed;
+    test_cfg_mask.reference_composed, perp bit for bit through perpneg_oracle.guided_net behind a
+    guidance_type="uncond" wrapper (a noise network) or test_perp_neg.reference_composed (the other model types);
   * a configuration the product refuses is {"error": exception}.
 """
 import contextlib
@@ -43,8 +49,9 @@ from apg_configs import APGRig, draw_apg, per_sample, reference_schedule
 from cfg_mask_oracle import MaskOracle
 from fdg_oracle import FDGOracle
 from gpu_configs import backend, really_channels_last, rel_err, same_bits, sample_kwargs
+from perpneg_oracle import PerpNegOracle
 
-FEATURES = ("cfgzero", "cfgpp", "mask", "tcfg", "fdg")
+FEATURES = ("cfgzero", "cfgpp", "mask", "tcfg", "fdg", "perp")
 BEYOND = 1000                 # a cfg_zero_init_steps above any run's number of evaluations: every evaluation is 0
 CFGPP_TOL = 1e-5              # tests/test_cfg_pp.py's bound against the fp64 transcription
 XSTART_ROUNDING = 3           # x_start under CFG++: multiples of what its fp32 x0 conversion alone moves a run
@@ -57,7 +64,9 @@ CFGPP_REFUSALS =("dpmsolver", "order3", "singlestep", "adaptive", "unipc", "thre
 FDG_PLANES = [(4, 64, 64), (3, 72, 64), (2, 64, 128), (1, 126, 130), (2, 6, 6), (3, 24, 40)]
 FDG_FORMS = ("floats", "listed", "vec", "rows", "rows", "bf16", "cpu")     # (+ "bad_rows" now and then: refused)
 FDG_VALUES = [7.0, 3.5, 1.5, 1.0, 0.0, -1.0, 10.0, 2.5]                  # (exact in bf16)
-CHUNKS, PER_CHUNK, SEED = 10, 20, 9900    # the device test: 10 chunks of 20 configurations
+PERP_SCALES = [7.5, 4.0, 1.0, 0.0, -1.0, -2.5, -0.5]
+PERP_REFUSALS = ("per_sample", "mask", "unipc", "single", "rr")
+CHUNKS, PER_CHUNK, SEED = 12, 22, 9900    # the device test: 12 chunks of 22 configurations
 
 
 def draw_guidance(rng):
@@ -67,8 +76,9 @@ def draw_guidance(rng):
     B = c["B"]
     c["zero_init"], c["K"], c["masks"], c["cfgpp_refusal"] = 0, 0, None, None
     c["fdg_levels"], c["fdg_form"], c["fdg_w"], c["fdg_equal"] = 0, None, None, False
+    c["perp_refusal"], c["perp_d1_zero"] = None, None
     if c["schedule"] in ("flow", "edm") and rng.random() < {"cfgzero": 0.25, "cfgpp": 0.25, "mask": 0.5, "tcfg": 0.25,
-                                                             "fdg": 0.25}[f]:
+                                                             "fdg": 0.25, "perp": 0.5}[f]:
         c.update(schedule=rng.choice(VP), model_type=rng.choice(["noise", "x_start", "v", "score"]))
     if f in ("cfgzero", "cfgpp"):
         ones = [1.0, 3.5, 7.5] if f == "cfgzero" else [0.2, 0.6, 1.0, 7.5]
@@ -102,6 +112,8 @@ def draw_guidance(rng):
             c["thresholding"] = True
     elif f == "fdg":
         draw_fdg(rng, c)
+    elif f == "perp":
+        draw_perp(rng, c)
     elif f == "cfgpp":
         c.update(sampler="dpm", method="multistep", order=rng.choice([1, 2]), algo="dpmsolver++", thresholding=False,
                  reference_rounding=False, steps=max(c["steps"], 3))
@@ -123,6 +135,65 @@ def draw_guidance(rng):
         c["masks"] = [(rng.choice(MASK_KINDS), rng.choice(MASK_FORMS)) for _ in range(K)]
         c.update(guidance="multi", cfg=None, scales=[rng.choice([7.5, -2.0, 0.0, 1.5, 3.0, 1.0]) for _ in range(K)])
     return c
+
+
+def draw_perp(rng, c):
+    """The perp part of a draw: K, the scales, a sample with ||d_1|| = 0 now and then, a refusal now and then."""
+    B = c["B"]
+    if c["sampler"] == "unipc":
+        c["sampler"] = "dpm"
+    c["steps"] = max(c["steps"], c["order"])
+    K = c["K"] = rng.randint(2, 4)
+    c.update(guidance="perp", cfg=None, scales=[rng.choice(PERP_SCALES) for _ in range(K)])
+    if rng.random() < 0.25:
+        c["perp_d1_zero"] = rng.randrange(B)
+    if rng.random() < 0.25:
+        why = c["perp_refusal"] = rng.choice(PERP_REFUSALS)
+        if why == "unipc":
+            c.update(sampler="unipc", variant="bh2", use_corrector=False, method="multistep", inverse=False)
+        elif why == "single":
+            c.update(K=1, scales=c["scales"][:1])
+        elif why == "rr":
+            c["reference_rounding"] = True
+
+
+def perp_refusal_reached(c):
+    """Whether Perp-Neg's own refusal decides a perp draw that carries one: the same draw without it (the single
+    condition, UniPC or reference_rounding undone) is one the product accepts, so no other check can refuse it first."""
+    if c["feature"] != "perp" or c["perp_refusal"] is None:
+        return False
+    undone = dict(c, perp_refusal=None, K=max(c["K"], 2), scales=c["scales"] + [1.0] * (2 - len(c["scales"])))
+    if c["perp_refusal"] == "unipc":
+        undone["sampler"] = "dpm"
+    if c["perp_refusal"] == "rr":
+        undone["reference_rounding"] = False
+    return not refused(undone)
+
+
+def perp_conditions(c, device):
+    """The K conditions [B, 1]: k + 1 for condition k, except 0 (the unconditional one) for condition 1 of sample
+    c["perp_d1_zero"]."""
+    cond = [torch.full((c["B"], 1), float(k + 1), device=device) for k in range(c["K"])]
+    if c["perp_d1_zero"] is not None:
+        cond[0][c["perp_d1_zero"]] = 0.0
+    return cond
+
+
+def perp_net(base):
+    """`base` (APGRig's network, whose conditional differences are all parallel) plus (c*c/100)*y*y with y = x clamped
+    to [-2, 2], a bounded condition term nonlinear in x: the differences d_k of distinct conditions are then not parallel, and Perp-Neg's perpendicular parts
+    do not vanish. A condition of 0 adds nothing (||d_1|| = 0 stays exact). Exact IEEE products and sums, in the
+    output's dtype and layout."""
+    def net(xx, tt, cc=None):
+        o = base(xx, tt, cc)
+        if cc is None:
+            return o
+        one = (-1,) + (1,) * (xx.dim() - 1)
+        y = xx.float().clamp(-2.0, 2.0)
+        r = (o.float() + ((0.01 * cc.reshape(one)) * cc.reshape(one)) * (y * y)).to(o.dtype)
+        cl = o.dim() == 4 and not o.is_contiguous() and o.is_contiguous(memory_format=torch.channels_last)
+        return r.contiguous(memory_format=torch.channels_last) if cl else r.contiguous()
+    return net
 
 
 def fdg_max_levels(shape):
@@ -181,7 +252,10 @@ def fdg_values(c):
 
 
 def executor(c):
-    """The numpy executor of `c`: FDGOracle (which also runs TCFG) for tcfg and fdg, MaskOracle(exact=True) else."""
+    """The numpy executor of `c`: FDGOracle (which also runs TCFG) for tcfg and fdg, PerpNegOracle(exact=True) for perp,
+    MaskOracle(exact=True) else."""
+    if c["feature"] == "perp":
+        return PerpNegOracle(exact=True)
     return FDGOracle() if c["feature"] in ("tcfg", "fdg") else MaskOracle(exact=True)
 
 
@@ -212,10 +286,10 @@ def make_masks(c, device):
 
 
 class GuidanceRig(APGRig):
-    """APGRig with CFG-Zero*, CFG++, regional guidance, TCFG or frequency-decoupled guidance in model_wrapper. `masks`
-    replaces the drawn masks, `fdg` the drawn fdg_scales."""
+    """APGRig with CFG-Zero*, CFG++, regional guidance, TCFG, frequency-decoupled guidance or Perp-Neg in model_wrapper.
+    `masks` replaces the drawn masks, `fdg` the drawn fdg_scales, `scales` the drawn Perp-Neg scales."""
 
-    def __init__(self, mod, c, device="cpu", masks=None, fdg=None):
+    def __init__(self, mod, c, device="cpu", masks=None, fdg=None, scales=None):
         super().__init__(mod, dict(c, guidance="none"), device)
         self.c = c
         B, dev = c["B"], self.device
@@ -226,6 +300,17 @@ class GuidanceRig(APGRig):
             self.fdg = make_fdg_scales(c, dev) if fdg is None else fdg
             self.fn = mod.model_wrapper(self.net, self.ns, condition=torch.ones(B, 1, device=dev), fdg_scales=self.fdg,
                                         **kw)
+            return
+        if c["feature"] == "perp":
+            why = c["perp_refusal"]
+            scale = list(c["scales"] if scales is None else scales)
+            if why == "per_sample":
+                scale = torch.tensor([scale] * B, dtype=torch.float32, device=dev).T.contiguous()    # [K, B]
+            if why == "mask":
+                kw["guidance_mask"] = [torch.ones(B, 1, 1, 1, device=dev)] + [None] * (c["K"] - 1)
+            self.net = perp_net(self.net)
+            self.fn = mod.model_wrapper(self.net, self.ns, condition=perp_conditions(c, dev), guidance_scale=scale,
+                                        perp_neg=True, **kw)
             return
         if c["feature"] == "mask":
             self.masks = make_masks(c, dev) if masks is None else masks
@@ -259,6 +344,8 @@ def refused(c):
     if unipc and c["steps"] < c["order"]:
         return True
     f = c["feature"]
+    if f == "perp":
+        return unipc or c["perp_refusal"] is not None
     if f == "fdg":
         # (the size rule, more than 5 levels, and a [B', N] tensor for a batch of B)
         return c["fdg_levels"] > fdg_max_levels(c["shape"]) or c["fdg_form"] == "bad_rows"
@@ -281,7 +368,7 @@ def _fp32(c):
 def reference_expressible(c):
     """cfgzero, tcfg and fdg: fp32 DPM_Solver, not adaptive, a network the reference's wrappers take on its schedule;
     cfgpp: fp32, a network with a closed-form x0, no denoise_to_zero; mask: fp32 DPM_Solver on a VP schedule, not
-    adaptive. Never inverse()."""
+    adaptive; perp: fp32 DPM_Solver on a VP schedule, not adaptive, the network's outputs row-major. Never inverse()."""
     if refused(c) or not _fp32(c) or c["inverse"] or c["sampler"] != "dpm" or c["method"] == "adaptive":
         return False
     sched, mt = c["schedule"], c["model_type"]
@@ -289,7 +376,15 @@ def reference_expressible(c):
         return mt == sched if sched in ("flow", "edm") else mt in ("noise", "x_start", "v", "score")
     if c["feature"] == "cfgpp":
         return mt in ("noise", "x_start", "v", "score", "flow") and sched != "edm" and not c["denoise_to_zero"]
+    if c["feature"] == "perp" and not row_major_outputs(c):
+        return False
     return sched not in ("flow", "edm") and mt in ("noise", "x_start", "v", "score")
+
+
+def row_major_outputs(c):
+    """Whether the network's outputs are row-major: it returns row-major ones, or keeps a row-major x's layout."""
+    x_cl = c["x_channels_last"] and really_channels_last(dict(c, channels_last=True))
+    return not (c["net_layout"] == "cl" and really_channels_last(c)) and not (c["net_layout"] == "keep" and x_cl)
 
 
 def _guided_net(c, rig):
@@ -344,6 +439,34 @@ def _reference_mask(c, rig, x):
     s.thresholding_max_val, s.dynamic_thresholding_ratio = c["max_val"], c["ratio"]
     with contextlib.redirect_stdout(io.StringIO()):
         return s.sample(x, **sample_kwargs(c)), n[0]
+
+
+def _reference_perp(c, rig, x):
+    """Perp-Neg in the reference: for a noise network perpneg_oracle.guided_net behind a guidance_type="uncond" wrapper,
+    else test_perp_neg.reference_composed, both on rig's network, conditions and the drawn scales."""
+    from perpneg_oracle import guided_net
+    from test_perp_neg import reference_composed
+    B, rns = c["B"], reference_schedule(c)
+    uc, cond = torch.zeros(B, 1), perp_conditions(c, "cpu")
+    n = [0]
+    if c["model_type"] == "noise":
+        from gpu_configs import reference
+        ref, calls = reference(), []
+        fn = ref.model_wrapper(guided_net(rig.net, uc, cond, c["scales"], calls), rns, model_type="noise")
+    else:
+        ref, _, composed = reference_composed(c["model_type"], c["K"], model=rig.net, batch=B, scales=c["scales"],
+                                              rns=rns, condition=cond)
+        calls = None
+
+        def fn(xx, t):
+            n[0] += 1
+            return composed(xx, t)
+    s = ref.DPM_Solver(fn, rns, algorithm_type=c["algo"],
+                       correcting_x0_fn="dynamic_thresholding" if c["thresholding"] else None)
+    s.thresholding_max_val, s.dynamic_thresholding_ratio = c["max_val"], c["ratio"]
+    with contextlib.redirect_stdout(io.StringIO()):
+        y = s.sample(x, **sample_kwargs(c))
+    return y, len(calls) if calls is not None else n[0]
 
 
 def _cfgpp_fp64(c, rig, x, rounded=False):
@@ -419,7 +542,7 @@ def reference_run(c, rig):
     if c["feature"] == "cfgpp":
         return _reference_cfgpp(c, rig, x)
     run = {"cfgzero": _reference_uncond, "tcfg": _reference_uncond, "fdg": _reference_uncond,
-           "mask": _reference_mask}[c["feature"]]
+           "mask": _reference_mask, "perp": _reference_perp}[c["feature"]]
     return run(c, rig, x) + (None,)
 
 
@@ -428,11 +551,14 @@ def cpu_oracle(c):
     compared; {"error": exception} when the product refuses the configuration."""
     import dpm_solver_b200 as new
     out = {}
-    with backend(executor(c)):
+    with backend(executor(c)) as be:
+        rig = None
         try:
             rig = GuidanceRig(new, c)
             out["y"], out["inter"], out["calls"] = rig.sample(rig.solver(), rig.x(), trace=True)
         except (ValueError, AssertionError) as e:
+            # a refusal comes before any launch and any network call
+            assert be.launch_count() == 0 and not getattr(rig, "trace_log", None), (c, e)
             return {"error": e}
         if c["fdg_equal"]:
             # equal scales: the pyramid terms vanish, so the run is the one-level run's bit for bit
@@ -477,7 +603,7 @@ def tally_static(c):
             keys.append("layout change:row-major outputs of a channels_last state")
     if c["net_layout"] == "cl" and not c["x_channels_last"] and really_channels_last(c):
         keys.append("layout change:channels_last outputs of a row-major state")
-    if f in ("tcfg", "fdg"):
+    if f in ("tcfg", "fdg", "perp"):
         keys += [f + ":" + k for k in keys if k.startswith("layout change:")]
     if c["sampler"] == "dpm":
         keys.append("method:" + c["method"])
@@ -510,6 +636,15 @@ def tally_static(c):
             keys.append("fdg:planes>1 per sample")
         if c["fdg_equal"] and c["fdg_levels"] > 1:
             keys.append("fdg:equal scales")
+    elif f == "perp":
+        keys.append("perp:K=%d" % c["K"])
+        if ps % 8:
+            keys.append("perp:words element path")
+        if ps > 8192:
+            keys.append("perp:words multi-chunk")
+        if c["perp_d1_zero"] is not None:
+            keys.append("perp:|d1|=0")
+        keys += ["perp:" + k for k in ("inverse", "d2z") if k in keys]
     elif f == "cfgpp":
         keys.append("cfgpp:order%d" % c["order"])
         if c["cfg"] == 1.0:
@@ -539,8 +674,10 @@ REQUIRED = (["feature:" + f for f in FEATURES] + ["schedule:vp", "schedule:flow"
             ["tcfg:bypass", "tcfg:per-sample row at 1", "tcfg:materialised"] +
             ["fdg:levels=1", "fdg:levels=5", "fdg:scalar path", "fdg:planes>1 per sample", "fdg:equal scales"] +
             ["fdg:scales:" + k for k in ("floats", "listed", "vec", "rows", "converted")] +
-            [f + ":layout change:" + k for f in ("tcfg", "fdg") for k in ("row-major outputs of a channels_last state",
-                                                                          "channels_last outputs of a row-major state")])
+            ["perp:K=%d" % k for k in (2, 3, 4)] +
+            ["perp:" + k for k in ("words element path", "words multi-chunk", "|d1|=0", "inverse", "d2z")] +
+            [f + ":layout change:" + k for f in ("tcfg", "fdg", "perp")
+             for k in ("row-major outputs of a channels_last state", "channels_last outputs of a row-major state")])
 REQUIRED_ON_DEVICE = ["rejected", "captured", "captured:zero-init", "captured:rewritten-mask", "second_stream",
                       "pinned", "fdg:frozen step served", "fdg:frozen step fell back", "captured:fdg rows rewritten"]
 

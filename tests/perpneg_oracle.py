@@ -6,6 +6,7 @@
   (apg_oracle.device_sum: the chunks, thread ownership, warp butterflies, warp order and chunk merge of words.cu).
 * `words_final`: k_perpneg_final's fold of the merged sums, fp64 left to right with each op rounded, rounded to fp32.
 * `words_exact`: both together, bit-exact with dpm_perpneg_words; `words_fsum`: the fold on exactly rounded sums.
+* `fold_order_case`: blocks whose words differ between the fold's order and its reverse (`words_final_reversed`).
 * `PerpNegOracle`: the numpy executor (cfg_mask_oracle.MaskOracle, which serves dpm_step_multi_masked) plus
   dpm_perpneg_words, operation for operation.
 * `guided_net`: a network for the UNMODIFIED reference's guidance_type="uncond" wrapper that runs a noise network on
@@ -118,3 +119,24 @@ def guided_net(net, uc, conds, scales, calls=None):
         w1 = words_exact(_storage_rows(outs[0]), [_storage_rows(o, outs[0]) for o in outs[1:]], scales)
         return perp_combine(outs[0], outs[1:], scales, torch.from_numpy(w1))
     return fn
+
+
+def words_final_reversed(N, P, scales):
+    """words_final with the terms s_k*c_k subtracted from s_1 last to first: the fold order a wrong kernel would use."""
+    return words_final(N, P[::-1], [scales[0]] + list(scales[1:])[::-1])
+
+
+def fold_order_case(B=16, D=96, seed=0):
+    """(u, [e_1 .. e_4], scales) as fp32 [B, D] arrays whose words expose the order of the fp64 fold. The blocks sit on
+    grids where every difference, product and sum is exact: d_2 = 2^13*d_1 and d_4 = -2^13*d_1, so c_2 = 2^13 and
+    c_4 = -2^13 exactly, and with s_2 = s_4 = 2^27 the terms s_2*c_2 = 2^40 and s_4*c_4 = -2^40 cancel exactly; d_3 is
+    noise, so s_3*c_3 is of order 1 with every fraction bit set. Folded first to last, t passes just below 2^40 (fp64
+    grid 2^-13) while s_1 and s_3*c_3 are pending; folded last to first, it passes just above 2^40 (grid 2^-12). The
+    two orders then round t differently by up to 2^-13 -- hundreds of fp32 ulps of a t near 1."""
+    rng = np.random.default_rng(seed)
+    u = (rng.integers(-4096, 4096, (B, D)) / 1024.0)
+    d1 = rng.choice([-8, -5, -3, -1, 1, 2, 4, 7], (B, D)) / 16.0
+    d3 = rng.integers(-4096, 4096, (B, D)) / 1024.0
+    es = [u + d1, u + 8192.0 * d1, u + d3, u - 8192.0 * d1]
+    assert all(np.array_equal(e.astype(f32).astype(np.float64), e) for e in [u] + es)
+    return u.astype(f32), [e.astype(f32) for e in es], [1.3, 2.0 ** 27, 1.7, 2.0 ** 27]

@@ -5,7 +5,9 @@
   expression of include/dpm_solver_b200.h plus cz*z in fp32, each op rounded. z is drawn by the contract, at the launch:
   `torch.empty_like(x, dtype=torch.float32).normal_(generator=g)` on x's device. On the GPU box that is the draw the
   kernel replays in registers, so the executor checks each launch bit for bit; on the CPU it is the CPU generator's.
-  `draws` keeps every z it drew, so a float64 run can be fed the same values.
+  `draws` keeps every z it drew, so a float64 run can be fed the same values. The update's output is laid out as the
+  CUDA backend lays it out (channels_last when x is, and no preallocated output says otherwise), so that the next
+  update's draw follows the same storage order.
 * `kdiff_sde`: k-diffusion's `sample_dpmpp_2m_sde` / `sample_dpmpp_3m_sde` loops restated in float64 in the VE
   coordinates x^ = x/alpha, sigma^ = sigma/alpha (t = -log sigma^ = lambda), with the first update(s) of lower order
   and the noise z_i given.
@@ -30,6 +32,10 @@ class SdeOracle(FDGOracle):
         super().__init__()
         self.draws = []
 
+    def draw(self, a):
+        """The noise of launch `a`: the contract's draw from its generator."""
+        return torch.empty_like(a.x, dtype=torch.float32).normal_(generator=a.sde.generator)
+
     def step(self, a):
         if getattr(a, "sde", None) is None:
             return super().step(a)
@@ -45,8 +51,7 @@ class SdeOracle(FDGOracle):
             self.launches += 1
             self.log.append((a.form, 0))
             m_out, T0 = None, _np(a.m0)
-        gen = a.sde.generator
-        z = torch.empty_like(a.x, dtype=torch.float32).normal_(generator=gen)
+        z = self.draw(a)
         self.draws.append(z.detach().cpu().clone())
         x, m1, m2, zz = _np(a.x), _np(a.m1), _np(a.m2), _np(z)
         A, c0, c1, c2 = f32(a.a), f32(a.c0), f32(a.c1), f32(a.c2)
@@ -62,6 +67,9 @@ class SdeOracle(FDGOracle):
             o = ((A * x + c0 * T0) + c1 * (D10 + w2 * dd)) + c2 * (w3 * dd)
         o = o + f32(a.sde.cz) * zz
         out = torch.from_numpy(np.ascontiguousarray(o.astype(f32))).to(sdt).reshape(ref.shape).to(ref.device)
+        if _launch_layout(a) == "cl":
+            # the state the launch writes keeps its layout, and the next update's draw follows that storage order
+            out = out.contiguous(memory_format=torch.channels_last if out.dim() == 4 else torch.channels_last_3d)
         if a.out is not None:
             a.out.copy_(out.reshape(a.out.shape))
             out = a.out
@@ -70,6 +78,17 @@ class SdeOracle(FDGOracle):
         if m_out is not None:
             m_out = m_out.to(ref.device) if a.want_m_out else None
         return m_out, out
+
+
+def _launch_layout(a):
+    """The storage order of a launch's outputs, as the CUDA backend picks it: x's dense layout ("c" or "cl"), or
+    row-major when x has none or a preallocated output is laid out otherwise."""
+    from dpm_solver_b200.ops import CudaBackend
+    layout = CudaBackend._layout(a.reference_tensor()) or "c"
+    for t in (a.out, a.m_out, a.out2):
+        if t is not None and CudaBackend._layout(t) != layout:
+            layout = "c"
+    return layout
 
 
 def kdiff_sde(x_T, denoise, alphas, sigmas, zs, eta, order, solver_type="dpmsolver"):

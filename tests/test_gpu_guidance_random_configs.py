@@ -1,11 +1,11 @@
-"""CFG-Zero*, CFG++, regional guidance, TCFG and frequency-decoupled guidance in `sample()`, `UniPC.sample()` and
-`inverse()` on the device over random configurations, bit for bit (tests/guidance_configs.py): paths A-E of
+"""CFG-Zero*, CFG++, regional guidance, TCFG, frequency-decoupled guidance and Perp-Neg in `sample()`, `UniPC.sample()`
+and `inverse()` on the device over random configurations, bit for bit (tests/guidance_configs.py): paths A-E of
 tests/test_gpu_apg_random_configs.py -- A the first call against the exact CPU executor (every intermediate and the
 trace of network calls), B the same call again (no guided evaluation frozen as a `PreparedStep`, except FDG's, which is
-one network output g: its frozen steps are served, and fall back when x comes in another layout), C another input on
-the same solver against a fresh solver (the zero-init count starts over), D `capture()` replays (zero-init included; a
-mask or an FDG [B, N] scale tensor read in place is rewritten after capture and the replay must follow it), E a fresh
-solver on a second stream. A refused configuration raises on the device and launches nothing. A module-wide tally
+one network output g: its frozen steps are served, and fall back when x comes in another layout), C another input on the
+same solver against a fresh solver (the zero-init count starts over), D `capture()` replays (zero-init included; a mask
+or an FDG [B, N] scale tensor read in place is rewritten after capture and the replay must follow it), E a fresh solver
+on a second stream. A refused configuration raises on the device before any launch or network call. A module-wide tally
 requires every path of interest to have been met by the fixed seeds."""
 import pytest
 import torch
@@ -66,10 +66,12 @@ def check_configuration(c, be, filler):
         want = cpu_oracle(c)
     if want is not None and "error" in want:
         before = be.launch_count()
+        rig = None
         with pytest.raises(ValueError):
             rig = GuidanceRig(new, c, "cuda:0")
-            rig.sample(rig.solver(), rig.x())
+            rig.sample(rig.solver(), rig.x(), trace=True)
         expect(be.launch_count() == before, "refused: the library launched")
+        expect(not getattr(rig, "trace_log", None), "refused: the network was called")
         hit("rejected")
         return bad
     if want is not None and not torch.isfinite(want["y"].float()).all():
@@ -123,8 +125,11 @@ def check_configuration(c, be, filler):
             if spy.fell_back and not bad:
                 hit("fdg:frozen step fell back")
     else:
-        # (key field [5]: e_uncond is None -- a frozen step holds one network output, never a guided pair)
+        # (key field [5]: e_uncond is None -- a frozen step holds one network output, never a guided pair or a
+        # Perp-Neg evaluation)
         expect(all(k[5] for k in s._prep_cache), "B: a guided step was frozen")
+        if c["feature"] == "perp":
+            expect(spy.dup + spy.plain == 0, "B: a Perp-Neg step was served by a PreparedStep")
     # ---- C: another input on the same solver against a fresh solver ----
     x2 = rig.x2()
     Cv = rig.sample(s, x2, trace=True)

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from oracle import ref_loader
-from perpneg_oracle import PerpNegOracle, words_exact
+from perpneg_oracle import PerpNegOracle, fold_order_case, words_exact
 from test_gpu_cfg_zero_star import DT, _on, same, unaligned
 from test_tcfg import product_schedule, reference_schedule
 
@@ -93,6 +93,15 @@ def test_words_ieee_edges(cuda_backend, dt):
     same(w, want)
     assert w[0] == np.float32(SCALES[K][0]) and w[6] == np.float32(SCALES[K][0])
     assert torch.isnan(w[3:6]).all() and torch.isnan(w[8])
+
+
+@pytest.mark.parametrize("seed", [0, 1, 2])
+def test_words_fold_order(cuda_backend, seed):
+    """Blocks whose words move by hundreds of fp32 ulps when the fp64 fold s_1 - s_2*c_2 - ... runs in another order
+    (perpneg_oracle.fold_order_case): bit for bit against the executor's left-to-right fold."""
+    u, es, s = fold_order_case(seed=seed)
+    w = cuda_backend.perpneg_words(torch.from_numpy(u).cuda(), [torch.from_numpy(e).cuda() for e in es], s)
+    assert np.array_equal(w.cpu().numpy().view(np.uint32), words_exact(u, es, s).view(np.uint32))
 
 
 def test_words_launch_beyond_2_31_elements(cuda_backend):

@@ -1,6 +1,7 @@
 """SDE-DPM-Solver++ on the H100: dpm_step_sde bit for bit against the numpy executor (tests/sde_oracle.py) with z drawn
 by the contract, the in-kernel normals against torch's normal_ at the edges of ATen's launch geometry (and beyond
 2^29 elements), sample() against the executor run, capture() replays and one full-size launch."""
+import dataclasses
 import random
 
 import pytest
@@ -65,23 +66,38 @@ def test_normals_beyond_2_29():
     assert off == g.get_offset()
 
 
-def _case(rng, i):
-    """One random launch: dtypes, outputs, form, guidance kind, thresholds, size and layout."""
+def _sized_shape(rng, n):
+    """A [B, C, 1, W] shape of exactly n elements: B and C drawn from the divisors of n in 1..4 (C > 1, when n has
+    one, so that channels_last is another storage order)."""
+    B = rng.choice([b for b in (1, 2, 3, 4) if n % b == 0])
+    Cs = [c for c in (3, 4, 2) if (n // B) % c == 0 and n // B // c > 1]
+    C = rng.choice(Cs) if Cs else 1
+    return (B, C, 1, n // (B * C))
+
+
+def _case(rng, i, n=None):
+    """One random launch: dtypes, outputs, form, guidance kind, thresholds, size and layout. `n`: the launch's number
+    of elements (a [B, C, 1, W] shape), else a small [B, C, H, H] one."""
     from dpm_solver_b200 import ops
     from dpm_solver_b200._lib import FORM_DIFF2, FORM_LIN1, FORM_MS3, PARAM_NOISE, PARAM_V, PARAM_X_START
     md, sd = rng.choice(PAIRS)
     md, sd = DT[md], DT[sd]
     ne = rng.choice([0, 1, 2, 2])
     form = rng.choice([FORM_LIN1, FORM_DIFF2, FORM_MS3])
-    B = rng.choice([1, 2, 3])
-    C = rng.choice([3, 4])
-    H = rng.choice([5, 8, 16, 33])
-    shape = (B, C, H, H)
+    if n is None:
+        B = rng.choice([1, 2, 3])
+        C = rng.choice([3, 4])
+        H = rng.choice([5, 8, 16, 33])
+        shape = (B, C, H, H)
+    else:
+        shape = _sized_shape(rng, n)
+        B = shape[0]
+    numel = shape[0] * shape[1] * shape[2] * shape[3]
     cl = rng.random() < 0.2
     unaligned = rng.random() < 0.15
 
     def t(dtype):
-        v = torch.randn((B * C * H * H + (1 if unaligned else 0)), device="cuda").to(dtype)
+        v = torch.randn((numel + (1 if unaligned else 0)), device="cuda").to(dtype)
         v = v[1:] if unaligned else v
         v = v.view(shape)
         return v.contiguous(memory_format=torch.channels_last) if cl and not unaligned else v
@@ -103,7 +119,7 @@ def _case(rng, i):
         a.alpha_e, a.sigma_e = 0.8, 0.6
         a.xe = a.x
         a.want_m_out = rng.random() < 0.7
-        per_sample = C * H * H
+        per_sample = numel // B
         if ne == 2:
             a.e_uncond = t(md)
             a.guidance = 3.5
@@ -155,6 +171,81 @@ def test_launches_match_executor():
         if a.out2 is not None:
             assert torch.equal(a.out2, o_k) and torch.equal(b.out2.float(), o_e.float())
     assert len(seen) >= 15
+
+
+def _sizes(G):
+    """Launch sizes around ATen's geometry: one element short of a round, one round, one element of lane 1, the last
+    lane of round 0, round 1, round k, and sizes just past a multiple of G that are not multiples of 8 (a packet that
+    crosses the segment's end)."""
+    return [G - 1, G, G + 1, 4 * G - 1, 4 * G + 3, 4 * G * 2 + 17, 2 * G + 5, 3 * G + 1003, 5 * G + 7, 6 * G + 2]
+
+
+def test_launches_at_the_edges_of_the_noise_geometry():
+    """Random launches (every dtype pair, NE 0/1/2, every guidance kind, thresholds, out2, unaligned views and
+    channels_last) at sizes whose noise reaches lanes 1-3 of each curand_normal4, rounds k >= 1 and packets that cross
+    the segment's end, each with a model stage: bit for bit against the executor, generator offset included."""
+    from dpm_solver_b200 import ops
+    G = _G(1 << 30)
+    sizes = _sizes(G)
+    assert all(n > G for n in sizes[2:]) and any(n % 8 for n in sizes)
+    rng = random.Random(2027)
+    be = ops.backend()
+    seen, staged = set(), set()
+    for i in range(3 * len(sizes)):
+        n = sizes[i % len(sizes)]
+        a, kind = _case(rng, i, n)
+        while i < len(sizes) and a.n_model == 0:
+            a, kind = _case(rng, i, n)          # (the first pass over the sizes: each with a model stage)
+        a.sde = ops.SdeNoise(0.37)
+        b = _clone(a)
+        (m_k, o_k), off_k = _launch(a, 3000 + i, be)
+        (m_e, o_e), off_e = _launch(b, 3000 + i, SdeOracle())
+        seen.add((a.n_model, kind, a.thr is not None, a.out2 is not None))
+        if a.n_model:
+            staged.add(n)
+        assert off_k == off_e, (i, n)
+        assert torch.equal(o_k.float().contiguous(), o_e.float().contiguous()), (i, n, a.form, a.n_model, kind)
+        if a.want_m_out and a.n_model:
+            assert torch.equal(m_k.float().contiguous(), m_e.float().contiguous()), (i, n, kind)
+        if a.out2 is not None:
+            assert torch.equal(a.out2, o_k) and torch.equal(b.out2.float(), o_e.float())
+        del a, b, m_k, o_k, m_e, o_e
+    kinds = {k for ne, k, _, _ in seen if ne == 2}
+    assert kinds == {"scalar", "per_sample", "rescale", "per_sample_rescale", "cfgzero", "tcfg"}, kinds
+    assert any(thr for _, _, thr, _ in seen) and any(o2 for _, _, _, o2 in seen)
+    assert staged == set(sizes), "sizes without a launch that has a model stage: %s" % sorted(set(sizes) - staged)
+
+
+@pytest.mark.parametrize("view", ["strided", "permuted"])
+def test_x_in_neither_layout_takes_the_torch_drawn_noise(view):
+    """x neither row-major nor channels_last: the launch runs row-major on copies, its noise drawn by torch on an
+    empty_like of x (in x's own storage order) -- the contract's draw, which the executor makes."""
+    from dpm_solver_b200 import ops
+    from dpm_solver_b200._lib import FORM_DIFF2, PARAM_NOISE
+    B, C, H, W = 2, 3, 40, 24
+    if view == "strided":
+        mk = lambda: torch.randn(B, C, H, 2 * W, device="cuda")[..., ::2]
+    else:
+        mk = lambda: torch.randn(B, H, C, W, device="cuda").permute(0, 2, 1, 3)
+    x, m1, ec, eu = mk(), mk(), mk(), mk()
+    assert ops.CudaBackend._layout(x) is None
+    for ne in (0, 2):
+        a = ops.StepArgs(form=FORM_DIFF2, n_model=ne, x=x, m1=m1, a=0.9, c0=0.1, c1=-0.2, w0=1.1, sde=ops.SdeNoise(0.3))
+        if ne:
+            a.e_cond, a.e_uncond, a.xe, a.predict_x0, a.param = ec, eu, x, True, PARAM_NOISE
+            a.alpha_e, a.sigma_e, a.guidance, a.want_m_out = 0.8, 0.6, 7.5, True
+        else:
+            a.m0 = ec
+        b = dataclasses.replace(a)
+        ex = SdeOracle()
+        (m_k, o_k), off_k = _launch(a, 11 + ne, ops.backend())
+        (m_e, o_e), off_e = _launch(b, 11 + ne, ex)
+        g = gen(11 + ne)
+        z = torch.empty_like(x, dtype=torch.float32).normal_(generator=g)
+        assert torch.equal(ex.draws[-1], z.cpu()) and off_k == off_e == g.get_offset()
+        assert torch.equal(o_k, o_e.to(o_k.device)), view
+        if ne:
+            assert torch.equal(m_k, m_e.to(m_k.device))
 
 
 def _sample(be, x, seed, state_dtype, order, eta, **kw):

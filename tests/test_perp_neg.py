@@ -10,8 +10,8 @@ import pytest
 import torch
 
 from oracle import ref_loader
-from perpneg_oracle import (NAN32, PerpNegOracle, guided_net, perp_combine, perpneg_reference, sums_exact,
-                            words_exact, words_final, words_fsum)
+from perpneg_oracle import (NAN32, PerpNegOracle, fold_order_case, guided_net, perp_combine, perpneg_reference,
+                            sums_exact, words_exact, words_final, words_final_reversed, words_fsum)
 
 needs_ref = pytest.mark.skipif(not ref_loader.available(), reason="no reference checkout and no oracle/_ref")
 f32 = np.float32
@@ -70,12 +70,15 @@ def wrap(mt, ns, K=2, model=net, batch=B, scales=None, **kw):
                              guidance_scale=SCALES[K] if scales is None else scales, **kw)
 
 
-def reference_composed(mt, K, model=net, batch=B):
+def reference_composed(mt, K, model=net, batch=B, scales=None, rns=None, condition=None):
     """(ref module, ref schedule, model_fn) of the reference composition: each block from the reference's model_wrapper
     for its condition at scale 1 (converted to noise), the words from the raw outputs those calls made, then
-    eps_u + w_1*(eps_1 - eps_u) + s_2*(eps_2 - eps_u) + ... in eager fp32 torch."""
+    eps_u + w_1*(eps_1 - eps_u) + s_2*(eps_2 - eps_u) + ... in eager fp32 torch. `scales` (default SCALES[K]), the
+    reference VP schedule `rns` (default "sd") and the K conditions `condition` (default conds(K, batch)) may be given;
+    the words read the raw outputs row-major, so the network must return row-major outputs."""
     from test_cfg_rescale import schedules
-    ref, rns, _ = schedules("sd")
+    ref, sd_rns, _ = schedules("sd")
+    rns = sd_rns if rns is None else rns
     uc = torch.zeros(batch, 1)
     raw = []
 
@@ -84,8 +87,9 @@ def reference_composed(mt, K, model=net, batch=B):
         raw.append(out)
         return out
     fs = [ref.model_wrapper(recorded, rns, model_type=mt, guidance_type="classifier-free", condition=c,
-                            unconditional_condition=uc, guidance_scale=1.0) for c in [uc] + conds(K, batch)]
-    scales = SCALES[K]
+                            unconditional_condition=uc, guidance_scale=1.0)
+          for c in [uc] + (conds(K, batch) if condition is None else list(condition))]
+    scales = SCALES[K] if scales is None else list(scales)
 
     def composed(x, t):
         raw.clear()
@@ -190,6 +194,18 @@ def test_constructed_words():
             assert w.view(np.uint32)[0] == NAN32.view(np.uint32)
     # the fold itself: left to right, each op rounded
     assert words_final([4.0], [[2.0], [-8.0]], [3.0, -1.0, 0.5])[0] == f32((3.0 - (-1.0) * 0.5) - 0.5 * (-2.0))
+
+
+@pytest.mark.parametrize("seed", [0, 1, 2])
+def test_fold_order_case_tells_the_orders_apart(seed):
+    """fold_order_case's words are exact where they should be (c_2 = 2^13, c_4 = -2^13) and differ in several samples
+    from the words of the reversed fold, so a device test on them fails for a kernel that folds in another order."""
+    u, es, s = fold_order_case(seed=seed)
+    N, P = sums_exact(u, es)
+    assert np.array_equal(P[0] / N, np.full(len(N), 8192.0)) and np.array_equal(P[2] / N, np.full(len(N), -8192.0))
+    w = words_exact(u, es, s)
+    assert np.array_equal(w, words_final(N, P, s))
+    assert (w != words_final_reversed(N, P, s)).sum() >= 2
 
 
 # ---- sample() against the reference ----------------------------------------------------------------------------------
