@@ -113,8 +113,7 @@ class TCFGOracle(CFGZeroOracle):
         with np.errstate(all="ignore"):
             us = ((u * wu).astype(f32) + (c * wc).astype(f32)).astype(f32)
             g = (us + (w * (c - us)).astype(f32)).astype(f32)
-            if a.guidance_b is not None:
-                g = np.where(w == 1, c, g)
+            g = np.where(w == 1, c, g)      # a sample whose scale is 1, per-sample or desc->guidance, gets c
         # the guided raw output is then converted like a single network output
         b = copy.copy(a)
         b.n_model, b.e_cond, b.e_uncond = 1, torch.from_numpy(np.ascontiguousarray(g)), None
